@@ -1,12 +1,12 @@
 #!/usr/bin/env python3
-"""bench.py -- headline benchmark of the B200-native SG-SLAM tracking hot path (driver contract in the task statement).
+"""bench.py -- headline benchmark of the H100-native SG-SLAM tracking hot path.
 
-  python bench.py --gpus N --steps K --warmup W [--impl ours|reference] [--config s2|720p|hamming]
+  python bench.py --gpus N --steps K --warmup W [--impl ours|reference] [--config s2|720p|hamming] [--dump-outputs DIR]
 
 config s2 (default; BASELINE.json configs[1], the configuration `metric` is quoted on): one "step" = one pass of the hot path over a batch of
 synthetic 640x480 frames per GPU,
 
-    colour frame -> Detector2D::detect (MobileNetV3-SSDLite, tcgen05 GEMMs) ------------------------\\
+    colour frame -> Detector2D::detect (MobileNetV3-SSDLite, wgmma GEMMs) --------------------------\\
     gray frame   -> ORB extract -> LK to the previous frame -> (join) findFundamentalMat -> dyn-reject (boxes + epipolar) -> SearchByProjection(cur, last)
 
 the detector's person boxes are produced on the device and consumed by the F estimate and the rejection in stream order (src/Frame.cc:474-500 joins
@@ -16,7 +16,7 @@ config 720p (configs[2]): the same step at 1280x720 / 2000 features.   config ha
 
   value : whole-job frames/s with all inputs resident in HBM (CUDA events on the launching stream, max over ranks)
   e2e   : the same step through sgs_tracker_step with HOST (pinned) buffers, H2D / D2H inside the timed region
-  roofline     : dominant kernel's algorithmic bytes / its CUDA-event time vs the measured HBM copy peak (MEASURED_PEAKS.json)
+  roofline     : dominant kernel's algorithmic bytes / its CUDA-event time vs the HBM peak (MEASURED_PEAKS.json when present, else the H100 SXM data sheet)
   cpu_baseline : the reference's CPU path (oracle port, C++ worker threads pinned one per core) on this box's host cores, bounded sample
   --impl reference : that CPU path alone, on the same workload / frames per step
 """
@@ -150,7 +150,7 @@ def make_track_inputs(kps, desc, counts, boxes, cap, point_cap, pidx, W, H, cam)
 
 # ----------------------------------------------------------------------------------------------------------------------
 class ClockSampler(threading.Thread):
-    """nvidia-smi clock / throttle-reason sampler for the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clock / throttle-reason sampler for the timed region; also records the card and its power limit, which belong to every number."""
 
     def __init__(self, gpu_index):
         super().__init__(daemon=True)
@@ -159,7 +159,7 @@ class ClockSampler(threading.Thread):
         self.proc = None
 
     def run(self):
-        q = 'clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap'
+        q = 'clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap,power.limit,name'
         try:
             self.proc = subprocess.Popen(['nvidia-smi', '-i', str(self.gpu), '--query-gpu=' + q, '--format=csv,noheader,nounits', '-lms', '100'],
                                          stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True)
@@ -171,9 +171,11 @@ class ClockSampler(threading.Thread):
     def stop(self):
         if self.proc:
             self.proc.terminate()
-        rows = [r for r in self.rows if len(r) >= 7 and r[0].replace('.', '').isdigit()]
+            self.proc.wait()
+        self.join(timeout=5)
+        rows = [r for r in self.rows if len(r) >= 9 and r[0].replace('.', '').isdigit()]
         if not rows:
-            return {'sm_mhz': None, 'sm_max_mhz': None, 'reasons': [], 'samples': 0}
+            return {'sm_mhz': None, 'sm_max_mhz': None, 'reasons': [], 'samples': 0, 'gpu': None, 'power_limit_w': None}
         sm = sorted(float(r[0]) for r in rows)
         load = [v for v in sm if v >= 0.6 * sm[-1]] or sm      # "under load": idle gaps do not drag the median down
         reasons = []
@@ -181,14 +183,14 @@ class ClockSampler(threading.Thread):
             if any(r[i].lower().startswith('active') for r in rows):
                 reasons.append(name)
         return {'sm_mhz': load[len(load) // 2], 'sm_max_mhz': float(rows[0][1]), 'reasons': reasons, 'samples': len(rows),
-                'power_w_max': max(float(r[2]) for r in rows if r[2].replace('.', '').isdigit())}
+                'power_w_max': max(float(r[2]) for r in rows if r[2].replace('.', '').isdigit()), 'gpu': rows[0][8], 'power_limit_w': rows[0][7]}
 
 
 def measured_peaks():
     try:
         return json.load(open(os.path.join(ROOT, 'MEASURED_PEAKS.json'))), 'measured'
     except Exception:
-        return {'hbm_gbs': 6650.0, 'bf16_tflops': 1590.0, 'bf16_tflops_sustained': 1400.0}, 'fallback'
+        return {'hbm_gbs': 3350.0, 'bf16_tflops': 989.0}, 'data sheet'      # H100 SXM, 700 W: HBM3 bandwidth and dense BF16
 
 
 # ----------------------------------------------------------------------------------------------------------------------
@@ -371,7 +373,7 @@ def run_hamming(args):
     warm = max(args.warmup, 3)
     rows = []
     sampler = ClockSampler(local); sampler.start(); time.sleep(0.2)
-    flush = torch.empty(160 * 1024 * 1024, dtype=torch.uint8, device='cuda')           # > 126 MB L2: written between timed iterations
+    flush = torch.empty(160 * 1024 * 1024, dtype=torch.uint8, device='cuda')           # > the 50 MB L2: written between timed iterations
     for n in HAMMING_SIZES:
         nq = n // world                                                               # this rank's share of the queries; the train set is replicated
         q = query[rank * nq:(rank + 1) * nq]
@@ -396,8 +398,9 @@ def run_hamming(args):
     if rank == 0:
         peaks, kind = measured_peaks()
         top = rows[-1]
-        sm_hz = (clocks.get('sm_mhz') or 1965.0) * 1e6
-        popc_pairs = 148 * 16 * sm_hz / 8                          # 16 POPC / clk / SM, 8 32-bit words per pair
+        sm_hz = (clocks.get('sm_mhz') or 1980.0) * 1e6
+        nsm = torch.cuda.get_device_properties(0).multi_processor_count
+        popc_pairs = nsm * 16 * sm_hz / 8                          # 16 POPC / clk / SM, 8 32-bit words per pair
         for r in rows:
             r['frac_of_popc_rate'] = r['pairs_per_s'] / popc_pairs
             r['alg_gbs'] = (32 * 2 * r['n'] + 12 * r['n']) / (r['ms'] * 1e-3) / 1e9
@@ -407,7 +410,7 @@ def run_hamming(args):
                          'sharding': 'queries split over the ranks, train descriptors replicated by one ncclBroadcast', 'l2_policy': 'a 160 MB buffer is written between timed iterations'},
               'clocks': clocks, 'gpu_launches': 2 * args.steps * len(HAMMING_SIZES),
               'roofline': {'bound': 'hbm', 'kernel': 'hamming_bf_kernel', 'achieved': top['alg_gbs'], 'peak': peaks['hbm_gbs'], 'unit': 'GB/s', 'frac': top['alg_gbs'] / peaks['hbm_gbs'],
-                           'traffic': None, 'peak_kind': kind, 'binding_roof': 'POPC issue rate: %.2f of 148 SM x 16 POPC/clk' % top['frac_of_popc_rate'],
+                           'traffic': None, 'peak_kind': kind, 'binding_roof': 'POPC issue rate: %.2f of %d SM x 16 POPC/clk' % (top['frac_of_popc_rate'], nsm),
                            'note': 'all-pairs matching re-uses every descriptor N times from shared memory: the HBM fraction is reported as asked, the binding roof is the integer pipe'},
               'e2e': None, 'cpu_baseline': None})
     if dist is not None:
@@ -422,14 +425,18 @@ def main():
     ap.add_argument('--warmup', type=int, default=3)
     ap.add_argument('--impl', default='ours', choices=['ours', 'reference'])
     ap.add_argument('--config', default='s2', choices=['s2', '720p', 'hamming'])
-    ap.add_argument('--batch', type=int, default=0, help='frames per GPU per step (default 512 at 640x480: 157 MB of gray input > the 126 MB L2)')
+    ap.add_argument('--batch', type=int, default=0, help='frames per GPU per step (default 512 at 640x480: 157 MB of gray input > the 50 MB L2)')
     ap.add_argument('--cpu-sample', type=int, default=0, help='frames of the cpu_baseline sample (0: four per host thread, at least 64)')
     ap.add_argument('--parity-frames', type=int, default=256, help='frames of the full-chain parity check against the pure oracle')
     ap.add_argument('--no-e2e', action='store_true')
     ap.add_argument('--no-pipeline', action='store_true', help='e2e: skip the steps-in-flight mode')
     ap.add_argument('--pipeline-handles', type=int, default=3, help='e2e: full-size handles taking whole steps in turn')
     ap.add_argument('--no-detector', action='store_true', help='tracker-only step with ground-truth boxes (the round-1 definition of the step)')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='after the timed steps, write what the last one computed as DIR/<name>.npy (float32 / float64; a fixed sample of the frames)')
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error('--steps must be at least 1')
     claim_stdout()
     cfg = CONFIGS.get(args.config)
     if args.impl == 'reference':
@@ -567,6 +574,8 @@ def main():
     sampler = ClockSampler(local); sampler.start(); time.sleep(0.3)
     total_ms = timed_steps(use_det, args.steps)
     clocks = sampler.stop()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, L, B, trk, NB, cap, use_det)
     value = world * NB * args.steps / (total_ms * 1e-3)
     # ---- the tracker-only step (ground-truth boxes as inputs: the round-1 definition), with per-stage device times -------
     B.check(L.sgs_extractor_set_profiling(exh, 1))
@@ -789,7 +798,7 @@ def main():
     dom_bytes = alg[dom] * NB
     achieved = dom_bytes / (all_ms[dom] * 1e-3) / 1e9
     step_alg = (ab['extract'] + ab['lk_pyr'] + ab['lk_track'] + ab['fm'] + ab['track']) * NB
-    peak_note = 'measured copy bandwidth (MEASURED_PEAKS.json)' if peak_kind == 'measured' else 'fallback 6650 GB/s'
+    peak_note = 'measured copy bandwidth (MEASURED_PEAKS.json)' if peak_kind == 'measured' else 'H100 SXM data sheet: 3350 GB/s, 989 TFLOP/s dense BF16'
     tracker_dom = {'kernel': dom, 'bound': 'hbm', 'achieved': achieved, 'peak': peaks['hbm_gbs'], 'unit': 'GB/s', 'frac': achieved / peaks['hbm_gbs'],
                    'algorithmic_bytes_per_launch': int(dom_bytes), 'kernel_ms': all_ms[dom],
                    'note': 'largest single launch of the step; instruction-issue bound (exact OpenCV fixed-point arithmetic), the HBM fraction is reported as asked'}
@@ -804,7 +813,7 @@ def main():
         # its algorithmic bytes per call / the sum of its launch durations, both for the NB frames of one step
         g_gbs = det_fam['bytes'] / (det_fam['ms'] * 1e-3) / 1e9
         g_tf = det_fam['flop'] / (det_fam['ms'] * 1e-3) / 1e12
-        roofline = dict({'bound': 'hbm', 'kernel': 'conv1x1_tc_kernel (the detector\'s 1x1-convolution GEMM: %d launches per call, TMA + tcgen05/TMEM)' % det_fam['launches'],
+        roofline = dict({'bound': 'hbm', 'kernel': 'conv1x1_tc_kernel (the detector\'s 1x1-convolution GEMM: %d launches per call, TMA + wgmma)' % det_fam['launches'],
                          'achieved': g_gbs, 'peak': peaks['hbm_gbs'], 'unit': 'GB/s', 'frac': g_gbs / peaks['hbm_gbs'], 'peak_kind': peak_note,
                          'algorithmic_bytes_per_launch': int(det_fam['bytes'] / det_fam['launches']), 'algorithmic_bytes_per_call': int(det_fam['bytes']),
                          'kernel_ms': det_fam['ms'], 'launches': det_fam['launches'],
@@ -823,7 +832,7 @@ def main():
         det_info = {'model': 'mobilenetv3_ssdlite_voc (the reference\'s trained ncnn model, 9.7 MB FP32 weights)', 'frames_per_call': NB, 'ms_per_call': det_ms, 'frames_per_s': NB / det_ms * 1e3,
                     'kernels_per_call': det.num_kernels,
                     'roofline': {'bound': 'tensor', 'achieved': tf, 'peak': peaks['bf16_tflops'], 'unit': 'TFLOP/s', 'frac': tf / peaks['bf16_tflops'],
-                                 'note': '1.115 GFLOP per 300x300 inference (SURVEY 8d) counted once; the 66 1x1 convolutions (90 % of the MACs) are TMA-fed tcgen05 / TMEM GEMMs with error-compensated TF32 operands (3 tcgen05.mma per k-step: the tensor pipe does 3x these FLOPs), the rest FP32 FMA; the layers are streaming-bound (K = 16..960), peak = measured dense bf16'}}
+                                 'note': '1.115 GFLOP per 300x300 inference (SURVEY 8d) counted once; the 66 1x1 convolutions (90 % of the MACs) are TMA-fed wgmma GEMMs with error-compensated TF32 operands (3 wgmma per k-step: the tensor pipe does 3x these FLOPs), the rest FP32 FMA; the layers are streaming-bound (K = 16..960), peak = dense bf16'}}
 
     # ---- parity: (1) the whole chain against the PURE oracle (own LK, own F; the detector's boxes as inputs) ---------------------------------
     parity = None
@@ -893,6 +902,47 @@ def main():
         emit(line)
     if dist is not None:
         dist.destroy_process_group()
+
+
+DUMP_FRAMES = 64          # frames of the per-keypoint arrays written by --dump-outputs (a seeded sample of the batch; per-frame counts cover all of it)
+
+
+def dump_outputs(out_dir, L, B, trk, nb, cap, use_det):
+    """What the last timed step left in the tracker: per frame the keypoints that survived the dynamic-point rejection, their descriptors, u_right
+    and matched last-frame point (sgs_tracker_results_device), the counts, and the detector's person boxes.  Rows past a frame's count are zeroed
+    (the device buffers keep stale rows there).  Per-keypoint arrays cover DUMP_FRAMES frames drawn with a fixed seed, so that the files stay small."""
+    import torch
+    torch.cuda.synchronize()
+    os.makedirs(out_dir, exist_ok=True)
+    v = C.c_void_p
+    pk, pd, pu, pc_, pm, pn, pnc = (v() for _ in range(7))
+    B.check(L.sgs_tracker_results_device(trk.h, *[C.byref(p) for p in (pk, pd, pu, pc_, pm, pn, pnc)]))
+    kps = B.memcpy_d2h(np.zeros((nb, cap), B.KP_DTYPE), pk.value)
+    desc = B.memcpy_d2h(np.zeros((nb, cap, 32), np.uint8), pd.value)
+    ur = B.memcpy_d2h(np.zeros((nb, cap), np.float32), pu.value)
+    cnt = B.memcpy_d2h(np.zeros(nb, np.int32), pc_.value)
+    mp = B.memcpy_d2h(np.zeros((nb, cap), np.int32), pm.value)
+    nm = B.memcpy_d2h(np.zeros(nb, np.int32), pn.value)
+    sel = np.sort(np.random.default_rng(0).choice(nb, min(nb, DUMP_FRAMES), replace=False))
+    valid = np.arange(cap)[None, :] < cnt[sel, None]
+    kp = np.stack([kps[sel][k].astype(np.float32) for k in B.KP_DTYPE.names], -1)
+    arrays = {'frame_index': sel.astype(np.float64), 'keypoint_count': cnt.astype(np.float64), 'match_count': nm.astype(np.float64),
+              'keypoints': np.where(valid[..., None], kp, 0).astype(np.float32),
+              'descriptors': np.where(valid[..., None], desc[sel], 0).astype(np.float32),
+              'u_right': np.where(valid, ur[sel], 0).astype(np.float32),
+              'matched_point': np.where(valid, mp[sel], 0).astype(np.float64)}
+    if use_det:
+        pb, pnb, ph = v(), v(), v()
+        B.check(L.sgs_tracker_boxes_device(trk.h, C.byref(pb), C.byref(pnb), C.byref(ph)))
+        nbox = B.memcpy_d2h(np.zeros(nb, np.int32), pnb.value)
+        boxes = B.memcpy_d2h(np.zeros((nb, 4, 4), np.float32), pb.value)
+        arrays['person_boxes'] = np.where(np.arange(4)[None, :, None] < nbox[:, None, None], boxes, 0).astype(np.float32)
+        arrays['person_box_count'] = nbox.astype(np.float64)
+        arrays['have_dynamic'] = B.memcpy_d2h(np.zeros(nb, np.uint8), ph.value).astype(np.float64)
+    assert sum(a.nbytes for a in arrays.values()) <= 64 << 20
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + '.npy'), a)
+    log('[bench] outputs of the last timed step written to %s (%s)' % (out_dir, ', '.join(sorted(arrays))))
 
 
 def detector_gemm_table(det, kernel_ms, ncalls, nframes):

@@ -1,5 +1,5 @@
 /* =====================================================================================
- * sgs_abi.h -- C ABI of libsgs_cuda.so: the B200-native (sm_100a) replacement for the
+ * sgs_abi.h -- C ABI of libsgs_cuda.so: the H100-native (sm_90a) replacement for the
  * SG-SLAM / ORB-SLAM2 per-frame tracking hot path.
  *
  * The reference has no FFI layer: the boundary is three C++ classes inside libsg-slam.so
@@ -642,8 +642,8 @@ typedef struct sgs_object2d {   /* Object2D, include/Detector2D.h:29-37 (name = 
  * max_frames = largest batch one sgs_detector_detect_device call may carry.  flags: bit 0 = diagnostic mode (every layer its own kernel,
  * every intermediate blob kept, readable with sgs_detector_blob); bit 1 = plan only (parse, shapes, kernel list and activation pool are
  * built, no device is touched; the handle serves sgs_detector_info / sgs_detector_describe only).
- * The 1x1 convolutions (90 % of the MACs) run as a TMA-fed tcgen05 / TMEM GEMM on [frame][h][w][c] activations with error-compensated TF32 operands
- * (three tcgen05.mma per 8-wide k-step, FP32 accumulate: ~1e-6 relative); there is no other GEMM path. */
+ * The 1x1 convolutions (90 % of the MACs) run as a TMA-fed wgmma GEMM on [frame][h][w][c] activations with error-compensated TF32 operands
+ * (three wgmma per 8-wide k-step, FP32 accumulate: ~1e-6 relative); there is no other GEMM path. */
 SGS_API int sgs_detector_create(const char* param_path, const char* bin_path, int max_frames, float detection_confidence_threshold,
                                 float dynamic_detection_confidence_threshold, int flags, int device, sgs_detector** out);
 SGS_API void sgs_detector_destroy(sgs_detector* d);

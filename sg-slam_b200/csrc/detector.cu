@@ -5,14 +5,14 @@
 // The handle parses the ncnn text graph and weight blob itself, infers every blob shape for the fixed 3x300x300 input (Detector2D.h:70),
 // folds the constant sub-graphs (MemoryData scalars, PriorBox, their Concat) on the host, and turns the rest into a flat list of kernels:
 //   preprocess     : Mat::from_pixels_resize + substract_mean_normalize (Detector2D.cc:39-40), fixed-point bilinear (bit-exact with cv::resize)
-//   conv1x1        : 90 % of the MACs; out[p][co] = bias[co] + sum_ci X[p][ci] * W[co][ci] over the pixels of all frames, as a TMA-fed tcgen05 / TMEM
+//   conv1x1        : 90 % of the MACs; out[p][co] = bias[co] + sum_ci X[p][ci] * W[co][ci] over the pixels of all frames, as a TMA-fed wgmma
 //                    GEMM with error-compensated TF32 operands (conv1x1_tc.cuh), bias + fused element-wise tail in its epilogue
 //   dwconv / conv  : depth-wise 3x3 / 5x5 (channel-vectorised) and the few dense convolutions the GEMM does not take (first layer, Cin not a multiple of 4)
 //   eltwise        : whatever element-wise chain could not be attached to a producer
 //   softmax, detection-output (per class: threshold, sort, top-k, greedy NMS; per frame: merge, top-k, Detector2D.cc:52-88)
 // Element-wise layers (BinaryOp with a constant / a tensor / the chain's own start value, Clip, ReLU) that follow a producer are applied in
 // the producer's epilogue in graph order, one rounding per op, so fused and unfused execution give identical bits.
-// Layout: every 3-D blob is [frames][h][w][c] FP32 (channels innermost): both GEMM operands are K-major for tcgen05.mma and TMA-addressable, the
+// Layout: every 3-D blob is [frames][h][w][c] FP32 (channels innermost): both GEMM operands are K-major for wgmma (tf32) and TMA-addressable, the
 // depth-wise kernels read channel vectors, and ncnn's Permute(order 3: c,h,w -> h,w,c) in front of the SSD heads becomes an alias -- the head
 // convolutions write straight into the concatenated mbox_loc / mbox_conf buffers.  sgs_detector_blob transposes back to ncnn's c,h,w on read-out.
 // Activations live in a pool planned by liveness.
@@ -206,9 +206,8 @@ struct EpiFn {
     __host__ __device__ bool reads_tensors() const { return e.kind == EK_ADD_T || e.kind == EK_SE_TAIL || e.kind == EK_SE_MUL || e.kind == EK_GENERIC; }
 };
 
-// The same with the tail kind fixed at compile time: one instantiation of the tcgen05 GEMM per kind, so that the epilogue warps carry the code of one
-// tail only (with the run-time switch every tail was inlined at every call site and the five warp roles of the kernel thrashed the instruction cache:
-// ncu stall_no_instruction 4.6 per issue, in-network times 1.5 - 1.8x those of the single-tail unit harness).
+// The same with the tail kind fixed at compile time: one instantiation of the GEMM per kind, so that the epilogue carries the code of one
+// tail only (with a run-time switch every tail is inlined at every call site of the epilogue, and the kernel's code outgrows the instruction cache).
 template <int KIND>
 struct EpiFnK {
     Epi e;
@@ -1029,7 +1028,7 @@ int build_graph(sgs_detector* D) {
             if (op.kind == OP_CONV1X1) {
                 const int m_tiles = (int)std::min<int64_t>(((int64_t)D->max_frames * op.g.OH * op.g.OW + tc::kBM - 1) / tc::kBM, 1 << 30);      // pixel tiles of a full batch
                 if (D->flags & 2) tc::plan_tiling(op.g.Cin, op.g.Cout, &op.gp, 0, m_tiles);
-                else if (!tc::plan_weights(L.weight.data(), op.g.Cin, op.g.Cout, &op.gp, 0, m_tiles)) { set_error("sgs_detector_create: layer %s: the tcgen05 GEMM could not be set up (TMA tensor maps need a CUDA 12 driver; %s)", L.name.c_str(), cudaGetErrorString(cudaGetLastError())); return SGS_ERR_CUDA; }
+                else if (!tc::plan_weights(L.weight.data(), op.g.Cin, op.g.Cout, &op.gp, 0, m_tiles)) { set_error("sgs_detector_create: layer %s: the wgmma GEMM could not be set up (TMA tensor maps need a CUDA 12 driver; %s)", L.name.c_str(), cudaGetErrorString(cudaGetLastError())); return SGS_ERR_CUDA; }
             } else if (op.kind == OP_DWCONV) {                    // [c][ky][kx] -> [ky][kx][c]: channel vectors
                 std::vector<float> wt(L.weight.size());
                 const int kk = op.g.k * op.g.k;
@@ -1376,7 +1375,7 @@ int sgs_detector_describe(const sgs_detector* D, char* out, int64_t cap, int64_t
            << D->blobs[root_of(*D, op.out)].buf << " n " << bo.n;
         if (op.kind <= OP_DWCONV) ss << " geom " << op.g.Cin << 'x' << op.g.H << 'x' << op.g.W << "->" << op.g.Cout << 'x' << op.g.OH << 'x' << op.g.OW << " k" << op.g.k << " s" << op.g.stride << " p" << op.g.pad;
         if (op.kind == OP_CONCAT_COPY || op.cat) ss << " off " << op.off;
-        if (op.kind == OP_CONV1X1) ss << " tile " << op.gp.NT << "x" << op.gp.n_tiles << " kb " << op.gp.KB << "x" << op.gp.BK << " stages " << op.gp.stages << (op.gp.b_resident ? " wres" : "") << " cps " << op.gp.ctas_per_sm;
+        if (op.kind == OP_CONV1X1) ss << " tile " << op.gp.NT << "x" << op.gp.n_tiles << " kb " << op.gp.KB << "x" << op.gp.BK << " stages " << op.gp.stages << (op.gp.b_resident ? " wres" : "");
         for (const auto& s : op.epi) {
             ss << " | " << opn[s.op] << (s.rev ? "(rev)" : "");
             if (s.op <= E_DIV) { if (s.src == SRC_SCALAR) ss << ' ' << s.a; else if (s.src == SRC_START) ss << " start"; else ss << ' ' << D->blobs[s.tblob].name << " buf " << D->blobs[root_of(*D, s.tblob)].buf; }

@@ -1,4 +1,4 @@
-// extract_kernels.cu -- hand-written sm_100a kernels of the batched ORB extractor.
+// extract_kernels.cu -- hand-written sm_90a kernels of the batched ORB extractor.
 //
 // Stage            reference (src/ORBextractor.cc)                kernel
 //   pyramid        ComputePyramid :1108-1133 (cv::resize)          resize_level_kernel   (1 launch per level >= 1, all frames)

@@ -1,12 +1,12 @@
 // fast_kernel.cu -- FAST-9-16 + cell-local 3x3 NMS + per-cell threshold fallback (ComputeKeyPointsOctTree, FAST part,
 // src/ORBextractor.cc:766-830; cv::FAST semantics pinned in tests/test_oracle_golden.py).
 //
-// B200 design: ONE WARP PER CELL (a cell == one cv::FAST call of the reference), 8 independent warps per block, no block
+// Design: ONE WARP PER CELL (a cell == one cv::FAST call of the reference), 8 independent warps per block, no block
 // barriers.  Each warp
 //   0. pulls its cell view (+3 px ring halo) into its private shared-memory tile with ONE TMA tensor copy
 //      (cp.async.bulk.tensor.3d, per-level tensor map {x, y, frame}) completing on a per-warp mbarrier -- or with plain loads
-//      when a level is not TMA-addressable.  MEASURED: the innermost TMA coordinate must be 16-byte aligned (an unaligned x
-//      raises "illegal instruction" on sm_100a), so the box starts at xa = (x0-4) & ~15 and the view sits `off` = x0 - xa
+//      when a level is not TMA-addressable.  The innermost TMA coordinate must be 16-byte aligned (an unaligned x
+//      raises "illegal instruction"), so the box starts at xa = (x0-4) & ~15 and the view sits `off` = x0 - xa
 //      (4..19) columns into the tile; the packed phase works on smem-aligned words and masks the partial first/last word;
 //   A. compass pre-test on 4 pixels per instruction: VABSDIFF4.U8 against the 4 compass ring pixels (0,4,8,12), a carry-free
 //      packed "> t" test, and "at least two of four" in three LOP3s (any 9-arc contains >= 2 compass pixels);

@@ -3,7 +3,7 @@
 //
 // sgs_hamming_bf: each thread owns one query descriptor in registers (two 128-bit loads); train descriptors are staged
 // through shared memory in tiles read as warp-wide broadcasts.  The train set is split across blockIdx.y so that small
-// query sets still fill the 148 SMs; partial (best, idx, second) triples are merged in train order, which preserves the
+// query sets still fill the GPU's SMs; partial (best, idx, second) triples are merged in train order, which preserves the
 // reference's "first strictly smaller wins" tie-break.  The all-pairs sweep is POPC/ALU bound, not HBM bound (DESIGN.md).
 #include <cuda_runtime.h>
 
@@ -73,7 +73,9 @@ __global__ void hamming_pairs_kernel(const uint4* __restrict__ a, const uint4* _
 // scratch: 3 * nsplit * nq int32.  Returns the split count through *nsplit_out when scratch == nullptr (sizing query).
 int bf_plan_splits(int nq, int nt) {
     const int qblocks = (nq + kBfThreads - 1) / kBfThreads;
-    int target = (2 * 148 + qblocks - 1) / qblocks;          // aim for >= 2 waves of blocks
+    static int sms = 0;
+    if (!sms) { int dev = 0; cudaGetDevice(&dev); if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms < 1) sms = 132; }
+    int target = (2 * sms + qblocks - 1) / qblocks;          // aim for >= 2 waves of blocks
     int max_split = (nt + kBfTile - 1) / kBfTile;            // at least one tile per split
     if (target > max_split) target = max_split;
     if (target < 1) target = 1;

@@ -1,7 +1,7 @@
 // quadtree_core.h -- deterministic, data-parallel restatement of ORBextractor::DistributeOctTree
 // (src/ORBextractor.cc:540-764) + ExtractorNode::DivideNode (:482-538).
 //
-// B200-first formulation (not a translation of the std::list/pointer code):
+// GPU-first formulation (not a translation of the std::list/pointer code):
 //   * every split position of the reference's quadtree is a pure function of the root rectangle
 //     (halfX = ceil(w/2)), so each candidate's path (2 bits per depth) is computed independently;
 //   * candidates are sorted once by (root, path): every node of every depth is then a contiguous

@@ -73,6 +73,8 @@ def main():
     d = depth[ky.astype(np.int32), kx.astype(np.int32)]
     ur = np.where(d > 0, kx - f32(40.0) / np.where(d > 0, d, 1).astype(f32), f32(-1)).astype(f32)
     dz = np.where(d > 0, d, f32(-1)).astype(f32)
+    looked_up = np.zeros_like(depth); looked_up[ky.astype(np.int32), kx.astype(np.int32)] = d
+    depth = looked_up                                                      # only the pixels under the keypoints are read: the rest is stored as 0 (keeps the file small)
     np.savez_compressed(os.path.join(HERE, 'frustum.npz'), Tcw=Tcw, cam=cam, xyz=xyz, normal=nrm, min_dist=mind, max_dist=maxd, logsf=logsf, depth=depth, kx=kx, ky=ky,
                         u_right=ur, depth_out=dz, cv2_version=np.array(cv2.__version__), **out)
     print('in view', int(out['inview'].sum()), 'of', n)

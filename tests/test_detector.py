@@ -168,7 +168,7 @@ def test_plan_of_the_reference_model():
     assert len(heads) == 12 and all(l.startswith('conv1x1 ') and ' off ' in l for l in heads)
     offs = sorted(int(l.split(' off ')[1].split()[0]) for l in heads if ' out mbox_conf ' in l)
     assert offs == [0, 30324, 42924, 46074, 47208, 47544]
-    # every 1x1 convolution of the model with Cin % 4 == 0 is planned for the tcgen05 GEMM: 66 of the 70 convolutions
+    # every 1x1 convolution of the model with Cin % 4 == 0 is planned for the wgmma GEMM: 66 of the 70 convolutions
     assert sum(l.startswith('conv1x1 ') for l in lines) == 66 and sum(l.startswith('conv ') for l in lines) == 4
     layers = NM.parse_param(REAL + '.param')
     used, total = NM.load_weights(layers, REAL + '.bin')

@@ -4,8 +4,7 @@ its OWN LK and its OWN F.  Extraction must be bit-exact; LK agrees to ~1e-4 px (
 a keypoint's epipolar distance across its 0.2 / 1.0 px threshold: the keep-set symmetric difference and the match-index difference per frame are measured and
 bounded.  With the S2 person box active (thresholds 0.2 px inside the box, ~210 of ~1006 keypoints rejected per frame) a sub-0.03 px LK difference can also
 hand RANSAC a different winning sample on a few frames, which then flips several verdicts at once.  Stated bound: mean <= 4 keypoints per frame (0.4 %),
-max <= 60 on any frame (6 %), at least half of the frames identical end to end; observed on B200: mean 1.5 / max 27 with the box, 0.05 / 3 without
-(bench.py, 256 frames, detector boxes)."""
+max <= 60 on any frame (6 %), at least half of the frames identical end to end (bench.py reports the same differences on 256 frames with detector boxes)."""
 import ctypes as C
 import os
 import sys

@@ -43,7 +43,7 @@ for j, op in enumerate(ops):
         cin, hh, ww = [int(x) for x in g.group(1).split('->')[0].split('x')]; cout = int(g.group(1).split('->')[1].split('x')[0])
         npx = hh * ww * F; by = (cin + cout) * 4 * npx; fl = 2 * cin * cout * npx
         gemm_t += t; gemm_fl += fl
-        tile = re.search(r'tile (\S+) kb (\S+) stages (\d+)( wres)? cps (\d)', op).group(0)
+        tile = re.search(r'tile (\S+) kb (\S+) stages (\d+)( wres)?', op).group(0)
         out.append((t, '%3d %-8s %-26s %-34s %7.1f us %6.0f GB/s %6.1f TF |%s' % (j, kind, g.group(1), tile, t, by / t * 1e-3, fl / t * 1e-6, tail)))
     else:
         out.append((t, '%3d %-8s %-26s %-34s %7.1f us |%s' % (j, kind, g.group(1) if g else '', '', t, tail)))

@@ -1,6 +1,6 @@
 #!/usr/bin/env python3
 """Secondary measurements (not the driver's bench line): BASELINE config 5 (Hamming BF sweep 1k..64k) and config 3's extraction
-geometry (1280x720, 2000 features).  Prints one JSON line per measurement; results are copied into profiles/."""
+geometry (1280x720, 2000 features).  Prints one JSON line per measurement."""
 import ctypes as C
 import json
 import os

@@ -9,9 +9,9 @@ cd $ROOT/sg-slam_b200/csrc
 SAN="-fsanitize=address,-fsanitize=undefined,-fno-omit-frame-pointer"
 for f in *.cu orb_plan.cpp; do
   b=${f%.*}
-  echo "nvcc -O1 -g -std=c++17 -gencode arch=compute_100a,code=sm_100a -Xcompiler -fPIC,-fvisibility=hidden,$SAN --expt-relaxed-constexpr -fmad=false -c -o $OUT/obj/$b.o $f 2>$OUT/obj/$b.log"
+  echo "nvcc -O1 -g -std=c++17 -gencode arch=compute_90a,code=sm_90a -Xcompiler -fPIC,-fvisibility=hidden,$SAN --expt-relaxed-constexpr -fmad=false -c -o $OUT/obj/$b.o $f 2>$OUT/obj/$b.log"
 done | xargs -P "$(nproc)" -I{} sh -c "{}"
-nvcc -gencode arch=compute_100a,code=sm_100a -shared -o $OUT/libsgs_cuda.so $OUT/obj/*.o -cudart static -Xcompiler -fsanitize=address,-fsanitize=undefined
+nvcc -gencode arch=compute_90a,code=sm_90a -shared -o $OUT/libsgs_cuda.so $OUT/obj/*.o -cudart static -Xcompiler -fsanitize=address,-fsanitize=undefined
 cat > $OUT/run.py <<'PY'
 import sys
 R = sys.argv[1]
