@@ -1375,7 +1375,8 @@ int sgs_detector_describe(const sgs_detector* D, char* out, int64_t cap, int64_t
            << D->blobs[root_of(*D, op.out)].buf << " n " << bo.n;
         if (op.kind <= OP_DWCONV) ss << " geom " << op.g.Cin << 'x' << op.g.H << 'x' << op.g.W << "->" << op.g.Cout << 'x' << op.g.OH << 'x' << op.g.OW << " k" << op.g.k << " s" << op.g.stride << " p" << op.g.pad;
         if (op.kind == OP_CONCAT_COPY || op.cat) ss << " off " << op.off;
-        if (op.kind == OP_CONV1X1) ss << " tile " << op.gp.NT << "x" << op.gp.n_tiles << " kb " << op.gp.KB << "x" << op.gp.BK << " stages " << op.gp.stages << (op.gp.b_resident ? " wres" : "");
+        if (op.kind == OP_CONV1X1) ss << " tile " << op.gp.NT << "x" << op.gp.n_tiles << " kb " << op.gp.KB << "x" << op.gp.BK << " stages " << op.gp.stages << (op.gp.b_resident ? " wres" : "")
+                                    << " smem " << op.gp.smem_bytes;
         for (const auto& s : op.epi) {
             ss << " | " << opn[s.op] << (s.rev ? "(rev)" : "");
             if (s.op <= E_DIV) { if (s.src == SRC_SCALAR) ss << ' ' << s.a; else if (s.src == SRC_START) ss << " start"; else ss << ' ' << D->blobs[s.tblob].name << " buf " << D->blobs[root_of(*D, s.tblob)].buf; }

@@ -29,14 +29,16 @@ class Graph:
         self.layers.insert(1, ['MemoryData', n, [], [n], '0=1', [np.array([v], np.float32)]])
         return n
 
-    def conv(self, x, cin, cout, k=1, s=1, p=0, gain=1.0, dw=False):
+    def conv(self, x, cin, cout, k=1, s=1, p=0, gain=1.0, dw=False, w=None, b=None, name=None):
         fan = k * k * (1 if dw else cin)
-        w = (self.rng.standard_normal((cout, 1 if dw else cin, k, k)) * gain * np.sqrt(2.0 / fan)).astype(np.float32)
-        b = (self.rng.standard_normal(cout) * 0.1).astype(np.float32)
+        if w is None:
+            w = (self.rng.standard_normal((cout, 1 if dw else cin, k, k)) * gain * np.sqrt(2.0 / fan)).astype(np.float32)
+        if b is None:
+            b = (self.rng.standard_normal(cout) * 0.1).astype(np.float32)
         prm = '0=%d 1=%d 11=%d 2=1 12=1 3=%d 13=%d 4=%d 14=%d 5=1 6=%d' % (cout, k, k, s, s, p, p, w.size)
         if dw:
             prm += ' 7=%d' % cout
-        return self.add('ConvolutionDepthWise' if dw else 'Convolution', [x], prm, [np.zeros(1, np.uint32), w, b])
+        return self.add('ConvolutionDepthWise' if dw else 'Convolution', [x], prm, [np.zeros(1, np.uint32), w, b], name=name)
 
     def relu(self, x): return self.add('ReLU', [x])
     def clip(self, x): return self.add('Clip', [x], '0=0.000000 1=6.000000')
@@ -120,6 +122,191 @@ def write_mini_model(dirpath, seed=0, conf_gain=1.0, person_bias=2.0, many_prior
     pp, bp = os.path.join(dirpath, 'mini.param'), os.path.join(dirpath, 'mini.bin')
     g.write(pp, bp)
     return pp, bp
+
+
+CHAIN = (150, 75, 38, 19, 10, 5, 3, 2, 1)        # map sizes of the probe graphs' depth-wise 3x3/s2 chain below the 150x150 stem output
+
+
+def _head(g, data, feats, npr, prior_params, ncls=21, person_bias=2.0):
+    """SSD head over [(blob, channels)]: conf / loc 1x1 convolutions -> Permute -> Flatten -> Concat, PriorBox, Softmax, DetectionOutput."""
+    locs, confs, priors = [], [], []
+    for f, c in feats:
+        cf = g.conv(f, c, npr * ncls)
+        g.layers[-1][5][2][15::ncls] += np.float32(person_bias)
+        confs.append(g.add('Flatten', [g.add('Permute', [cf], '0=3')]))
+        locs.append(g.add('Flatten', [g.add('Permute', [g.conv(f, c, npr * 4)], '0=3')]))
+        priors.append(g.add('PriorBox', [f, data], prior_params + ' 3=0.100000 4=0.100000 5=0.200000 6=0.200000 8=0 9=-233 10=-233 11=-233.000000 '
+                                                                   '12=-233.000000 13=0.500000 14=1 15=1'))
+    loc = g.add('Concat', locs, '0=0', name='mbox_loc')
+    conf = g.add('Concat', confs, '0=0', name='mbox_conf')
+    pri = g.add('Concat', priors, '0=1', name='mbox_priorbox')
+    sm = g.add('Softmax', [g.add('Reshape', [conf], '0=%d 1=-1' % ncls)], '0=1 1=1')
+    g.add('DetectionOutput', [loc, g.add('Flatten', [sm]), pri], '0=%d 1=0.450000 2=300 3=100 4=0.010000' % ncls, name='detection_out')
+
+
+def _probe_weights(rng, cin, cout, mode):
+    """Weights [cout][cin][1][1] and bias of a probe GEMM.  'dense': normal; 'onehot': one full-mantissa float32 per output channel at input channel
+    perm[co % cin] (a permutation, repeated when cout > cin); 'pow2': the same pattern with powers of two and a zero bias; 'zero': zeros."""
+    b = (rng.standard_normal(cout) * 0.1).astype(np.float32)
+    if mode == 'dense':
+        return (rng.standard_normal((cout, cin, 1, 1)) * np.sqrt(2.0 / cin)).astype(np.float32), b
+    if mode == 'zero':
+        return np.zeros((cout, cin, 1, 1), np.float32), np.zeros(cout, np.float32)
+    w = np.zeros((cout, cin, 1, 1), np.float32)
+    src = rng.permutation(cin)[np.arange(cout) % cin]
+    sign = np.where(rng.random(cout) < 0.5, -1.0, 1.0)
+    if mode == 'onehot':
+        v = (sign * rng.uniform(0.5, 2.0, cout)).astype(np.float32)
+        v = (v.view(np.uint32) | np.uint32(0x00000fff)).view(np.float32)         # low mantissa bits set: the hi / lo residual of the split is never zero
+    elif mode == 'pow2':
+        v = (sign * np.exp2(rng.integers(-3, 4, cout))).astype(np.float32)
+        b = np.zeros(cout, np.float32)
+    else:
+        raise ValueError(mode)
+    w[np.arange(cout), src, 0, 0] = v
+    return w, b
+
+
+def write_probe_model(dirpath, probes, seed=0, c0=16, weights='dense', name='probe'):
+    """A graph that puts chosen convolution shapes on real activations, for kernel-level parity checks in diagnostic mode.
+
+    Input 3x300x300 -> dense 3x3/s2 stem 3 -> c0 (no activation; per-channel gains 2^[-3, 3] give signed values of varied magnitude) -> a chain of
+    depth-wise 3x3/s2 layers down to the smallest map a probe needs (CHAIN).  Each probe hangs off the chain at its map size and is a dead end:
+      ('gemm', cin, cout, hw)           1x1 convolution (the wgmma GEMM when cin % 4 == 0), fed by a 1x1 expansion c0 -> cin unless cin == c0;
+                                        its weights follow `weights` (see _probe_weights), every other layer is dense;
+      ('dw', c, k, s, hw)               depth-wise k x k / stride s, padding k // 2, fed by an expansion c0 -> c unless c == c0;
+      ('conv', cin, cout, k, s, hw)     dense k x k / stride s, padding k // 2, fed the same way.
+    A minimal SSD head (4 priors per location, 21 classes) on the 19x19 map closes the graph.
+    Returns (param path, bin path, convs): convs maps every convolution layer name to a dict with 'role' (stem / chain / expand / probe / head), 'dw',
+    'in' / 'out' (blob names), 'cin', 'cout', 'k', 's', 'p', 'hw' (input map size), 'w' ([cout][cin or 1][k][k] float32) and 'b'."""
+    g = Graph(seed)
+    convs = {}
+
+    def conv(role, x, cin, cout, hw, k=1, s=1, dw=False, w=None, b=None, gain=1.0):
+        y = g.conv(x, cin, cout, k, s, k // 2, gain=gain, dw=dw, w=w, b=b, name=g.name('%s_%s' % (name, role)))
+        L = g.layers[-1]
+        convs[y] = dict(role=role, dw=dw, cin=cin, cout=cout, k=k, s=s, p=k // 2, hw=hw, w=L[5][1], b=L[5][2], out=y, **{'in': x})
+        return y
+
+    data = g.add('Input', [], name='input')
+    ws = (g.rng.standard_normal((c0, 3, 3, 3)) * np.sqrt(2.0 / 27) * np.exp2(g.rng.uniform(-3, 3, (c0, 1, 1, 1))) / 64).astype(np.float32)
+    chain = {150: conv('stem', data, 3, c0, 300, 3, 2, w=ws)}
+    smallest = min([19] + [p[-1] for p in probes])
+    for a, bsz in zip(CHAIN, CHAIN[1:]):
+        if bsz < smallest:
+            break
+        chain[bsz] = conv('chain', chain[a], c0, c0, a, 3, 2, dw=True, gain=1.5)
+
+    def feed(c, hw):
+        return chain[hw] if c == c0 else conv('expand', chain[hw], c0, c, hw)
+
+    for pr in probes:
+        if pr[0] == 'gemm':
+            _, cin, cout, hw = pr
+            w, b = _probe_weights(g.rng, cin, cout, weights)
+            conv('probe', feed(cin, hw), cin, cout, hw, w=w, b=b)
+        elif pr[0] == 'dw':
+            _, c, k, s, hw = pr
+            conv('probe', feed(c, hw), c, c, hw, k, s, dw=True)
+        elif pr[0] == 'conv':
+            _, cin, cout, k, s, hw = pr
+            conv('probe', feed(cin, hw), cin, cout, hw, k, s)
+        else:
+            raise ValueError(pr)
+    n0 = len(g.layers)
+    _head(g, data, [(chain[19], c0)], 4, '-23300=1,60.000000 -23301=1,105.0 -23302=1,2.000000 7=1')
+    for L in g.layers[n0:]:
+        if L[0] == 'Convolution':
+            convs[L[3][0]] = dict(role='head', dw=False, cin=c0, cout=len(L[5][2]), k=1, s=1, p=0, hw=19, w=L[5][1], b=L[5][2], out=L[3][0],
+                                  **{'in': chain[19]})
+    os.makedirs(dirpath, exist_ok=True)
+    pp, bp = os.path.join(dirpath, name + '.param'), os.path.join(dirpath, name + '.bin')
+    g.write(pp, bp)
+    return pp, bp, convs
+
+
+def write_tail_model(dirpath, seed=0, name='tails'):
+    """Odd channel counts through the fused epilogues.  A 16-channel 19x19 map feeds seven 1x1 GEMMs 16 -> 7, one per tail kind the planner
+    recognises (ReLU, clip, hard-swish, +tensor, SE gate, SE tail) plus a generic chain (mul by a scalar, ReLU); each result goes back through a
+    dense 1x1 convolution 7 -> 16 added onto the map.  The SSD head has 3 priors per location (min, max, one aspect ratio, no flip) on 19x19 and
+    10x10: 63-channel confidence pieces, the second at the odd concat offset 19 * 19 * 63 = 22743, written straight into mbox_conf."""
+    g = Graph(seed)
+    data = g.add('Input', [], name='input')
+    x = g.conv(data, 3, 16, 3, 2, 1, gain=1 / 64)                                # activations of order one
+    for _ in range(3):
+        x = g.relu(g.conv(x, 16, 16, 3, 2, 1, dw=True))                           # 75, 38, 19
+    f = x
+
+    def gm():
+        return g.conv(f, 16, 7, gain=2.0)
+
+    a = g.relu(gm())                                                              # relu
+    cl = g.clip(gm())                                                             # clip
+    hs = g.hswish(gm())                                                           # hard-swish
+    ad = g.binop(gm(), a, 0)                                                      # + tensor
+    se = g.binop(cl, g.hsigmoid(gm()), 2)                                         # SE gate
+    st = g.binop(g.binop(hs, g.hsigmoid(gm()), 2), ad, 0)                         # SE tail
+    gen = g.relu(g.binop(gm(), g.const(0.5), 2))                                  # generic
+    h = f
+    for t in (a, cl, hs, ad, se, st, gen):
+        h = g.binop(g.conv(t, 7, 16, gain=0.5), h, 0)
+    h2 = g.relu(g.conv(h, 16, 16, 3, 2, 1, dw=True))                              # 10
+    _head(g, data, [(h, 16), (h2, 16)], 3, '-23300=1,60.000000 -23301=1,105.0 -23302=1,2.000000 7=0')
+    os.makedirs(dirpath, exist_ok=True)
+    pp, bp = os.path.join(dirpath, name + '.param'), os.path.join(dirpath, name + '.bin')
+    g.write(pp, bp)
+    return pp, bp
+
+
+# GEMM shapes (cin, cout, map) for the parity tests, at PROBE_FRAMES frames per batch: BK = 16 (cin <= 16) and 32 with a partial last k-step /
+# k-block (20, 36, 100, 964), streamed weights with more k-blocks than ring stages (960, 964), cout < 32 and odd (1, 21, 63: scalar stores),
+# an exact tile (32, 256), one channel past a tile (257), several output-channel tiles (600, 1000), 1 / 4 / 25 / 9 pixels per frame, and
+# 150 x 150 x 8 pixels (about ten 128-pixel tiles per persistent CTA).  The expansions c0 -> cin are GEMMs as well.
+PROBE_FRAMES = 8
+GEMM_PROBES = [('gemm', 16, 32, 150), ('gemm', 4, 21, 38), ('gemm', 12, 1, 1), ('gemm', 20, 63, 19), ('gemm', 36, 257, 10), ('gemm', 100, 600, 5),
+               ('gemm', 32, 256, 2), ('gemm', 960, 1000, 19), ('gemm', 964, 256, 3)]
+# depth-wise: V = 1 (c = 6, 10) and V = 4, k 3 / 5, stride 1 / 2, output maps under 4 rows (YT = 1) and larger, widths that are not a multiple of 4
+# (the chain itself adds 3x3/s2 on 16 channels at every size); dense: 3x3 with cin % 4 != 0, 1x1 / stride 2, 1x1 with cin % 4 != 0 and odd cout
+KERNEL_PROBES = [('dw', 6, 5, 1, 19), ('dw', 10, 3, 1, 5), ('dw', 6, 3, 2, 10), ('dw', 10, 5, 2, 3), ('dw', 16, 5, 1, 38), ('dw', 16, 5, 2, 19),
+                 ('dw', 16, 3, 1, 3), ('dw', 20, 3, 1, 10), ('conv', 6, 8, 3, 1, 19), ('conv', 16, 12, 1, 2, 19), ('conv', 6, 5, 1, 1, 10),
+                 ('conv', 10, 20, 3, 2, 10)]
+
+
+def check_probe_plans(plans):
+    """The plan features the GEMM parity tests rely on, on the conv1x1 lines (parse_plan) of a probe graph built from GEMM_PROBES at PROBE_FRAMES."""
+    by = {(p['cin'], p['cout'], p['h']): p for p in plans}
+    for _, cin, cout, hw in GEMM_PROBES:
+        assert (cin, cout, hw) in by, (cin, cout, hw)
+    assert by[(16, 32, 150)]['bk'] == 16 and by[(4, 21, 38)]['bk'] == 16 and by[(12, 1, 1)]['bk'] == 16                  # 64-byte swizzle
+    for cin in (20, 36, 100):
+        assert by[[k for k in by if k[0] == cin][0]]['bk'] == 32
+    assert any(p['bk'] == 32 and p['cin'] % 8 for p in plans) and any(p['bk'] == 32 and p['cin'] % 32 and p['kb'] > 1 for p in plans)
+    for key in ((960, 1000, 19), (964, 256, 3)):
+        p = by[key]
+        assert not p['wres'] and p['kb'] > p['stages'], p['line']                                                     # the ring wraps inside a tile
+    assert by[(960, 1000, 19)]['n_tiles'] >= 3 and by[(100, 600, 5)]['n_tiles'] >= 3                                 # several output-channel tiles
+    assert by[(36, 257, 10)]['n_tiles'] >= 2 and by[(32, 256, 2)]['nt'] * by[(32, 256, 2)]['n_tiles'] == 256
+    assert by[(16, 32, 150)]['nt'] == 32 and by[(16, 32, 150)]['n_tiles'] == 1
+    assert -(-PROBE_FRAMES * 150 * 150 // 128) >= 10 * 132                                                           # ~10 pixel tiles per CTA
+    for key in ((12, 1, 1), (4, 21, 38), (20, 63, 19)):
+        assert by[key]['cout'] % 2 and by[key]['off'] is None                                                         # odd pitch: scalar stores
+    assert by[(12, 1, 1)]['nt'] == 32 and by[(4, 21, 38)]['nt'] == 32                                                 # fewer than 32 real channels
+
+
+def parse_plan(describe_text):
+    """The conv1x1 lines of sgs_detector_describe as dicts: name, cin, cout, h, w, nt, n_tiles, kb, bk, stages, wres, smem, off (or None), line."""
+    import re
+    out = []
+    for l in describe_text.splitlines():
+        if not l.startswith('conv1x1 '):
+            continue
+        m = re.search(r'geom (\d+)x(\d+)x(\d+)->(\d+)x(\d+)x(\d+) .* tile (\d+)x(\d+) kb (\d+)x(\d+) stages (\d+)( wres)? smem (\d+)', l)
+        cin, h, w, cout, _, _, nt, ntl, kb, bk, st, wres, smem = m.groups()
+        off = re.search(r' off (\d+)', l)
+        out.append(dict(name=l.split()[1], out=l.split()[l.split().index('out') + 1], cin=int(cin), cout=int(cout), h=int(h), w=int(w), nt=int(nt),
+                        n_tiles=int(ntl), kb=int(kb), bk=int(bk), stages=int(st), wres=bool(wres), smem=int(smem), off=int(off.group(1)) if off else None,
+                        line=l))
+    return out
 
 
 def synthetic_rgb(h, w, seed):

@@ -118,6 +118,63 @@ def test_plan_fuses_elementwise_tails(tmp_path):
     assert sum(l.startswith('eltwise') for l in txt2.splitlines()) >= 20
 
 
+def test_probe_graphs_reach_the_planned_gemm_features(tmp_path):
+    """The probe graph of tests/test_gpu_detector_kernels.py, planned at the batch the GPU test runs: every GEMM plan feature its parity checks
+    rely on is reached (BK 16 / 32, partial k-steps, streamed weights with a wrapping ring, several N-tiles, odd output pitches), so that a planner
+    change cannot retire a case unnoticed; the odd-head graph fuses one tail of each kind into a 7-channel GEMM and writes a 63-channel
+    confidence piece at the odd offset 22743."""
+    pp, bp, convs = DM.write_probe_model(str(tmp_path), DM.GEMM_PROBES + DM.KERNEL_PROBES, 0)
+    d = B.Detector(pp, bp, max_frames=DM.PROBE_FRAMES, flags=B.DET_PLAN_ONLY)
+    txt = d.describe()
+    d.close()
+    plans = DM.parse_plan(txt)
+    DM.check_probe_plans(plans)
+    assert {p['name'] for p in plans} == {n for n, c in convs.items() if not c['dw'] and c['k'] == 1 and c['s'] == 1 and c['cin'] % 4 == 0}
+    ops = [l.split()[0] for l in txt.splitlines()[1:]]
+    assert ops.count('conv') == 1 + sum(p[0] == 'conv' for p in DM.KERNEL_PROBES) and txt.splitlines()[1].startswith('conv ')
+    pp, bp = DM.write_tail_model(str(tmp_path / 'tails'), 0)
+    d = B.Detector(pp, bp, max_frames=4, flags=B.DET_PLAN_ONLY)
+    txt = d.describe()
+    d.close()
+    tails = [p['line'].split(' | ', 1)[1] if ' | ' in p['line'] else '' for p in DM.parse_plan(txt) if p['cout'] == 7]
+    assert len(tails) == 7
+    pats = ['^relu$', '^clip 0 6$', r'^add 3 \| clip 0 6 \| mul\(rev\) start \| div 6$', r'^add \S+ buf \d+$',
+            r'^add 3 \| clip 0 6 \| div 6 \| mul\(rev\) \S+ buf \d+$', r'^add 3 \| clip 0 6 \| div 6 \| mul\(rev\) \S+ buf \d+ \| add \S+ buf \d+$',
+            r'^mul 0.5 \| relu$']
+    import re
+    for pat in pats:
+        assert sum(bool(re.match(pat, t)) for t in tails) == 1, (pat, tails)
+    heads = {(p['cout'], p['off']) for p in DM.parse_plan(txt) if p['off'] is not None}
+    assert heads == {(63, 0), (63, 22743), (12, 0), (12, 4332)}
+
+
+def test_gemm_plans_stay_inside_what_the_kernel_launches(tmp_path):
+    """Plans of 1x1 convolutions with 4 <= Cin <= 4096 (multiples of 4) and 1 <= Cout <= 4096 on maps of 1 to 150 pixels a side, at batches of 1,
+    8 and 64 frames: the shared memory fits a CTA (226 KB), the ring has 2..8 stages, the N-tile is a multiple of the 32-channel wgmma width of at
+    most 256 channels and the tiles cover Cout without an empty one -- launch_conv1x1_tc_map rejects anything else at run time."""
+    rng = np.random.default_rng(5)
+    cins = [4, 8, 12, 16, 20, 28, 32, 36, 60, 64, 100, 128, 132, 252, 256, 260, 512, 964, 1024, 2044, 4096]
+    couts = [1, 2, 31, 32, 33, 63, 96, 127, 129, 255, 256, 257, 300, 511, 513, 600, 1000, 1025, 2049, 4095, 4096]
+    pairs = list(zip(cins, rng.permutation(couts)))
+    pairs += [(4096, 4096), (4096, 1), (4, 4096), (256, 512), (1024, 1000)]
+    maps = [1, 2, 5, 19, 38, 150]
+    probes = [('gemm', cin, int(cout), maps[i % len(maps)]) for i, (cin, cout) in enumerate(pairs)]
+    pp, bp, _ = DM.write_probe_model(str(tmp_path), probes, 1, weights='zero')
+    seen = 0
+    for mf in (1, 8, 64):
+        d = B.Detector(pp, bp, max_frames=mf, flags=B.DET_PLAN_ONLY)
+        plans = DM.parse_plan(d.describe())
+        d.close()
+        for p in plans:
+            assert p['smem'] <= 226 * 1024, p['line']
+            assert 2 <= p['stages'] <= 8, p['line']
+            assert p['nt'] % 32 == 0 and 32 <= p['nt'] <= 256, p['line']
+            assert p['nt'] * (p['n_tiles'] - 1) < p['cout'] <= p['nt'] * p['n_tiles'], p['line']
+            assert p['bk'] == (16 if p['cin'] <= 16 else 32) and p['kb'] == -(-p['cin'] // p['bk']), p['line']
+            seen += 1
+    assert seen >= 3 * len(pairs)
+
+
 def test_folded_prior_boxes_match_the_oracle_bitwise(tmp_path):
     """The product folds PriorBox + Concat on the host at create time; in plan-only diagnostic mode the constant is readable without a device."""
     pp, bp = DM.write_mini_model(str(tmp_path), 0)

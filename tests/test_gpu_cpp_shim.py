@@ -13,21 +13,22 @@ from pysgs import synth
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-def _build():
-    exe = os.path.join(ROOT, 'tests', 'cpp', 'test_shim')
+def _build(out_dir):
+    """Compiles tests/cpp/test_shim.cpp into out_dir (the source tree may be read-only)."""
+    exe = os.path.join(out_dir, 'test_shim')
     src = os.path.join(ROOT, 'tests', 'cpp', 'test_shim.cpp')
     lib = os.path.join(ROOT, 'sg-slam_b200', 'lib')
     subprocess.check_call(['g++', '-O1', '-std=c++17', '-I', os.path.join(ROOT, 'include'), src, '-o', exe, '-L', lib, '-lsgs_cuda', '-Wl,-rpath,' + lib, '-ldl', '-lpthread', '-lrt'])
     return exe
 
 
-def test_shim_compiles_without_gpu():
-    _build()
+def test_shim_compiles_without_gpu(tmp_path):
+    _build(str(tmp_path))
 
 
 @pytest.mark.gpu
-def test_shim_on_gpu(tmp_path):
-    exe = _build()
+def test_shim_on_gpu_built_in_tmp(tmp_path):
+    exe = _build(str(tmp_path))
     img = synth.frame_s1(640, 480, 21)
     kps, desc = O.extract(img)
     s = S.random_lastframe_scenario(3, n_cur=900, n_last=1000)
