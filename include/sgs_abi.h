@@ -560,8 +560,9 @@ SGS_API int sgs_extractor_level0_device(const sgs_extractor* ex, const uint8_t**
 
 /* ------------------------------------------------------------------------------------
  * cv::calcOpticalFlowPyrLK as called at src/Frame.cc:445 (window 21x21, maxLevel 3, COUNT|EPS 30 / 0.01): tracks the CURRENT
- * frame's keypoints into the PREVIOUS gray image.  Positions agree with OpenCV to ~1e-4 px (float summation order), status/err
- * are not produced (the reference ignores them).
+ * frame's keypoints into the PREVIOUS gray image.  Window sums are exact integer sums, so positions equal bit for bit the exact-sum
+ * restatement in tests/lk_exact.py; that restatement agrees with OpenCV to ~1e-4 px (OpenCV sums in float, in SIMD order; tolerance
+ * in tests/test_gpu_lk.py).  status/err are not produced (the reference ignores them).
  *   sgs_lk_track              : one host image pair, n points (x, y) -> out (x, y)
  *   sgs_lk_track_batch_device : `nframes` device image pairs; points are the keypoints d_kps [F][cap] (counts [F]); writes
  *                               d_prev_xy [F][cap][2] -- the `prev_xy` input of the dyn-reject stage.  The previous images are
@@ -577,6 +578,11 @@ SGS_API int sgs_lk_track_batch_device(sgs_lk* k, const uint8_t* d_cur, const uin
                                       const int32_t* d_counts, int cap, float* d_prev_xy, void* stream);
 /* parity accessor: pyramid level (1..3) of frame 0 of the last call; which = 0 current image, 1 previous image */
 SGS_API int sgs_lk_read_level(sgs_lk* k, int which, int level, uint8_t* out, int out_pitch);
+/* parity accessor: the whole padded level (0..max_level) of batch frame `frame` as the tracker reads it, border included, after the
+ * stream of the last call has finished.  img [h + 2 pad][w + 2 pad] (REFLECT_101 border); for which == 0 also, when deriv != NULL,
+ * the derivative plane [h + 2 pad][w + 2 pad] as dx | dy << 16 (int16 halves, zero border); *pad (may be NULL) = the border width.
+ * which = 1 (the previous images) is only built by calls given d_prev, not d_prev_index. */
+SGS_API int sgs_lk_read_padded(sgs_lk* k, int which, int level, int frame, uint8_t* img, uint32_t* deriv, int* pad);
 /* Stage timing with CUDA events on the launching stream, like sgs_extractor_set_profiling / _stage_times:
  * ms_total2 = accumulated {pyramid build (cv::pyrDown levels), lk_track_kernel} over *ncalls calls. */
 SGS_API int sgs_lk_set_profiling(sgs_lk* k, int enable);

@@ -2,8 +2,9 @@
 // I = current gray, J = previous gray, window 21x21, 4 pyramid levels, <= 30 iterations or |delta|^2 <= 1e-4.
 // Follows OpenCV video/lkpyramid.cpp: cv::pyrDown levels (bit-exact integers), Scharr derivatives of I (int16, zero outside the
 // image), 14-bit fixed-point bilinear window extraction, float 2x2 solve.  Sums of integer products are accumulated EXACTLY
-// (int32/int64) and rounded once; OpenCV accumulates them in float in SIMD order, so positions agree to ~1e-4 px, not bit-for-bit
-// (tolerance stated in tests/test_gpu_lk.py).  status/err are not produced (the reference ignores them, quirk Q4); a level
+// (int32/int64) and rounded once, and every float step is an explicit round-to-nearest intrinsic, so the result equals the int64
+// restatement tests/lk_exact.py bit for bit (tests/test_gpu_lk_exact.py); OpenCV accumulates the sums in float in SIMD order, so
+// positions agree with it to ~1e-4 px, not bit-for-bit (tolerance stated in tests/test_gpu_lk.py).  status/err are not produced (the reference ignores them, quirk Q4); a level
 // that fails leaves the running estimate untouched (SURVEY A10).
 //
 // Like buildOpticalFlowPyramid, every level is stored with a border of kLkPad pixels (REFLECT_101) and has a derivative image
@@ -506,6 +507,19 @@ SGS_API int sgs_lk_read_level(sgs_lk* k, int which, int level, uint8_t* out, int
     SGS_CUDA_TRY(cudaStreamSynchronize(k->st));
     SGS_CUDA_TRY(cudaMemcpy2D(out, out_pitch, (which ? k->d_pyrJ : k->d_pyrI) + k->loff[level] + k->lorg[level], k->lp[level], k->lw[level], k->lh[level],
                               cudaMemcpyDeviceToHost));
+    return SGS_OK;
+}
+
+SGS_API int sgs_lk_read_padded(sgs_lk* k, int which, int level, int frame, uint8_t* img, uint32_t* deriv, int* pad) {   // parity accessor: a whole padded level
+    if (!k || !img || (which != 0 && which != 1) || (which == 1 && deriv) || level < 0 || level > k->max_level || frame < 0 || frame >= k->max_batch)
+        return lk_bad("sgs_lk_read_padded: bad argument");
+    SGS_CUDA_TRY(cudaSetDevice(k->device));
+    SGS_CUDA_TRY(cudaStreamSynchronize(k->st));
+    const int64_t o = k->loff[level] + (int64_t)frame * k->lfs[level];
+    const size_t pw = (size_t)k->lw[level] + 2 * kLkPad, ph = (size_t)k->lh[level] + 2 * kLkPad;
+    SGS_CUDA_TRY(cudaMemcpy2D(img, pw, (which ? k->d_pyrJ : k->d_pyrI) + o, k->lp[level], pw, ph, cudaMemcpyDeviceToHost));
+    if (deriv) SGS_CUDA_TRY(cudaMemcpy2D(deriv, 4 * pw, k->d_der + o, 4 * (size_t)k->lp[level], 4 * pw, ph, cudaMemcpyDeviceToHost));
+    if (pad) *pad = kLkPad;
     return SGS_OK;
 }
 

@@ -125,7 +125,7 @@ ABI_SYMBOLS = [
     'sgs_tracker_create', 'sgs_tracker_destroy', 'sgs_tracker_max_keypoints', 'sgs_tracker_extract', 'sgs_tracker_track',
     'sgs_tracker_extract_device', 'sgs_tracker_track_device', 'sgs_tracker_results_device', 'sgs_tracker_extractor',
     'sgs_extractor_set_profiling', 'sgs_extractor_stage_times',
-    'sgs_lk_create', 'sgs_lk_destroy', 'sgs_lk_track', 'sgs_lk_track_batch_device', 'sgs_lk_read_level',
+    'sgs_lk_create', 'sgs_lk_destroy', 'sgs_lk_track', 'sgs_lk_track_batch_device', 'sgs_lk_read_level', 'sgs_lk_read_padded',
     'sgs_tracker_lk_device', 'sgs_tracker_prev_xy_device', 'sgs_tracker_track_lk', 'sgs_extractor_level0_device', 'sgs_memcpy_d2h',
     'sgs_lk_set_profiling', 'sgs_lk_stage_times', 'sgs_tracker_lk',
     'sgs_pose_optimization_batch_device', 'sgs_pose_optimization', 'sgs_distinctive_descriptor_batch_device', 'sgs_fuse_search_batch_device', 'sgs_fuse_search', 'sgs_match_project_keyframe_batch_device', 'sgs_match_project_keyframe',
@@ -425,6 +425,7 @@ class Tracker:
 
 class LK:
     """cv::calcOpticalFlowPyrLK with the reference's parameters (sgs_lk_* of include/sgs_abi.h)."""
+    PAD = 24            # border of every padded pyramid level (kLkPad)
 
     def __init__(self, width, height, max_batch=1, device=0):
         self.h = C.c_void_p()
@@ -457,9 +458,24 @@ class LK:
         check(lib().sgs_lk_read_level(self.h, which, level, _p(out), w))
         return out
 
-    def track_batch_device(self, d_cur, d_prev, nframes, frame_stride, pitch, d_kps, d_counts, cap, d_prev_xy, stream=0):
+    def read_padded(self, which, level, frame=0):
+        """Padded level `level` of batch frame `frame`, border included: (image [h + 2 pad, w + 2 pad] u8, derivative plane
+        dx | dy << 16 of the same shape as uint32 for which == 0, else None)."""
+        w, h = self.width, self.height
+        for _ in range(level):
+            w, h = (w + 1) // 2, (h + 1) // 2
+        p, pad = self.PAD, C.c_int()
+        img = np.zeros((h + 2 * p, w + 2 * p), np.uint8)
+        der = np.zeros((h + 2 * p, w + 2 * p), np.uint32) if which == 0 else None
+        check(lib().sgs_lk_read_padded(self.h, which, level, frame, _p(img), _p(der), C.byref(pad)))
+        assert pad.value == p, pad.value
+        return img, der
+
+    def track_batch_device(self, d_cur, d_prev, nframes, frame_stride, pitch, d_kps, d_counts, cap, d_prev_xy, stream=0, d_prev_index=0):
+        """Previous images: d_prev [F], or frames of d_cur itself when d_prev_index [F] is given (then d_prev may be 0)."""
         v = C.c_void_p
-        check(lib().sgs_lk_track_batch_device(self.h, v(d_cur), v(d_prev), v(0), nframes, C.c_size_t(frame_stride), pitch, v(d_kps), v(d_counts), cap, v(d_prev_xy), v(stream)))
+        check(lib().sgs_lk_track_batch_device(self.h, v(d_cur), v(d_prev), v(d_prev_index), nframes, C.c_size_t(frame_stride), pitch, v(d_kps), v(d_counts),
+                                              cap, v(d_prev_xy), v(stream)))
 
 
 def fundamental_ransac(pts1, pts2, thresh=1.0, confidence=0.99, max_iters=1000, device=0):
