@@ -9,7 +9,7 @@
 //     lo*hi + hi*lo + hi*hi (the dropped lo*lo term is < 2^-22 relative).  Weights are split once at load time, activations in registers,
 //   * epilogue straight from the accumulator registers: bias -> fused element-wise tail -> NHWC store (each warp store covers whole 32-byte sectors).
 // One CTA = two consumer warpgroups + one TMA producer warpgroup, persistent over the pixel tiles of one output-channel tile: the producer refills the
-// ring while the consumers run the epilogue of the previous tile.
+// ring while the consumers run the epilogue of the previous tile.  Narrow tiles run two CTAs per SM, so one CTA's epilogue overlaps the other's MMAs.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -28,6 +28,10 @@ constexpr int kWN = 32;         // output channels per wgmma (m64n32k8)
 constexpr int kMaxNT = 256;     // output channels per tile (128 accumulator registers per consumer thread)
 constexpr int kMaxChunks = kMaxNT / kWN;
 constexpr int kThreads = 3 * 128;       // two consumer warpgroups + the producer warpgroup (one thread of it issues the loads)
+// Narrow tiles (one 32-channel chunk) run two CTAs per SM (conv1x1_tc_kernel): the accumulators and the split fragments of a k-block then fit the
+// 80 registers per thread that two 384-thread CTAs leave.  (Two CTAs of 64-channel tiles measured slower than one: see DESIGN.md section 4.)
+constexpr int kNarrowChunks = 1;
+constexpr int kNarrowSmem = 110 * 1024; // dynamic shared memory of such a CTA: two fit the 228 KB of an SM with their 1 KB reserves and static barriers
 
 // ---------------------------------------------------------------------------------------------------------------- PTX wrappers
 __device__ __forceinline__ uint32_t smem_addr(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -105,10 +109,17 @@ struct TcGeom {
 // mbarriers: full[s] (TMA -> consumers), empty[s] (every consumer warp's MMAs on slot s have completed -> producer), bfull (resident weights).
 // EpiFn: struct with  template <int N> __device__ void run(float (&v)[N], int64_t idx0) const   applied to N consecutive channels of one pixel;
 // idx0 = pixel * Cout + channel (the NHWC index of same-shape operand tensors).
-template <class EpiFn, int BKT>
-__global__ void __launch_bounds__(kThreads, 1) conv1x1_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapBh,
+// MAXC: the most 32-channel chunks a tile of this instantiation has (NT <= 32 * MAXC).  Narrow tiles (MAXC = kNarrowChunks) run two CTAs per SM
+// (ctas_per_sm): each CTA's epilogue -- the stores and the fused tail's operand loads -- overlaps the other CTA's MMAs; every thread keeps the
+// at most 80 registers that two 384-thread CTAs leave (no setmaxnreg split).  Wide tiles run one CTA per SM with the 232 / 40 split.
+template <int MAXC>
+constexpr int ctas_per_sm() { return MAXC < kMaxChunks ? 2 : 1; }
+template <class EpiFn, int BKT, int MAXC>
+__global__ void __launch_bounds__(kThreads, ctas_per_sm<MAXC>()) conv1x1_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapBh,
                                                               const __grid_constant__ CUtensorMap mapBl, const float* __restrict__ bias,
                                                               float* __restrict__ out, const TcGeom G, const EpiFn epi) {
+    static_assert(MAXC >= 1 && MAXC <= kMaxChunks, "chunks per tile");
+    constexpr bool kSplitRegs = ctas_per_sm<MAXC>() == 1;
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     __shared__ __align__(8) uint64_t s_full[kMaxStages], s_empty[kMaxStages], s_bfull;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -136,7 +147,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv1x1_tc_kernel(const __grid_co
 
     if (warp >= 8) {
         // ------------------------------------------------------------------------------------------------ TMA producer
-        asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");
+        if constexpr (kSplitRegs) asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");
         if (warp == 8 && lane == 0) {
             if (G.b_resident) {
                 mbar_expect_tx(smem_addr(&s_bfull), (uint32_t)G.KB * 2 * b_bytes);
@@ -167,17 +178,17 @@ __global__ void __launch_bounds__(kThreads, 1) conv1x1_tc_kernel(const __grid_co
     // ---------------------------------------------------------------------------------------------------- consumers
     // Fragment ownership (wgmma m64nNk8, tf32): warp w of the warpgroup owns rows 16w + g and 16w + g + 8 (g = lane / 4); the A fragment holds
     // columns t and t + 4 of the k-step (t = lane % 4), the accumulator of a 32-channel chunk the channel pairs 8j + 2t, j = 0..3.
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory");
+    if constexpr (kSplitRegs) asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory");
     const int wg = warp >> 2, g = lane >> 2, t = lane & 3;
     const int r0 = 64 * wg + 16 * (warp & 3) + g;                            // tile row of fragment rows 0 (and r0 + 8)
-    const int nch = G.NT / kWN;                                              // 32-channel chunks of the tile (uniform)
+    const int nch = G.NT / kWN;                                              // 32-channel chunks of the tile (uniform, <= MAXC)
     const int ncol = min(G.NT, G.Cout - n0);                                 // real output channels of this tile (uniform)
     if (G.b_resident) mbar_wait(smem_addr(&s_bfull), 0);
-    float acc[kMaxChunks][16];
+    float acc[MAXC][16];
     uint32_t g_ring = 0;
     for (int it = 0; it < my_tiles; ++it) {
 #pragma unroll
-        for (int c = 0; c < kMaxChunks; ++c)
+        for (int c = 0; c < MAXC; ++c)
 #pragma unroll
             for (int i = 0; i < 16; ++i) acc[c][i] = 0.f;
         for (int kb = 0; kb < G.KB; ++kb, ++g_ring) {
@@ -203,7 +214,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv1x1_tc_kernel(const __grid_co
             for (int j = 0; j < KS; ++j) {
                 if (j < ksteps) {
 #pragma unroll
-                    for (int c = 0; c < kMaxChunks; ++c) {
+                    for (int c = 0; c < MAXC; ++c) {
                         if (c < nch) {
                             const uint32_t b = bh0 + (uint32_t)(c * kWN * ROWB + j * 32);
                             wgmma_tf32_n32(acc[c], al[j], kmajor_desc<ROWB>(b));
@@ -230,7 +241,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv1x1_tc_kernel(const __grid_co
             float* o = out + G.base_off + off + n0;
             const int64_t idx = (int64_t)p * G.Cout + n0;
 #pragma unroll
-            for (int c = 0; c < kMaxChunks; ++c) {
+            for (int c = 0; c < MAXC; ++c) {
                 if (c * kWN >= ncol) break;
 #pragma unroll
                 for (int j = 0; j < 4; ++j) {
@@ -300,7 +311,8 @@ inline void split_tf32_host(float x, float& hi, float& lo) {
 }
 
 // Tiling of one layer (no device access): output-channel tiles of at most kMaxNT channels (a multiple of the 32-channel wgmma width), weights
-// resident when all their k-blocks fit in 128 KB, ring depth from what is left of the 227 KB of shared memory a CTA may use.
+// resident when all their k-blocks fit in 128 KB, ring depth from what is left of the 227 KB of shared memory a CTA may use.  Narrow tiles (at most
+// 32 channels, two CTAs per SM) fit everything in kNarrowSmem: weights resident when a ring of two stages still fits beside them.
 // m_tiles (128-pixel tiles of the largest batch, 0 = unknown) picks the number of output-channel tiles: every tile of a pixel block re-reads the
 // activations and pays the pipeline's fill, so fewer, wider tiles win as long as they still fill the machine.  The cost of a plan is modelled as
 // waves of the persistent grid (one CTA per SM) x (NT + 100)  and the cheapest tile count between Cout / 256 and Cout / 128 is taken.
@@ -324,8 +336,10 @@ inline void plan_tiling(int Cin, int Cout, GemmPlan* P, int force_nt = 0, int m_
     P->Kp = P->KB * P->BK; P->Np = P->n_tiles * P->NT;
     const int a_stage = kBM * P->BK * 4, b_block = 2 * P->NT * P->BK * 4;
     const int b_all = P->KB * b_block;
-    P->b_resident = b_all <= 128 * 1024 ? 1 : 0;
-    const int budget = 226 * 1024 - 1024 - (P->b_resident ? b_all : 0);
+    const bool narrow = P->NT <= kNarrowChunks * kWN;            // two CTAs per SM: each gets at most kNarrowSmem
+    const int cap = narrow ? kNarrowSmem : 226 * 1024;
+    P->b_resident = (narrow ? b_all + 2 * a_stage + 1024 <= cap : b_all <= 128 * 1024) ? 1 : 0;
+    const int budget = cap - 1024 - (P->b_resident ? b_all : 0);
     const int stage_bytes = a_stage + (P->b_resident ? 0 : b_block);
     int st = budget / stage_bytes;
     if (st > kMaxStages) st = kMaxStages;
@@ -377,16 +391,25 @@ inline bool launch_conv1x1_tc_map(const GemmPlan& P, const CUtensorMap& mapA, in
     G.HW = HW; G.frame_stride = frame_stride; G.base_off = base_off; G.pitch = pitch;
     G.vec_ok = ((pitch & 1) == 0 && (frame_stride & 1) == 0 && (base_off & 1) == 0 && (((uintptr_t)out) & 7) == 0) ? 1 : 0;
     G.coalesce = (frame_stride == 0 || frame_stride == (int64_t)HW * pitch) ? 1 : 0;
-    int gx = sm_count() / P.n_tiles;                                    // one wave of persistent CTAs
-    if (gx < 1) gx = 1;
-    if (gx > G.m_tiles) gx = G.m_tiles;
-    const dim3 grid(gx, P.n_tiles);
+    const bool narrow = P.NT <= kNarrowChunks * kWN;
+    if (narrow && P.smem_bytes > kNarrowSmem) return false;
     auto go = [&](auto kern) -> bool {
         if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024) != cudaSuccess) return false;   // cheap; per device
-        kern<<<grid, kThreads, P.smem_bytes, st>>>(mapA, P.map_hi, P.map_lo, bias, out, G, epi);
+        // one wave of persistent CTAs: as many per SM as the registers and shared memory hold (two for narrow tiles, one otherwise)
+        int per_sm = 1;
+        if (narrow && (cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared) != cudaSuccess ||
+                       cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kThreads, P.smem_bytes) != cudaSuccess || per_sm < 1))
+            return false;
+        int gx = sm_count() * per_sm / P.n_tiles;
+        if (gx < 1) gx = 1;
+        if (gx > G.m_tiles) gx = G.m_tiles;
+        kern<<<dim3(gx, P.n_tiles), kThreads, P.smem_bytes, st>>>(mapA, P.map_hi, P.map_lo, bias, out, G, epi);
         return true;
     };
-    if (!(P.BK == 16 ? go(conv1x1_tc_kernel<EpiFn, 16>) : go(conv1x1_tc_kernel<EpiFn, 32>))) return false;
+    bool ok;
+    if (narrow) ok = P.BK == 16 ? go(conv1x1_tc_kernel<EpiFn, 16, kNarrowChunks>) : go(conv1x1_tc_kernel<EpiFn, 32, kNarrowChunks>);
+    else ok = P.BK == 16 ? go(conv1x1_tc_kernel<EpiFn, 16, kMaxChunks>) : go(conv1x1_tc_kernel<EpiFn, 32, kMaxChunks>);
+    if (!ok) return false;
     return cudaGetLastError() == cudaSuccess;
 }
 
