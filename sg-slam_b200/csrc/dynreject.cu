@@ -7,6 +7,7 @@
 
 #include <vector>
 
+#include "host_stage.cuh"
 #include "sgs_common.h"
 
 namespace sgs {
@@ -126,21 +127,21 @@ SGS_API int sgs_dynreject(const float* cur_xy, const float* prev_xy, int n, cons
     *nkeep = n;
     if (restored) *restored = 0;
     SGS_CUDA_TRY(cudaSetDevice(device));
-    void *dc = nullptr, *dp = nullptr, *dF = nullptr, *db = nullptr, *dk = nullptr, *dd = nullptr;
-    struct Guard { void** p[6]; ~Guard() { for (auto q : p) if (*q) cudaFree(*q); } } guard{{&dc, &dp, &dF, &db, &dk, &dd}};
     if (n > 0) {
-        SGS_CUDA_TRY(cudaMalloc(&dc, 8 * (size_t)n)); SGS_CUDA_TRY(cudaMalloc(&dp, 8 * (size_t)n));
-        SGS_CUDA_TRY(cudaMalloc(&dF, 72)); SGS_CUDA_TRY(cudaMalloc(&db, sizeof(sgs_rect) * (size_t)(nboxes > 0 ? nboxes : 1)));
-        SGS_CUDA_TRY(cudaMalloc(&dk, n)); SGS_CUDA_TRY(cudaMalloc(&dd, 8 * (size_t)n));
-        SGS_CUDA_TRY(cudaMemcpy(dc, cur_xy, 8 * (size_t)n, cudaMemcpyHostToDevice));
-        SGS_CUDA_TRY(cudaMemcpy(dp, prev_xy, 8 * (size_t)n, cudaMemcpyHostToDevice));
-        if (F) SGS_CUDA_TRY(cudaMemcpy(dF, F, 72, cudaMemcpyHostToDevice));
-        if (nboxes) SGS_CUDA_TRY(cudaMemcpy(db, boxes, sizeof(sgs_rect) * nboxes, cudaMemcpyHostToDevice));
-        dynreject_flags_kernel<<<(n + 255) / 256, 256>>>((const float2*)dc, (const float2*)dp, n, (const double*)dF, F ? 1 : 0, (const sgs_rect*)db, nboxes,
-                                                         have_dyn, (uint8_t*)dk, (double*)dd);
-        SGS_CUDA_TRY(cudaGetLastError());
-        SGS_CUDA_TRY(cudaMemcpy(keep, dk, n, cudaMemcpyDeviceToHost));
-        if (dist) SGS_CUDA_TRY(cudaMemcpy(dist, dd, 8 * (size_t)n, cudaMemcpyDeviceToHost));
+        const float *dc, *dp;
+        const double* dF;
+        const sgs_rect* db;
+        uint8_t* dk;
+        double* dd;
+        HostStage S("sgs_dynreject");
+        S.in(&dc, cur_xy, 2 * (size_t)n); S.in(&dp, prev_xy, 2 * (size_t)n); S.opt(&dF, F, 9); S.in(&db, boxes, nboxes);
+        S.out(&dk, n); S.out(&dd, n);
+        if (S.commit() != SGS_OK) return SGS_ERR_CUDA;
+        dynreject_flags_kernel<<<(n + 255) / 256, 256>>>((const float2*)dc, (const float2*)dp, n, dF, F ? 1 : 0, db, nboxes, have_dyn, dk, dd);
+        S.check(cudaGetLastError());
+        S.to_host(keep, dk, n);
+        if (dist) S.to_host(dist, dd, n);
+        if (S.status() != SGS_OK) return SGS_ERR_CUDA;
     }
     int sum = 0;
     for (int i = 0; i < n; ++i) sum += keep[i];

@@ -114,8 +114,22 @@ def test_host_variants():
                                       C.c_float(0.7), 1, m.ctypes.data_as(v), C.byref(nm), 0))
         onm, om = O.search_by_bow(kn, kw, s['kf_valid'], s['kf_desc'], s['kf_angle'], fn, fw, s['f_desc'], s['f_angle'], 0.7, True)
         assert nm.value == onm and np.array_equal(m, om)
+        B.check(B.lib().sgs_bow_transform(gv.h, None, 0, 1, None, None, None))              # nothing to transform: no device work
     finally:
         gv.close()
+
+
+def _match_bow_keyframes_host(mode, k1, k2, nnratio, ori, F12=None, epipole=None, sigma2=None, sf=None, only_stereo=0):
+    """sgs_match_bow_keyframes, the single-pair host entry point: (nmatches, match12)."""
+    P = lambda a, dt=None: None if a is None else np.ascontiguousarray(a, dt).ctypes.data_as(C.c_void_p)
+    side = lambda k: [P(k['node'], np.int32), P(k['weight'], np.float64), P(k['valid'], np.uint8), P(k['desc'], np.uint8), P(k['angle'], np.float32)]
+    n1, n2 = len(k1['desc']), len(k2['desc'])
+    m = np.full(n1, 7, np.int32); nm = C.c_int(-1)
+    B.check(B.lib().sgs_match_bow_keyframes(mode, n1, *side(k1), n2, *side(k2), C.c_float(nnratio), int(ori), P(k1.get('stereo'), np.uint8), P(k2.get('stereo'), np.uint8),
+                                            P(k1.get('xy'), np.float32), P(k2.get('xy'), np.float32), P(k2.get('octave'), np.int32), P(F12, np.float32),
+                                            P(epipole, np.float32), P(sigma2, np.float32), P(sf, np.float32), 0 if sf is None else len(sf), int(only_stereo),
+                                            P(m), C.byref(nm), 0))
+    return nm.value, m
 
 
 @pytest.mark.parametrize('seed,n1,n2,nnratio', [(1, 1000, 1000, 0.8), (2, 600, 1100, 0.75)])
@@ -152,6 +166,9 @@ def test_search_by_bow_keyframe_pair(seed, n1, n2, nnratio):
             assert int(nm.cpu()[0]) == onm and np.array_equal(m.cpu().numpy()[0, :n1], om) and onm > 30
             sel = om >= 0
             assert np.all(valid2[om[sel]] == 1) and len(set(om[sel].tolist())) == int(sel.sum())       # only good map points, each used once
+            hnm, hm = _match_bow_keyframes_host(1, dict(node=on1, weight=ow1, valid=s['kf_valid'], desc=s['kf_desc'], angle=s['kf_angle']),
+                                                dict(node=on2, weight=ow2, valid=valid2, desc=s['f_desc'], angle=s['f_angle']), nnratio, ori)
+            assert hnm == onm and np.array_equal(hm, om)
     finally:
         gv.close()
 
@@ -210,6 +227,9 @@ def test_search_for_triangulation(seed, only_stereo):
             assert np.all(free1[sel] == 1) and np.all(free2[om[sel]] == 1)
             if only_stereo:
                 assert np.all(st1[sel] == 1) and np.all(st2[om[sel]] == 1)
+            hnm, hm = _match_bow_keyframes_host(2, dict(k1, valid=free1), dict(k2, valid=free2), 0.6, ori, F12=F12, epipole=np.array([ex, ey], np.float32),
+                                                sigma2=sigma2, sf=sf, only_stereo=only_stereo)
+            assert hnm == onm and np.array_equal(hm, om)
     finally:
         gv.close()
 

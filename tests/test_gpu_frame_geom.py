@@ -50,6 +50,16 @@ def test_frustum_golden(golden_dir):
     out = _frustum_gpu(g['Tcw'].reshape(1, 16), g['cam'], g['xyz'].reshape(1, n, 3), g['normal'].reshape(1, n, 3), g['min_dist'].reshape(1, n),
                        g['max_dist'].reshape(1, n), [n], n)
     _same({k: v[0] for k, v in out.items()}, g, g['level_arg'])
+    # the host entry point on the same inputs
+    cam9 = g['cam']
+    cam = B.make_camera(640, 480, dict(fx=cam9[0], fy=cam9[1], cx=cam9[2], cy=cam9[3], bf=cam9[4]), S.scale_factors())
+    cam.min_x, cam.min_y, cam.max_x, cam.max_y = [float(x) for x in cam9[5:9]]
+    h = dict(inview=np.full(n, 7, np.uint8), proj_x=np.zeros(n, np.float32), proj_y=np.zeros(n, np.float32), proj_xr=np.zeros(n, np.float32),
+             level=np.zeros(n, np.int32), view_cos=np.zeros(n, np.float32))
+    P = lambda a: np.ascontiguousarray(a).ctypes.data_as(C.c_void_p)
+    B.check(B.lib().sgs_frustum(C.byref(cam), P(g['Tcw'].astype(np.float32)), n, P(g['xyz']), P(g['normal']), P(g['min_dist']), P(g['max_dist']), C.c_float(0.5),
+                                *[P(h[k]) for k in ('inview', 'proj_x', 'proj_y', 'proj_xr', 'level', 'view_cos')], 0))
+    _same(h, g, g['level_arg'])
 
 
 def test_frustum_batch_against_oracle():

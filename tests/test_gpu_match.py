@@ -238,6 +238,22 @@ def test_fuse_search(seed, ncur, nmp, th, sim3):
     B.check(B.lib().sgs_fuse_search_batch_device(C.byref(a), 1, C.c_void_p(0)))
     torch.cuda.synchronize()
     assert np.array_equal(bi.cpu().numpy()[0, :nmp], bi_o) and np.array_equal(bd.cpu().numpy()[0, :nmp], bd_o)
+    # the host entry point on the same inputs
+    fg = B.HostFrame(s['kps'], s['uright'], s['desc'], 640, 480, cam['fx'], cam['fy'], cam['cx'], cam['cy'], cam['bf'], s['sf'])
+    nm_h, bi_h, bd_h = _fuse_search_host(fg, s['Tcw_cur'], Ow, s, nrm, th, inv_s2, sim3, xf, None)
+    assert np.array_equal(bi_h, bi_o) and np.array_equal(bd_h, bd_o) and nm_h == 0
+
+
+def _fuse_search_host(fg, Tcw, Ow, s, nrm, th, inv_s2, sim3, xf, kf_matched):
+    """sgs_fuse_search, the single-frame host entry point: (nmatches, best_idx, best_dist); kf_matched is updated in place."""
+    import ctypes as C
+    nmp = len(s['kf_valid'])
+    P = lambda a: None if a is None else np.ascontiguousarray(a).ctypes.data_as(C.c_void_p)
+    bi = np.full(nmp, 7, np.int32); bd = np.full(nmp, 7, np.int32); nm = C.c_int(-1)
+    B.check(B.lib().sgs_fuse_search(C.byref(fg.c), P(Tcw.astype(np.float32).reshape(16)), P(Ow.astype(np.float32)), nmp, P(s['kf_valid']), P(s['last_xyz']), P(nrm),
+                                    P(s['min_dist']), P(s['max_dist']), P(s['last_desc']), C.c_float(th), P(inv_s2), sim3, P(xf), P(bi), P(bd),
+                                    P(kf_matched), C.byref(nm), 0))
+    return nm.value, bi, bd
 
 
 @pytest.mark.parametrize('seed,ncur,nmp,th', [(11, 600, 900, 10), (12, 300, 1500, 10), (13, 800, 800, 4), (14, 1000, 3000, 10)])
@@ -282,6 +298,11 @@ def test_search_by_projection_sim3(seed, ncur, nmp, th):
         claimed = np.nonzero((matched < 0) & (m_o >= 0))[0]
         assert np.array_equal(np.sort(bi_h[k, m_o[claimed]]), np.sort(claimed))             # best_idx[i] = the feature point i claimed
         assert (bi_h[k, :nmp] >= 0).sum() == nm_o
+        # the host entry point on the same key frame
+        fg = B.HostFrame(s['kps'], s['uright'], s['desc'], 640, 480, s['cam']['fx'], s['cam']['fy'], s['cam']['cx'], s['cam']['cy'], s['cam']['bf'], s['sf'])
+        km = matched.astype(np.int32).copy()
+        nm_h, bi_1, _ = _fuse_search_host(fg, s['Tcw_cur'], Ow, s, nrm, float(th), None, 3, None, km)
+        assert nm_h == nm_o and np.array_equal(km, m_o) and np.array_equal(bi_1, bi_h[k, :nmp])
     a.kf_matched = None
     with pytest.raises(B.SgsError):
         B.check(B.lib().sgs_fuse_search_batch_device(C.byref(a), 2, C.c_void_p(0)))

@@ -48,17 +48,46 @@ def _gpu(scs, cap, use_index):
     return Tout.cpu().numpy().reshape(F, 4, 4), outl.cpu().numpy(), nin.cpu().numpy()
 
 
-@pytest.mark.parametrize('use_index', [False, True])
-def test_pose_optimization_batch(use_index):
+def _host(s):
+    """sgs_pose_optimization, the single-frame host entry point."""
+    m = len(s['xy'])
+    kps = np.zeros(m, B.KP_DTYPE); kps['x'] = s['xy'][:, 0]; kps['y'] = s['xy'][:, 1]; kps['octave'] = s['octave']
+    s2 = np.zeros(16, np.float32); s2[:len(s['inv_s2'])] = s['inv_s2']
+    T = np.zeros(16, np.float32); outl = np.full(m, 9, np.uint8); nin = C.c_int(-1)
+    P = lambda a: np.ascontiguousarray(a).ctypes.data_as(C.c_void_p)
+    cam = B.make_camera(640, 480, s['cam'], S.scale_factors())
+    B.check(B.lib().sgs_pose_optimization(C.byref(cam), P(s['T0'].astype(np.float32).reshape(16)), m, P(kps), P(s['uright'].astype(np.float32)), P(s['has']),
+                                          P(s['xyz'].astype(np.float32)), P(s2), P(T), P(outl), C.byref(nin), 0))
+    return T.reshape(4, 4), outl, nin.value
+
+
+def _scenarios():
     scs = [S.pose_scenario(1), S.pose_scenario(2, n=300, outlier_frac=0.3), S.pose_scenario(3, n=1000, mono_frac=1.0), S.pose_scenario(4, n=1000, mono_frac=0.0, noise=1.0),
            S.pose_scenario(5, n=600, outlier_frac=0.0, noise=0.2), S.pose_scenario(6, n=900, pose_err=(0.08, 0.2))]
     few = dict(S.pose_scenario(7, n=40)); few['has'] = np.zeros(40, np.uint8); few['has'][:2] = 1; scs.append(few)           # < 3 correspondences
     few2 = dict(S.pose_scenario(8, n=40)); few2['has'] = np.zeros(40, np.uint8); few2['has'][:8] = 1; scs.append(few2)       # < 10 edges: one round
+    return scs
+
+
+def _check(f, s, T, outl, nin):
+    c = s['cam']; m = len(s['xy'])
+    rn, rT, ro = O.pose_optimization(s['T0'], s['has'], s['xyz'], s['xy'], s['octave'], s['uright'], s['inv_s2'], c['fx'], c['fy'], c['cx'], c['cy'], c['bf'])
+    assert np.abs(T - rT).max() <= 1e-6, (f, np.abs(T - rT).max())
+    used = s['has'] == 1
+    assert np.array_equal(outl[:m][used], ro[used]), (f, int((outl[:m][used] != ro[used]).sum()))
+    assert nin == rn, (f, nin, rn)
+
+
+@pytest.mark.parametrize('use_index', [False, True])
+def test_pose_optimization_batch(use_index):
+    scs = _scenarios()
     T, outl, nin = _gpu(scs, 1000, use_index)
     for f, s in enumerate(scs):
-        c = s['cam']; m = len(s['xy'])
-        rn, rT, ro = O.pose_optimization(s['T0'], s['has'], s['xyz'], s['xy'], s['octave'], s['uright'], s['inv_s2'], c['fx'], c['fy'], c['cx'], c['cy'], c['bf'])
-        assert np.abs(T[f] - rT).max() <= 1e-6, (f, np.abs(T[f] - rT).max())
-        used = s['has'] == 1
-        assert np.array_equal(outl[f, :m][used], ro[used]), (f, int((outl[f, :m][used] != ro[used]).sum()))
-        assert nin[f] == rn, (f, nin[f], rn)
+        _check(f, s, T[f], outl[f], nin[f])
+
+
+def test_pose_optimization_host_entry_point():
+    for f, s in enumerate(_scenarios()):
+        T, outl, nin = _host(s)
+        _check(f, s, T, outl, nin)
+        assert (outl[s['has'] == 0] == 0).all()             # the outlier flags are cleared before the optimisation
