@@ -103,18 +103,23 @@ def prior_boxes(L, fw, fh, iw, ih):
     return np.stack([box, np.tile(np.array(var, np.float32), len(box) // 4)])
 
 
-def detection_output(L, loc, conf, prior):
-    """ncnn DetectionOutput: decode with the prior variances, per-class threshold + top-k + greedy NMS, global top-k.
-    Returns rows [label, score, xmin, ymin, xmax, ymax] (normalised coordinates)."""
-    ncls, nms_thr, nms_topk, keep_topk, conf_thr = L.p(0), np.float32(L.p(1, 0.05)), L.p(2, 300), L.p(3, 100), np.float32(L.p(4, 0.5))
+def decode_boxes(loc, prior):
+    """DetectionOutput's box decoding: prior boxes moved by the location offsets scaled by the prior variances -> [prior][xmin, ymin, xmax, ymax]"""
     loc = loc.reshape(-1, 4).astype(np.float32); pb = prior[0].reshape(-1, 4); var = prior[1].reshape(-1, 4)
-    conf = conf.reshape(-1, ncls).astype(np.float32)
     half = np.float32(0.5)
     pw = pb[:, 2] - pb[:, 0]; ph = pb[:, 3] - pb[:, 1]
     pcx = (pb[:, 0] + pb[:, 2]) * half; pcy = (pb[:, 1] + pb[:, 3]) * half
     cx = var[:, 0] * loc[:, 0] * pw + pcx; cy = var[:, 1] * loc[:, 1] * ph + pcy
     w = np.exp(var[:, 2] * loc[:, 2]).astype(np.float32) * pw; h = np.exp(var[:, 3] * loc[:, 3]).astype(np.float32) * ph
-    boxes = np.stack([cx - w * half, cy - h * half, cx + w * half, cy + h * half], 1).astype(np.float32)
+    return np.stack([cx - w * half, cy - h * half, cx + w * half, cy + h * half], 1).astype(np.float32)
+
+
+def detection_output(L, loc, conf, prior):
+    """ncnn DetectionOutput: decode with the prior variances, per-class threshold + top-k + greedy NMS, global top-k.
+    Returns rows [label, score, xmin, ymin, xmax, ymax] (normalised coordinates)."""
+    ncls, nms_thr, nms_topk, keep_topk, conf_thr = L.p(0), np.float32(L.p(1, 0.05)), L.p(2, 300), L.p(3, 100), np.float32(L.p(4, 0.5))
+    conf = conf.reshape(-1, ncls).astype(np.float32)
+    boxes = decode_boxes(loc, prior)
     rows = []
     for c in range(1, ncls):
         idx = np.nonzero(conf[:, c] > conf_thr)[0]
@@ -123,17 +128,12 @@ def detection_output(L, loc, conf, prior):
         picked = []
         for i in idx:
             b = boxes[i]; area = (b[2] - b[0]) * (b[3] - b[1])
-            keep = True
-            for jdx in picked:
-                a = boxes[jdx]
-                if b[0] > a[2] or b[2] < a[0] or b[1] > a[3] or b[3] < a[1]:
-                    inter = np.float32(0)
-                else:
-                    inter = (min(a[2], b[2]) - max(a[0], b[0])) * (min(a[3], b[3]) - max(a[1], b[1]))
-                union = (a[2] - a[0]) * (a[3] - a[1]) + area - inter
-                if inter / union > nms_thr:
-                    keep = False; break
-            if keep: picked.append(i)
+            a = boxes[picked].T                                  # every kept box at once: the same float32 operations, element by element
+            apart = (b[0] > a[2]) | (b[2] < a[0]) | (b[1] > a[3]) | (b[3] < a[1])
+            inter = np.where(apart, np.float32(0), (np.minimum(a[2], b[2]) - np.maximum(a[0], b[0])) * (np.minimum(a[3], b[3]) - np.maximum(a[1], b[1])))
+            union = (a[2] - a[0]) * (a[3] - a[1]) + area - inter
+            if not (inter / union > nms_thr).any():
+                picked.append(i)
         rows += [(c, conf[i, c], i) for i in picked]
     rows.sort(key=lambda r: (-r[1], r[0], r[2]))
     rows = rows[:keep_topk]

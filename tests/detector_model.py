@@ -309,6 +309,121 @@ def parse_plan(describe_text):
     return out
 
 
+def head_prior_count(maps):
+    """Priors per location of each head map (hw, min_size, max_size or None, aspect ratios, flip): min box, max box, each ratio (and its flip)."""
+    return [1 + (mx is not None) + len(ars) * (2 if flip else 1) for _, _, mx, ars, flip in maps]
+
+
+def _f9(v):
+    """a float32 parameter as ncnn text that reads back as the same float32"""
+    return '%.9g' % float(np.float32(v))
+
+
+def write_head_model(dirpath, maps, ncls, weights='zero', conf_bias=None, loc_bias=None, nms_thr=0.45, nms_topk=300, keep_topk=100, conf_thr=0.01,
+                     seed=0, c=8, conf_gain=1.0, loc_gain=1.0, name='head'):
+    """A graph that is mostly SSD head, for the Softmax / DetectionOutput parity tests.
+
+    Input 3x300x300 -> dense 3x3/s2 stem 3 -> c + ReLU -> depth-wise 3x3/s2 + ReLU chain (CHAIN).  A map size off the chain is reached from the
+    nearest larger chain map of the same parity by unpadded depth-wise 5x5 / 3x3 layers (-4 / -2 per layer).  Each entry of `maps`,
+    (hw, min_size, max_size or None, aspect ratios, flip), gets a conf and a loc 1x1 convolution and a PriorBox (head_prior_count priors per
+    location, mmdetection centres, no clip), concatenated in order into mbox_conf / mbox_loc / mbox_priorbox, then
+    Reshape -> Softmax (blob mbox_conf_softmax) -> Flatten -> DetectionOutput with the given parameters, written so that they read back as the
+    same float32.
+      weights='zero'    head weights are zero: conf_bias[i] ([npr][ncls], broadcast) and loc_bias[i] ([npr][4], default 0) are the outputs at every
+                        location of map i, so every location of a prior type scores the same and, with loc 0, every box is its prior box decoded with zero offsets
+                        (the same float32 operations on the device and in the restatement);
+      weights='random'  normal head weights (gain conf_gain / loc_gain); biases as given, else random.
+    Returns (param path, bin path, priors per location of each map)."""
+    g = Graph(seed)
+    data = g.add('Input', [], name='input')
+    chain = {150: g.relu(g.conv(data, 3, c, 3, 2, 1, gain=1 / 64))}
+    for a, b in zip(CHAIN, CHAIN[1:]):
+        chain[b] = g.relu(g.conv(chain[a], c, c, 3, 2, 1, dw=True, gain=1.5))
+    nprs = head_prior_count(maps)
+    locs, confs, priors = [], [], []
+    for i, ((hw, mn, mx, ars, flip), npr) in enumerate(zip(maps, nprs)):
+        size = min(s for s in CHAIN if s >= hw and (s - hw) % 2 == 0)
+        f = chain[size]
+        while size > hw:
+            k = 5 if size - hw >= 4 else 3
+            f = g.relu(g.conv(f, c, c, k, 1, 0, dw=True, gain=1.5))
+            size -= k - 1
+        zero = weights == 'zero'
+        if not zero and weights != 'random':
+            raise ValueError(weights)
+        cb = conf_bias[i] if conf_bias is not None else (None if not zero else 0.0)
+        lb = loc_bias[i] if loc_bias is not None else (None if not zero else 0.0)
+        cb = None if cb is None else np.broadcast_to(np.asarray(cb, np.float32), (npr, ncls)).reshape(-1).copy()
+        lb = None if lb is None else np.broadcast_to(np.asarray(lb, np.float32), (npr, 4)).reshape(-1).copy()
+        cf = g.conv(f, c, npr * ncls, gain=conf_gain, w=np.zeros((npr * ncls, c, 1, 1), np.float32) if zero else None, b=cb)
+        confs.append(g.add('Flatten', [g.add('Permute', [cf], '0=3')]))
+        lc = g.conv(f, c, npr * 4, gain=loc_gain, w=np.zeros((npr * 4, c, 1, 1), np.float32) if zero else None, b=lb)
+        locs.append(g.add('Flatten', [g.add('Permute', [lc], '0=3')]))
+        pb = '-23300=1,%s' % _f9(mn)
+        if mx is not None:
+            pb += ' -23301=1,%s' % _f9(mx)
+        if ars:
+            pb += ' -23302=%d,%s' % (len(ars), ','.join(_f9(a) for a in ars))
+        priors.append(g.add('PriorBox', [f, data], pb + ' 3=0.100000 4=0.100000 5=0.200000 6=0.200000 7=%d 8=0 9=-233 10=-233 11=-233.000000 '
+                                                        '12=-233.000000 13=0.500000 14=1 15=1' % (1 if flip else 0)))
+    loc = g.add('Concat', locs, '0=0', name='mbox_loc')
+    conf = g.add('Concat', confs, '0=0', name='mbox_conf')
+    pri = g.add('Concat', priors, '0=1', name='mbox_priorbox')
+    sm = g.add('Softmax', [g.add('Reshape', [conf], '0=%d 1=-1' % ncls)], '0=1 1=1', name='mbox_conf_softmax')
+    g.add('DetectionOutput', [loc, g.add('Flatten', [sm]), pri], '0=%d 1=%s 2=%d 3=%d 4=%s' % (ncls, _f9(nms_thr), nms_topk, keep_topk, _f9(conf_thr)),
+          name='detection_out')
+    os.makedirs(dirpath, exist_ok=True)
+    pp, bp = os.path.join(dirpath, name + '.param'), os.path.join(dirpath, name + '.bin')
+    g.write(pp, bp)
+    return pp, bp, nprs
+
+
+HEAD_MAPS = [(19, 60.0, 105.0, (2.0,), True), (10, 105.0, 150.0, (2.0, 3.0), True)]        # 19 * 19 * 4 + 10 * 10 * 6 = 2044 priors
+CAP_MAP = (32, 30.0, 45.0, (2.0,), True)                                                 # 32 * 32 * 4 = 4096 priors (kDetSortCap)
+
+
+def head_scene(name):
+    """write_head_model keyword arguments of the graphs of tests/test_gpu_detector_head.py.
+      planted  zero head weights, 21 classes; conf logits per (prior type, class) from {-3, 0, 1, 2.5} (background 2): exact score ties inside a
+               class (every location of a prior type) and across classes (equal logits of one prior type); the person class (15) high on one prior
+               type of the 10x10 map; several classes with more candidates than nms_top_k,
+               keep_top_k 200 (a score tie across two classes falls inside it);
+      iou      one 1x1 map with a min and a max box (concentric): class 1 scores the min box above the max box;
+      cap      4096 priors, 33 classes, every prior above conf_thr in every class (logits {-0.5, 0, 0.5}), nms_thr 1 (nothing suppressed),
+               nms_top_k 256: (33 - 1) * 256 = 8192 kept entries reach the merge (kMergeCap), keep_top_k 1024;
+      random   random head weights and biases, 21 classes (random32 / random40: 32 / 40, the last Softmax register width and the loop path),
+               conf_thr 0.3; candidates depend on the frame."""
+    rng = np.random.default_rng(5)
+    if name == 'planted':
+        nprs = head_prior_count(HEAD_MAPS)
+        cb = [rng.choice(np.array([-3.0, 0.0, 1.0, 2.5], np.float32), (n, 21)) for n in nprs]
+        for b in cb:
+            b[:, 0] = 2.0
+        cb[1][2, 15] = 4.0
+        return dict(maps=HEAD_MAPS, ncls=21, conf_bias=cb, keep_topk=200)
+    if name == 'iou':
+        return dict(maps=[(1, 60.0, 105.0, (), False)], ncls=2, conf_bias=[[[0.0, 1.0], [0.0, 0.0]]])
+    if name == 'cap':
+        return dict(maps=[CAP_MAP], ncls=33, conf_bias=[rng.choice(np.array([-0.5, 0.0, 0.5], np.float32), (4, 33))], nms_thr=1.0, nms_topk=256,
+                    keep_topk=1024, conf_thr=0.001)
+    if name in ('random', 'random32', 'random40'):
+        ncls = int(name[6:] or 21)
+        cb = [np.concatenate([np.full((n, 1), 4.0), rng.normal(0, 0.5, (n, ncls - 1))], 1) for n in head_prior_count(HEAD_MAPS)]
+        return dict(maps=HEAD_MAPS, ncls=ncls, weights='random', conf_bias=cb, conf_gain=2.0, loc_gain=1.0, conf_thr=0.3, seed=7,
+                    nms_topk=300 if ncls == 21 else 200)
+    raise ValueError(name)
+
+
+def nms_iou(a, b):
+    """float32 IoU of box b against kept box a ([xmin, ymin, xmax, ymax]) in detout_class_kernel's operation order"""
+    a, b = np.asarray(a, np.float32), np.asarray(b, np.float32)
+    inter = np.float32(0)
+    if not (b[0] > a[2] or b[2] < a[0] or b[1] > a[3] or b[3] < a[1]):
+        inter = (min(a[2], b[2]) - max(a[0], b[0])) * (min(a[3], b[3]) - max(a[1], b[1]))
+    area = (b[2] - b[0]) * (b[3] - b[1])
+    return np.float32(inter / ((a[2] - a[0]) * (a[3] - a[1]) + area - inter))
+
+
 def synthetic_rgb(h, w, seed):
     rng = np.random.default_rng(seed)
     img = np.full((h, w, 3), 110, np.float32) + rng.normal(0, 6, (h, w, 3))
