@@ -17,13 +17,16 @@
 #include <cstdio>
 
 #include <cstring>
+#include <memory>
 #include <vector>
 
 #include "host_stage.cuh"
 #include "sgs_common.h"
 
 struct sgs_vocabulary {
-    int device = 0, k = 0, L = 0, nnodes = 0;
+    explicit sgs_vocabulary(int dev) : device(dev), res(dev) {}
+    int device, k = 0, L = 0, nnodes = 0;
+    sgs::HandleResources res;
     int32_t* d_first = nullptr; int32_t* d_count = nullptr; int32_t* d_children = nullptr; int32_t* d_word = nullptr;
     uint8_t* d_desc = nullptr; double* d_weight = nullptr;
 };
@@ -263,12 +266,7 @@ using namespace sgs;
 
 extern "C" {
 
-SGS_API void sgs_vocabulary_destroy(sgs_vocabulary* v) {
-    if (!v) return;
-    cudaSetDevice(v->device);
-    cudaFree(v->d_first); cudaFree(v->d_count); cudaFree(v->d_children); cudaFree(v->d_word); cudaFree(v->d_desc); cudaFree(v->d_weight);
-    delete v;
-}
+SGS_API void sgs_vocabulary_destroy(sgs_vocabulary* v) { delete v; }
 
 static int vocabulary_create_impl(int device, int k, int L, int nnodes, const int32_t* parent, const uint8_t* node_desc, bool desc_on_device,
                                   const double* node_weight, sgs_vocabulary** out) {
@@ -286,22 +284,22 @@ static int vocabulary_create_impl(int device, int k, int L, int nnodes, const in
     int w = 0;
     for (int i = 1; i < nnodes; ++i) if (count[i] == 0) word[i] = w++;
     SGS_CUDA_TRY(cudaSetDevice(device));
-    sgs_vocabulary* v = new sgs_vocabulary();
-    v->device = device; v->k = k; v->L = L; v->nnodes = nnodes;
-    cudaError_t e = cudaMalloc(&v->d_first, 4 * (size_t)nnodes);
-    if (e == cudaSuccess) e = cudaMalloc(&v->d_count, 4 * (size_t)nnodes);
-    if (e == cudaSuccess) e = cudaMalloc(&v->d_children, 4 * (size_t)nnodes);
-    if (e == cudaSuccess) e = cudaMalloc(&v->d_word, 4 * (size_t)nnodes);
-    if (e == cudaSuccess) e = cudaMalloc(&v->d_desc, 32 * (size_t)nnodes);
-    if (e == cudaSuccess) e = cudaMalloc(&v->d_weight, 8 * (size_t)nnodes);
-    if (e == cudaSuccess) e = cudaMemcpy(v->d_first, first.data(), 4 * (size_t)nnodes, cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) e = cudaMemcpy(v->d_count, count.data(), 4 * (size_t)nnodes, cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) e = cudaMemcpy(v->d_children, children.data(), 4 * (size_t)(nnodes - 1), cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) e = cudaMemcpy(v->d_word, word.data(), 4 * (size_t)nnodes, cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) e = cudaMemcpy(v->d_desc, node_desc, 32 * (size_t)nnodes, desc_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) e = cudaMemcpy(v->d_weight, node_weight, 8 * (size_t)nnodes, cudaMemcpyHostToDevice);
-    if (e != cudaSuccess) { set_error("sgs_vocabulary_create: %s", cudaGetErrorString(e)); sgs_vocabulary_destroy(v); return SGS_ERR_CUDA; }
-    *out = v;
+    auto v = std::make_unique<sgs_vocabulary>(device);
+    v->k = k; v->L = L; v->nnodes = nnodes;
+    const char* const fn = "sgs_vocabulary_create";
+    SGS_CUDA_TRY_AT(fn, v->res.alloc(&v->d_first, 4 * (size_t)nnodes));
+    SGS_CUDA_TRY_AT(fn, v->res.alloc(&v->d_count, 4 * (size_t)nnodes));
+    SGS_CUDA_TRY_AT(fn, v->res.alloc(&v->d_children, 4 * (size_t)nnodes));
+    SGS_CUDA_TRY_AT(fn, v->res.alloc(&v->d_word, 4 * (size_t)nnodes));
+    SGS_CUDA_TRY_AT(fn, v->res.alloc(&v->d_desc, 32 * (size_t)nnodes));
+    SGS_CUDA_TRY_AT(fn, v->res.alloc(&v->d_weight, 8 * (size_t)nnodes));
+    SGS_CUDA_TRY_AT(fn, cudaMemcpy(v->d_first, first.data(), 4 * (size_t)nnodes, cudaMemcpyHostToDevice));
+    SGS_CUDA_TRY_AT(fn, cudaMemcpy(v->d_count, count.data(), 4 * (size_t)nnodes, cudaMemcpyHostToDevice));
+    SGS_CUDA_TRY_AT(fn, cudaMemcpy(v->d_children, children.data(), 4 * (size_t)(nnodes - 1), cudaMemcpyHostToDevice));
+    SGS_CUDA_TRY_AT(fn, cudaMemcpy(v->d_word, word.data(), 4 * (size_t)nnodes, cudaMemcpyHostToDevice));
+    SGS_CUDA_TRY_AT(fn, cudaMemcpy(v->d_desc, node_desc, 32 * (size_t)nnodes, desc_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice));
+    SGS_CUDA_TRY_AT(fn, cudaMemcpy(v->d_weight, node_weight, 8 * (size_t)nnodes, cudaMemcpyHostToDevice));
+    *out = v.release();
     return SGS_OK;
 }
 

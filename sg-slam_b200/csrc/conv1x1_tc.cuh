@@ -18,6 +18,8 @@
 #include <cstring>
 #include <vector>
 
+#include "host_stage.cuh"
+
 namespace sgs {
 namespace tc {
 
@@ -348,19 +350,18 @@ inline void plan_tiling(int Cin, int Cout, GemmPlan* P, int force_nt = 0, int m_
     P->smem_bytes = st * stage_bytes + (P->b_resident ? b_all : 0) + 1024;
 }
 
-// Splits and uploads W [Cout][Cin], picks the tiling.  Returns false when TMA is unavailable or an allocation fails.
-inline bool plan_weights(const float* W, int Cin, int Cout, GemmPlan* P, int force_nt = 0, int m_tiles = 0) {
+// Splits and uploads W [Cout][Cin] into buffers owned by `res`, picks the tiling.  Returns false when TMA is unavailable or an allocation fails.
+inline bool plan_weights(HandleResources& res, const float* W, int Cin, int Cout, GemmPlan* P, int force_nt = 0, int m_tiles = 0) {
     plan_tiling(Cin, Cout, P, force_nt, m_tiles);
     std::vector<float> hi((size_t)P->Np * P->Kp, 0.f), lo((size_t)P->Np * P->Kp, 0.f);
     for (int co = 0; co < Cout; ++co)
         for (int c = 0; c < Cin; ++c) split_tf32_host(W[(size_t)co * Cin + c], hi[(size_t)co * P->Kp + c], lo[(size_t)co * P->Kp + c]);
-    if (cudaMalloc((void**)&P->d_whi, hi.size() * 4) != cudaSuccess) return false;
-    if (cudaMalloc((void**)&P->d_wlo, lo.size() * 4) != cudaSuccess) return false;
+    if (res.alloc(&P->d_whi, hi.size() * 4) != cudaSuccess) return false;
+    if (res.alloc(&P->d_wlo, lo.size() * 4) != cudaSuccess) return false;
     if (cudaMemcpy(P->d_whi, hi.data(), hi.size() * 4, cudaMemcpyHostToDevice) != cudaSuccess) return false;
     if (cudaMemcpy(P->d_wlo, lo.data(), lo.size() * 4, cudaMemcpyHostToDevice) != cudaSuccess) return false;
     return encode_kmajor_map(&P->map_hi, P->d_whi, P->Np, P->Kp, P->Kp, P->NT, P->BK) && encode_kmajor_map(&P->map_lo, P->d_wlo, P->Np, P->Kp, P->Kp, P->NT, P->BK);
 }
-inline void free_plan(GemmPlan* P) { cudaFree(P->d_whi); cudaFree(P->d_wlo); P->d_whi = P->d_wlo = nullptr; }
 
 // x / c.  For c == 6 (the hard-swish / hard-sigmoid divisor of the model) the quotient comes from the reciprocal and one FMA correction:
 // q = RN(x * r), q' = RN(q + RN(x - 6q) * r), which equals the correctly rounded RN(x / 6) for every float with |x| >= 2^-100 and for zeros up to the

@@ -23,6 +23,7 @@
 #include <cstring>
 #include <fstream>
 #include <map>
+#include <memory>
 #include <sstream>
 #include <stdexcept>
 
@@ -699,7 +700,9 @@ using namespace sgs;
 using namespace sgs::det;
 
 struct sgs_detector {
-    int device = 0, max_frames = 0, flags = 0;
+    explicit sgs_detector(int dev) : device(dev), res(dev) {}
+    int device, max_frames = 0, flags = 0;
+    HandleResources res;              // nothing in plan-only mode (flags bit 1)
     float det_thr = 0, dyn_thr = 0;
     int T = 300;
     std::vector<Layer> layers;
@@ -710,7 +713,6 @@ struct sgs_detector {
     DetOutParams dp{};
     std::vector<float*> pool;          // activation buffers (max_frames x size)
     std::vector<int64_t> pool_size;
-    std::vector<float*> weights;       // device allocations to free
     float* d_prior = nullptr; float* d_var = nullptr;
     unsigned long long* d_picked = nullptr; int32_t* d_picked_n = nullptr;
     // host-call scratch
@@ -719,7 +721,7 @@ struct sgs_detector {
     sgs_object2d* d_obj = nullptr; int32_t* d_cnt = nullptr;
     int last_frames = 0;
     // optional per-kernel timing (sgs_detector_set_profiling): events around every launch of a call, read back at the next call / by sgs_detector_kernel_times
-    bool profiling = false, pending = false; std::vector<cudaEvent_t> ev; std::vector<double> ms_acc; int prof_calls = 0;
+    StageTimer timer;
 };
 
 namespace {
@@ -838,8 +840,7 @@ bool is_eltwise(const Layer& L) { return L.type == "ReLU" || L.type == "Clip" ||
 int upload(sgs_detector* D, const std::vector<float>& h, float** d) {
     *d = nullptr;
     if (h.empty() || (D->flags & 2)) return SGS_OK;
-    SGS_CUDA_TRY(cudaMalloc((void**)d, h.size() * sizeof(float)));
-    D->weights.push_back(*d);
+    SGS_CUDA_TRY(D->res.alloc(d, h.size() * sizeof(float)));
     SGS_CUDA_TRY(cudaMemcpy(*d, h.data(), h.size() * sizeof(float), cudaMemcpyHostToDevice));
     return SGS_OK;
 }
@@ -1028,7 +1029,7 @@ int build_graph(sgs_detector* D) {
             if (op.kind == OP_CONV1X1) {
                 const int m_tiles = (int)std::min<int64_t>(((int64_t)D->max_frames * op.g.OH * op.g.OW + tc::kBM - 1) / tc::kBM, 1 << 30);      // pixel tiles of a full batch
                 if (D->flags & 2) tc::plan_tiling(op.g.Cin, op.g.Cout, &op.gp, 0, m_tiles);
-                else if (!tc::plan_weights(L.weight.data(), op.g.Cin, op.g.Cout, &op.gp, 0, m_tiles)) { set_error("sgs_detector_create: layer %s: the wgmma GEMM could not be set up (TMA tensor maps need a CUDA 12 driver; %s)", L.name.c_str(), cudaGetErrorString(cudaGetLastError())); return SGS_ERR_CUDA; }
+                else if (!tc::plan_weights(D->res, L.weight.data(), op.g.Cin, op.g.Cout, &op.gp, 0, m_tiles)) { set_error("sgs_detector_create: layer %s: the wgmma GEMM could not be set up (TMA tensor maps need a CUDA 12 driver; %s)", L.name.c_str(), cudaGetErrorString(cudaGetLastError())); return SGS_ERR_CUDA; }
             } else if (op.kind == OP_DWCONV) {                    // [c][ky][kx] -> [ky][kx][c]: channel vectors
                 std::vector<float> wt(L.weight.size());
                 const int kk = op.g.k * op.g.k;
@@ -1125,15 +1126,15 @@ int build_graph(sgs_detector* D) {
     }
     D->pool.assign(D->pool_size.size(), nullptr);
     if (D->flags & 2) return SGS_OK;                     // plan only
-    for (size_t q = 0; q < D->pool_size.size(); ++q) SGS_CUDA_TRY(cudaMalloc((void**)&D->pool[q], (size_t)D->pool_size[q] * D->max_frames * sizeof(float)));
+    for (size_t q = 0; q < D->pool_size.size(); ++q) SGS_CUDA_TRY(D->res.alloc(&D->pool[q], (size_t)D->pool_size[q] * D->max_frames * sizeof(float)));
     for (auto& b : B) { const int r = root_of(*D, (int)(&b - &B[0])); if (B[r].buf >= 0) b.dev = D->pool[B[r].buf]; }
     for (auto& op : D->ops)                                   // the GEMMs' activation operand: [max_frames * H * W][Cin], rows past the batch are never stored
         if (op.kind == OP_CONV1X1 && !tc::encode_kmajor_map(&op.map_in, B[op.in].dev, (int64_t)D->max_frames * op.g.H * op.g.W, op.g.Cin, op.g.Cin, tc::kBM, op.gp.BK)) {
             set_error("sgs_detector_create: layer %s: cuTensorMapEncodeTiled failed", D->layers[op.layer].name.c_str()); return SGS_ERR_CUDA; }
-    SGS_CUDA_TRY(cudaMalloc((void**)&D->d_picked, (size_t)D->max_frames * (D->dp.ncls - 1) * D->dp.nms_topk * sizeof(unsigned long long)));
-    SGS_CUDA_TRY(cudaMalloc((void**)&D->d_picked_n, (size_t)D->max_frames * (D->dp.ncls - 1) * sizeof(int32_t)));
-    SGS_CUDA_TRY(cudaMalloc((void**)&D->d_obj, (size_t)D->dp.keep_topk * sizeof(sgs_object2d)));
-    SGS_CUDA_TRY(cudaMalloc((void**)&D->d_cnt, 4 * sizeof(int32_t)));
+    SGS_CUDA_TRY(D->res.alloc(&D->d_picked, (size_t)D->max_frames * (D->dp.ncls - 1) * D->dp.nms_topk * sizeof(unsigned long long)));
+    SGS_CUDA_TRY(D->res.alloc(&D->d_picked_n, (size_t)D->max_frames * (D->dp.ncls - 1) * sizeof(int32_t)));
+    SGS_CUDA_TRY(D->res.alloc(&D->d_obj, (size_t)D->dp.keep_topk * sizeof(sgs_object2d)));
+    SGS_CUDA_TRY(D->res.alloc(&D->d_cnt, 4 * sizeof(int32_t)));
     return SGS_OK;
 }
 
@@ -1167,13 +1168,13 @@ int sgs_detector_create(const char* param_path, const char* bin_path, int max_fr
     if (!out || !param_path || !bin_path || max_frames < 1) { set_error("sgs_detector_create: bad argument"); return SGS_ERR_INVALID; }
     *out = nullptr;
     if (!(flags & 2)) SGS_CUDA_TRY(cudaSetDevice(device));
-    sgs_detector* D = new sgs_detector();
-    D->device = device; D->max_frames = max_frames; D->flags = flags; D->det_thr = det_thr; D->dyn_thr = dyn_thr;
+    auto D = std::make_unique<sgs_detector>(device);
+    D->max_frames = max_frames; D->flags = flags; D->det_thr = det_thr; D->dyn_thr = dyn_thr;
     int rc = SGS_OK;
     try {                                              // malformed files must come back as a status, never as an exception through the C ABI
         rc = parse_param(param_path, D->layers);
         if (rc == SGS_OK) rc = load_bin(bin_path, D->layers);
-        if (rc == SGS_OK) rc = build_graph(D);
+        if (rc == SGS_OK) rc = build_graph(D.get());
     } catch (const std::exception& ex) {
         set_error("sgs_detector_create: %s while reading %s / %s", ex.what(), param_path, bin_path);
         rc = SGS_ERR_INVALID;
@@ -1184,22 +1185,13 @@ int sgs_detector_create(const char* param_path, const char* bin_path, int max_fr
         if (e == cudaSuccess) e = cudaFuncSetAttribute(conv_small_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024);
         if (e != cudaSuccess) { set_error("sgs_detector_create: cudaFuncSetAttribute -> %s", cudaGetErrorString(e)); rc = SGS_ERR_CUDA; }
     }
-    if (rc != SGS_OK) { sgs_detector_destroy(D); return rc; }
-    *out = D;
+    if (rc != SGS_OK) return rc;
+    D->timer = StageTimer((int)D->ops.size() + 3);
+    *out = D.release();
     return SGS_OK;
 }
 
-void sgs_detector_destroy(sgs_detector* D) {
-    if (!D) return;
-    if (D->flags & 2) { delete D; return; }
-    cudaSetDevice(D->device);
-    for (float* p : D->pool) cudaFree(p);
-    for (float* p : D->weights) cudaFree(p);
-    for (auto& op : D->ops) if (op.kind == OP_CONV1X1) tc::free_plan(&op.gp);
-    cudaFree(D->d_picked); cudaFree(D->d_picked_n); cudaFree(D->d_img); cudaFree(D->d_obj); cudaFree(D->d_cnt); cudaFree(D->d_pre_tab);
-    for (auto& e : D->ev) if (e) cudaEventDestroy(e);
-    delete D;
-}
+void sgs_detector_destroy(sgs_detector* D) { delete D; }
 
 int sgs_detector_info(const sgs_detector* D, int* rows_cap, int* input_size, int* num_layers, int* num_kernels) {
     if (!D) { set_error("sgs_detector_info: NULL handle"); return SGS_ERR_INVALID; }
@@ -1210,22 +1202,10 @@ int sgs_detector_info(const sgs_detector* D, int* rows_cap, int* input_size, int
     return SGS_OK;
 }
 
-static void det_collect_times(sgs_detector* D) {
-    if (!D->pending) return;
-    const size_t nk = D->ops.size() + 3;
-    if (cudaEventSynchronize(D->ev[nk]) == cudaSuccess) {
-        for (size_t i = 0; i < nk; ++i) { float ms = 0; if (cudaEventElapsedTime(&ms, D->ev[i], D->ev[i + 1]) == cudaSuccess) D->ms_acc[i] += ms; }
-        D->prof_calls++;
-    }
-    D->pending = false;
-}
-
 int sgs_detector_set_profiling(sgs_detector* D, int enable) {
     if (!D || (D->flags & 2)) { set_error("sgs_detector_set_profiling: NULL or plan-only handle"); return SGS_ERR_INVALID; }
     SGS_CUDA_TRY(cudaSetDevice(D->device));
-    const size_t nk = D->ops.size() + 3;
-    if (enable && D->ev.empty()) { D->ev.resize(nk + 1); for (auto& e : D->ev) SGS_CUDA_TRY(cudaEventCreate(&e)); }
-    D->profiling = enable != 0; D->pending = false; D->ms_acc.assign(nk, 0.0); D->prof_calls = 0;
+    SGS_CUDA_TRY(D->timer.enable(D->res, enable != 0));
     return SGS_OK;
 }
 
@@ -1233,11 +1213,11 @@ int sgs_detector_kernel_times(sgs_detector* D, double* ms_total, int cap, int* n
     if (!D || !nkernels || !ncalls) { set_error("sgs_detector_kernel_times: NULL"); return SGS_ERR_INVALID; }
     const int nk = (int)D->ops.size() + 3;
     *nkernels = nk; *ncalls = 0;
-    if (!D->profiling) return SGS_OK;
+    if (!D->timer.on()) return SGS_OK;
     SGS_CUDA_TRY(cudaSetDevice(D->device));
-    det_collect_times(D);
-    *ncalls = D->prof_calls;
-    if (ms_total) { if (cap < nk) { set_error("sgs_detector_kernel_times: %d entries needed", nk); return SGS_ERR_CAPACITY; } for (int i = 0; i < nk; ++i) ms_total[i] = D->ms_acc[i]; }
+    D->timer.fold();        // a failed wait leaves the last call out of the totals
+    *ncalls = D->timer.calls();
+    if (ms_total) { if (cap < nk) { set_error("sgs_detector_kernel_times: %d entries needed", nk); return SGS_ERR_CAPACITY; } for (int i = 0; i < nk; ++i) ms_total[i] = D->timer.totals()[i]; }
     return SGS_OK;
 }
 
@@ -1255,19 +1235,18 @@ int sgs_detector_detect_device(sgs_detector* D, const uint8_t* d_rgb, int64_t fr
     cudaStream_t st = (cudaStream_t)stream;
     const int F = nframes, T = D->T;
     auto& B = D->blobs;
-    const bool prof = D->profiling;
-    if (prof) det_collect_times(D);
-    size_t evi = 0;
-#define SGS_DET_MARK() do { if (prof) cudaEventRecord(D->ev[evi++], st); } while (0)
-    if (!D->d_pre_tab) SGS_CUDA_TRY(cudaMalloc((void**)&D->d_pre_tab, (size_t)6 * T * sizeof(int)));
+    StageTimer& timer = D->timer;
+    timer.begin();
+    int stage = 0;
+    if (!D->d_pre_tab) SGS_CUDA_TRY(D->res.alloc(&D->d_pre_tab, (size_t)6 * T * sizeof(int)));
     if (D->pre_w != width || D->pre_h != height) {          // stream-ordered in front of the resize; calls on one handle are serial (they share the activation pool)
         preprocess_table_kernel<<<nblk(T), 256, 0, st>>>(width, height, T, D->d_pre_tab);
         D->pre_w = width; D->pre_h = height;
     }
-    SGS_DET_MARK();
+    timer.mark(stage++, st);
     preprocess_kernel<<<dim3(nblk((int64_t)T * T), F), 256, 0, st>>>(d_rgb, frame_stride, pitch, T, D->d_pre_tab, 123.675f, 116.28f, 103.53f, B[D->input_blob].dev);
     for (const Op& op : D->ops) {
-        SGS_DET_MARK();
+        timer.mark(stage++, st);
         const Blob& bi = B[op.in]; const Blob& bo = B[op.out];
         const Epi epi = make_epi(D, op.epi);
         switch (op.kind) {
@@ -1328,17 +1307,15 @@ int sgs_detector_detect_device(sgs_detector* D, const uint8_t* d_rgb, int64_t fr
         }
     }
     const DetOutParams P = D->dp;
-    SGS_DET_MARK();
+    timer.mark(stage++, st);
     detout_class_kernel<<<dim3(P.ncls - 1, F), 256, kDetSortCap * 8 + P.nms_topk * 20, st>>>(B[D->loc_blob].dev, B[D->conf_blob].dev, D->d_prior, D->d_var, P,
                                                                                                 D->d_picked, D->d_picked_n);
     PostParams Q{D->det_thr, D->dyn_thr, (float)T, width, height, 15, P.keep_topk, max_boxes};
-    SGS_DET_MARK();
+    timer.mark(stage++, st);
     detout_merge_kernel<<<F, 256, kMergeCap * 8 + P.keep_topk * 24, st>>>(B[D->loc_blob].dev, D->d_prior, D->d_var, P, D->d_picked, D->d_picked_n, Q, d_rows,
                                                                           d_nrows, d_objects, d_nobjects, d_dyn_map, d_ndyn_map, d_dyn_rm, d_ndyn_rm,
                                                                           d_have_dyn_rm, d_status);
-    SGS_DET_MARK();
-#undef SGS_DET_MARK
-    if (prof) D->pending = true;
+    timer.end(st);
     SGS_CUDA_TRY(cudaGetLastError());
     D->last_frames = F;
     return SGS_OK;
@@ -1348,7 +1325,7 @@ int sgs_detect(sgs_detector* D, const uint8_t* rgb, int width, int height, int p
     if (!D || !rgb || !n || (cap > 0 && !objects) || width < 2 || height < 2 || pitch < width * 3) { set_error("sgs_detect: bad argument"); return SGS_ERR_INVALID; }
     SGS_CUDA_TRY(cudaSetDevice(D->device));
     const int64_t bytes = (int64_t)pitch * height;
-    if (bytes > D->d_img_cap) { cudaFree(D->d_img); D->d_img = nullptr; D->d_img_cap = 0; SGS_CUDA_TRY(cudaMalloc((void**)&D->d_img, (size_t)bytes)); D->d_img_cap = bytes; }
+    if (bytes > D->d_img_cap) { D->d_img_cap = 0; SGS_CUDA_TRY(D->res.regrow(&D->d_img, (size_t)bytes)); D->d_img_cap = bytes; }
     SGS_CUDA_TRY(cudaMemcpy(D->d_img, rgb, (size_t)bytes, cudaMemcpyHostToDevice));
     int rc = sgs_detector_detect_device(D, D->d_img, bytes, pitch, width, height, 1, nullptr, nullptr, D->d_obj, D->d_cnt, nullptr, nullptr, nullptr, nullptr, nullptr, 0,
                                         nullptr, nullptr);

@@ -7,15 +7,19 @@
 
 #include <cstdlib>
 #include <cstring>
+#include <memory>
 #include <vector>
 
 #include "extract_kernels.h"
+#include "host_stage.cuh"
 
 using namespace sgs;
 
 struct sgs_extractor {
+    explicit sgs_extractor(int dev) : device(dev), res(dev) {}
     OrbPlan plan;
-    int device = 0;
+    int device;
+    HandleResources res;
     int max_batch = 0;
     cudaStream_t stream = nullptr;
     cudaStream_t copy_stream = nullptr;      // host -> device copies of the chunked host path run here, ahead of the kernels
@@ -51,36 +55,13 @@ struct sgs_extractor {
     int last_nframes = 0;
     bool last_level0_external = false;
     // optional per-stage timing (CUDA events on the launching stream): pyramid, FAST, quadtree, blur, describe
-    bool profiling = false;
-    cudaEvent_t ev[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
-    double stage_ms_acc[5] = {0, 0, 0, 0, 0};
-    int stage_calls = 0;
-    bool stage_pending = false;
+    StageTimer timer{5};
     cudaStream_t last_stream = nullptr;
 };
 
 namespace {
 
 int fail_invalid(const char* msg) { set_error("%s", msg); return SGS_ERR_INVALID; }
-
-void free_all(sgs_extractor* ex) {
-    if (!ex) return;
-    cudaSetDevice(ex->device);
-    if (ex->copy_stream) cudaStreamDestroy(ex->copy_stream);
-    for (auto& e : ex->chunk_ev) if (e) cudaEventDestroy(e);
-    if (ex->chunk_done) cudaEventDestroy(ex->chunk_done);
-    cudaFree(ex->d_pyr); cudaFree(ex->d_blur); cudaFree(ex->d_cand); cudaFree(ex->d_cand_count); cudaFree(ex->d_kp_stage);
-    cudaFree(ex->d_kp_stage_n); cudaFree(ex->d_out_kps); cudaFree(ex->d_out_desc); cudaFree(ex->d_out_count); cudaFree(ex->d_error);
-    cudaFree(ex->d_cells); cudaFree(ex->d_tabs); cudaFree(ex->d_key_scratch); cudaFree(ex->d_key_scratch_off);
-    if (ex->h_in) cudaFreeHost(ex->h_in);
-    if (ex->h_kps) cudaFreeHost(ex->h_kps);
-    if (ex->h_desc) cudaFreeHost(ex->h_desc);
-    if (ex->h_count) cudaFreeHost(ex->h_count);
-    if (ex->h_error) cudaFreeHost(ex->h_error);
-    for (auto& e : ex->ev) if (e) cudaEventDestroy(e);
-    if (ex->stream) cudaStreamDestroy(ex->stream);
-    delete ex;
-}
 
 // Enqueue the whole pipeline for frames [frame0, frame0 + nframes) of a batch whose level 0 is (d_l0, pitch, fstride).  A chunk
 // (frame0 > 0 or fewer frames than the batch) works on the same buffers through shifted base pointers; only the TMA tensor maps
@@ -105,20 +86,14 @@ int enqueue(sgs_extractor* ex, const uint8_t* d_l0, int pitch, int64_t fstride, 
         P.out_kps += (int64_t)frame0 * P.out_cap; P.out_desc += (int64_t)frame0 * P.out_cap * 32; P.out_count += frame0;
         if (key_scratch) key_scratch += (int64_t)frame0 * ex->key_scratch_fstride;
     }
-    const bool prof = ex->profiling && allow_prof;
-    if (prof && ex->stage_pending) {  // fold the previous call's events before reusing them
-        if (cudaEventSynchronize(ex->ev[5]) == cudaSuccess) {
-            for (int i = 0; i < 5; ++i) { float ms = 0; cudaEventElapsedTime(&ms, ex->ev[i], ex->ev[i + 1]); ex->stage_ms_acc[i] += ms; }
-            ex->stage_calls++;
-        }
-        ex->stage_pending = false;
-    }
+    StageTimer& T = ex->timer;
+    T.begin(allow_prof);
     SGS_CUDA_TRY(cudaMemsetAsync(P.cand_count, 0, sizeof(int32_t) * (size_t)nframes * L, st));
-    if (prof) cudaEventRecord(ex->ev[0], st);
+    T.mark(0, st);
     for (int l = 1; l < L; ++l) {
         if (resize_tile_supported(P, l)) launch_resize_tile(P, l, st); else launch_resize(P, l, st);
     }
-    if (prof) cudaEventRecord(ex->ev[1], st);
+    T.mark(1, st);
     {   // tiles by TMA when every level could be described by a tensor map (16-byte aligned base / pitch); the same kernel with plain loads otherwise
         bool tma = ex->maps_ok;
         if (tma && !(ex->map0_ok && ex->map0_ptr == d_l0 && ex->map0_pitch == pitch && ex->map0_fstride == fstride && ex->map0_frames >= map_frames)) {
@@ -127,13 +102,13 @@ int enqueue(sgs_extractor* ex, const uint8_t* d_l0, int pitch, int64_t fstride, 
         }
         launch_fast_v2(P, ex->fast_maps, tma && ex->map0_ok, ex->fast_plan, ex->d_cells, (int)ex->plan.cells.size(), frame0, st);
     }
-    if (prof) cudaEventRecord(ex->ev[2], st);
+    T.mark(2, st);
     launch_quadtree(P, ex->smem_key_cap, ex->node_cap, ex->qt_smem, key_scratch, ex->key_scratch_fstride, ex->d_key_scratch_off, st);
-    if (prof) cudaEventRecord(ex->ev[3], st);
+    T.mark(3, st);
     launch_blur_all(P, st);
-    if (prof) cudaEventRecord(ex->ev[4], st);
+    T.mark(4, st);
     launch_describe(P, st);
-    if (prof) { cudaEventRecord(ex->ev[5], st); ex->stage_pending = true; }
+    T.end(st);
     SGS_CUDA_TRY(cudaGetLastError());
     ex->last_nframes = frame0 + nframes;
     ex->last_stream = st;
@@ -160,24 +135,16 @@ SGS_API int sgs_extractor_create(const sgs_orb_params* params, int width, int he
     if (!params || !out) return fail_invalid("sgs_extractor_create: NULL argument");
     if (max_batch < 1 || max_batch > 65535) return fail_invalid("sgs_extractor_create: max_batch outside [1,65535]");
     *out = nullptr;
-    sgs_extractor* ex = new sgs_extractor();
+    auto ex = std::make_unique<sgs_extractor>(device);
     int st = make_plan(*params, width, height, &ex->plan);
-    if (st != SGS_OK) { delete ex; return st; }
-    ex->device = device; ex->max_batch = max_batch;
-#define TRY_OR_FREE(expr)                                                                                         \
-    do {                                                                                                          \
-        cudaError_t _e = (expr);                                                                                  \
-        if (_e != cudaSuccess) {                                                                                  \
-            set_error("%s:%d: %s -> %s", __FILE__, __LINE__, #expr, cudaGetErrorString(_e));                      \
-            free_all(ex);                                                                                         \
-            return SGS_ERR_CUDA;                                                                                  \
-        }                                                                                                         \
-    } while (0)
-    TRY_OR_FREE(cudaSetDevice(device));
-    TRY_OR_FREE(cudaStreamCreateWithFlags(&ex->stream, cudaStreamNonBlocking));
-    TRY_OR_FREE(cudaStreamCreateWithFlags(&ex->copy_stream, cudaStreamNonBlocking));
-    for (auto& e : ex->chunk_ev) TRY_OR_FREE(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-    TRY_OR_FREE(cudaEventCreateWithFlags(&ex->chunk_done, cudaEventDisableTiming));
+    if (st != SGS_OK) return st;
+    ex->max_batch = max_batch;
+    HandleResources& R = ex->res;
+    SGS_CUDA_TRY(cudaSetDevice(device));
+    SGS_CUDA_TRY(R.stream(&ex->stream));
+    SGS_CUDA_TRY(R.stream(&ex->copy_stream));
+    for (auto& e : ex->chunk_ev) SGS_CUDA_TRY(R.event(&e, cudaEventDisableTiming));
+    SGS_CUDA_TRY(R.event(&ex->chunk_done, cudaEventDisableTiming));
     const OrbPlan& PL = ex->plan;
     const int L = PL.nlevels;
     const int64_t B = max_batch;
@@ -185,24 +152,24 @@ SGS_API int sgs_extractor_create(const sgs_orb_params* params, int width, int he
     ex->lvl_off.assign(L, 0);
     int64_t total = 0;
     for (int l = 0; l < L; ++l) { ex->lvl_off[l] = total; total += B * PL.lv[l].frame_stride; }
-    TRY_OR_FREE(cudaMalloc(&ex->d_pyr, (size_t)total + 256));
-    TRY_OR_FREE(cudaMalloc(&ex->d_blur, (size_t)total + 256));
-    TRY_OR_FREE(cudaMalloc(&ex->d_cand, sizeof(uint32_t) * (size_t)(B * PL.cand_per_frame)));
-    TRY_OR_FREE(cudaMalloc(&ex->d_cand_count, sizeof(int32_t) * (size_t)(B * L)));
-    TRY_OR_FREE(cudaMalloc(&ex->d_kp_stage, sizeof(uint32_t) * (size_t)(B * PL.max_kp_per_frame)));
-    TRY_OR_FREE(cudaMalloc(&ex->d_kp_stage_n, sizeof(int32_t) * (size_t)(B * L)));
-    TRY_OR_FREE(cudaMalloc(&ex->d_out_kps, sizeof(sgs_keypoint) * (size_t)(B * PL.max_kp_per_frame)));
-    TRY_OR_FREE(cudaMalloc(&ex->d_out_desc, (size_t)(B * PL.max_kp_per_frame) * 32));
-    TRY_OR_FREE(cudaMalloc(&ex->d_out_count, sizeof(int32_t) * (size_t)B));
-    TRY_OR_FREE(cudaMalloc(&ex->d_error, sizeof(int32_t)));
-    TRY_OR_FREE(cudaMemset(ex->d_error, 0, sizeof(int32_t)));
-    TRY_OR_FREE(cudaMemset(ex->d_out_count, 0, sizeof(int32_t) * (size_t)B));
-    TRY_OR_FREE(cudaMalloc(&ex->d_cells, sizeof(FastCell) * PL.cells.size()));
-    TRY_OR_FREE(cudaMemcpy(ex->d_cells, PL.cells.data(), sizeof(FastCell) * PL.cells.size(), cudaMemcpyHostToDevice));
+    SGS_CUDA_TRY(R.alloc(&ex->d_pyr, (size_t)total + 256));
+    SGS_CUDA_TRY(R.alloc(&ex->d_blur, (size_t)total + 256));
+    SGS_CUDA_TRY(R.alloc(&ex->d_cand, sizeof(uint32_t) * (size_t)(B * PL.cand_per_frame)));
+    SGS_CUDA_TRY(R.alloc(&ex->d_cand_count, sizeof(int32_t) * (size_t)(B * L)));
+    SGS_CUDA_TRY(R.alloc(&ex->d_kp_stage, sizeof(uint32_t) * (size_t)(B * PL.max_kp_per_frame)));
+    SGS_CUDA_TRY(R.alloc(&ex->d_kp_stage_n, sizeof(int32_t) * (size_t)(B * L)));
+    SGS_CUDA_TRY(R.alloc(&ex->d_out_kps, sizeof(sgs_keypoint) * (size_t)(B * PL.max_kp_per_frame)));
+    SGS_CUDA_TRY(R.alloc(&ex->d_out_desc, (size_t)(B * PL.max_kp_per_frame) * 32));
+    SGS_CUDA_TRY(R.alloc(&ex->d_out_count, sizeof(int32_t) * (size_t)B));
+    SGS_CUDA_TRY(R.alloc(&ex->d_error, sizeof(int32_t)));
+    SGS_CUDA_TRY(cudaMemset(ex->d_error, 0, sizeof(int32_t)));
+    SGS_CUDA_TRY(cudaMemset(ex->d_out_count, 0, sizeof(int32_t) * (size_t)B));
+    SGS_CUDA_TRY(R.alloc(&ex->d_cells, sizeof(FastCell) * PL.cells.size()));
+    SGS_CUDA_TRY(cudaMemcpy(ex->d_cells, PL.cells.data(), sizeof(FastCell) * PL.cells.size(), cudaMemcpyHostToDevice));
     // bilinear tables
     size_t ntab = 0;
     for (int l = 1; l < L; ++l) ntab += PL.xtab[l].size() / 4 + PL.ytab[l].size() / 4;
-    TRY_OR_FREE(cudaMalloc(&ex->d_tabs, sizeof(short4) * (ntab + 1)));
+    SGS_CUDA_TRY(R.alloc(&ex->d_tabs, sizeof(short4) * (ntab + 1)));
     {
         std::vector<short4> h(ntab + 1);
         size_t o = 0;
@@ -214,7 +181,7 @@ SGS_API int sgs_extractor_create(const sgs_orb_params* params, int width, int he
                 o += t.size() / 4;
             }
         }
-        TRY_OR_FREE(cudaMemcpy(ex->d_tabs, h.data(), sizeof(short4) * ntab, cudaMemcpyHostToDevice));
+        SGS_CUDA_TRY(cudaMemcpy(ex->d_tabs, h.data(), sizeof(short4) * ntab, cudaMemcpyHostToDevice));
     }
     // quadtree: shared-memory budget and the global fallback for the sort keys
     ex->node_cap = 0;
@@ -224,11 +191,11 @@ SGS_API int sgs_extractor_create(const sgs_orb_params* params, int width, int he
     }
     const size_t node_bytes = (quadtree_node_bytes(ex->node_cap) + 15) & ~(size_t)15;
     const size_t smem_limit = 200 * 1024;
-    if (node_bytes + 1024 * 8 > smem_limit) { set_error("nfeatures too large for the shared-memory quadtree (node arrays need %zu bytes)", node_bytes); free_all(ex); return SGS_ERR_UNSUPPORTED; }
+    if (node_bytes + 1024 * 8 > smem_limit) { set_error("nfeatures too large for the shared-memory quadtree (node arrays need %zu bytes)", node_bytes); return SGS_ERR_UNSUPPORTED; }
     ex->smem_key_cap = 4096;
     while (node_bytes + (size_t)ex->smem_key_cap * 8 > 96 * 1024 && ex->smem_key_cap > 1024) ex->smem_key_cap >>= 1;
     ex->qt_smem = node_bytes + (size_t)ex->smem_key_cap * 8;
-    TRY_OR_FREE(configure_quadtree_smem(ex->qt_smem));
+    SGS_CUDA_TRY(configure_quadtree_smem(ex->qt_smem));
     {
         std::vector<int64_t> off(L);
         int64_t o = 0;
@@ -237,9 +204,9 @@ SGS_API int sgs_extractor_create(const sgs_orb_params* params, int width, int he
             off[l] = o; o += ns;
         }
         ex->key_scratch_fstride = o;
-        TRY_OR_FREE(cudaMalloc(&ex->d_key_scratch, sizeof(uint64_t) * (size_t)(B * o)));
-        TRY_OR_FREE(cudaMalloc(&ex->d_key_scratch_off, sizeof(int64_t) * L));
-        TRY_OR_FREE(cudaMemcpy(ex->d_key_scratch_off, off.data(), sizeof(int64_t) * L, cudaMemcpyHostToDevice));
+        SGS_CUDA_TRY(R.alloc(&ex->d_key_scratch, sizeof(uint64_t) * (size_t)(B * o)));
+        SGS_CUDA_TRY(R.alloc(&ex->d_key_scratch_off, sizeof(int64_t) * L));
+        SGS_CUDA_TRY(cudaMemcpy(ex->d_key_scratch_off, off.data(), sizeof(int64_t) * L, cudaMemcpyHostToDevice));
     }
     // device plan template
     DevPlan& D = ex->dev;
@@ -262,45 +229,36 @@ SGS_API int sgs_extractor_create(const sgs_orb_params* params, int width, int he
     }
     // warp-per-cell FAST: tile geometry, shared-memory opt-in, TMA tensor maps of the own pyramid levels
     ex->fast_plan = make_fast_launch_plan(PL);
-    if (ex->fast_plan.smem_bytes > 200 * 1024) { set_error("sgs_extractor_create: FAST cells of this geometry need %d bytes of shared memory per block", ex->fast_plan.smem_bytes); free_all(ex); return SGS_ERR_UNSUPPORTED; }
-    TRY_OR_FREE(configure_fast_smem(ex->fast_plan.smem_bytes));
+    if (ex->fast_plan.smem_bytes > 200 * 1024) { set_error("sgs_extractor_create: FAST cells of this geometry need %d bytes of shared memory per block", ex->fast_plan.smem_bytes); return SGS_ERR_UNSUPPORTED; }
+    SGS_CUDA_TRY(configure_fast_smem(ex->fast_plan.smem_bytes));
     ex->maps_ok = true;
     for (int l = 1; l < L && ex->maps_ok; ++l)
         ex->maps_ok = encode_level_map(&ex->fast_maps.m[l], D.lv[l].img, D.lv[l].w, D.lv[l].h, D.lv[l].pitch, D.lv[l].fstride, max_batch, ex->fast_plan.tp, ex->fast_plan.th);
     // pinned result staging
-    TRY_OR_FREE(cudaMallocHost(&ex->h_kps, sizeof(sgs_keypoint) * (size_t)(B * PL.max_kp_per_frame)));
-    TRY_OR_FREE(cudaMallocHost(&ex->h_desc, (size_t)(B * PL.max_kp_per_frame) * 32));
-    TRY_OR_FREE(cudaMallocHost(&ex->h_count, sizeof(int32_t) * (size_t)B));
-    TRY_OR_FREE(cudaMallocHost(&ex->h_error, sizeof(int32_t)));
+    SGS_CUDA_TRY(R.host_alloc(&ex->h_kps, sizeof(sgs_keypoint) * (size_t)(B * PL.max_kp_per_frame)));
+    SGS_CUDA_TRY(R.host_alloc(&ex->h_desc, (size_t)(B * PL.max_kp_per_frame) * 32));
+    SGS_CUDA_TRY(R.host_alloc(&ex->h_count, sizeof(int32_t) * (size_t)B));
+    SGS_CUDA_TRY(R.host_alloc(&ex->h_error, sizeof(int32_t)));
     ex->h_in_bytes = (size_t)(B * PL.lv[0].frame_stride);
-    TRY_OR_FREE(cudaMallocHost(&ex->h_in, ex->h_in_bytes));
-#undef TRY_OR_FREE
-    *out = ex;
+    SGS_CUDA_TRY(R.host_alloc(&ex->h_in, ex->h_in_bytes));
+    *out = ex.release();
     return SGS_OK;
 }
 
-SGS_API void sgs_extractor_destroy(sgs_extractor* ex) { free_all(ex); }
+SGS_API void sgs_extractor_destroy(sgs_extractor* ex) { delete ex; }
 
 SGS_API int sgs_extractor_set_profiling(sgs_extractor* ex, int enable) {
     if (!ex) return fail_invalid("sgs_extractor_set_profiling: NULL handle");
     SGS_CUDA_TRY(cudaSetDevice(ex->device));
-    if (enable && !ex->ev[0]) for (auto& e : ex->ev) SGS_CUDA_TRY(cudaEventCreate(&e));
-    ex->profiling = enable != 0;
-    ex->stage_pending = false; ex->stage_calls = 0;
-    for (double& v : ex->stage_ms_acc) v = 0;
+    SGS_CUDA_TRY(ex->timer.enable(ex->res, enable != 0));
     return SGS_OK;
 }
 
 SGS_API int sgs_extractor_stage_times(sgs_extractor* ex, double* ms_total5, int* ncalls) {
     if (!ex || !ms_total5 || !ncalls) return fail_invalid("sgs_extractor_stage_times: NULL");
-    if (ex->stage_pending) {
-        SGS_CUDA_TRY(cudaEventSynchronize(ex->ev[5]));
-        for (int i = 0; i < 5; ++i) { float ms = 0; SGS_CUDA_TRY(cudaEventElapsedTime(&ms, ex->ev[i], ex->ev[i + 1])); ex->stage_ms_acc[i] += ms; }
-        ex->stage_calls++;
-        ex->stage_pending = false;
-    }
-    for (int i = 0; i < 5; ++i) ms_total5[i] = ex->stage_ms_acc[i];
-    *ncalls = ex->stage_calls;
+    SGS_CUDA_TRY(ex->timer.fold());
+    for (int i = 0; i < 5; ++i) ms_total5[i] = ex->timer.totals()[i];
+    *ncalls = ex->timer.calls();
     return SGS_OK;
 }
 

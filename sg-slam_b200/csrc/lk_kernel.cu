@@ -14,8 +14,10 @@
 #include <cuda_runtime.h>
 
 #include <cstdint>
+#include <memory>
 #include <vector>
 
+#include "host_stage.cuh"
 #include "sgs_common.h"
 
 namespace sgs {
@@ -321,18 +323,20 @@ __global__ void __launch_bounds__(kLkWarps * 32) lk_track_kernel(const __grid_co
 using namespace sgs;
 
 struct sgs_lk {
-    int device = 0, w = 0, h = 0, max_batch = 0, max_level = 0;
+    explicit sgs_lk(int dev) : device(dev), res(dev) {}
+    int device, w = 0, h = 0, max_batch = 0, max_level = 0;
     int lw[kLkMaxLevel + 1], lh[kLkMaxLevel + 1], lp[kLkMaxLevel + 1];      // level sizes; lp = padded pitch in pixels
     int64_t lfs[kLkMaxLevel + 1], loff[kLkMaxLevel + 1];                    // pixels per padded frame; offset of the level inside a pyramid buffer
     int64_t lorg[kLkMaxLevel + 1];                                          // offset of pixel (0, 0) inside a padded frame
     int64_t pyr_elems = 0;
+    HandleResources res;
     uint8_t* d_pyrI = nullptr; uint8_t* d_pyrJ = nullptr;     // padded levels 0..max_level, each [max_batch][h + 2 pad][pitch]
     uint32_t* d_der = nullptr;                                // derivative planes of I, same geometry (borders stay zero)
     // staging for the single-pair host API
     uint8_t* d_img = nullptr; float* d_pts = nullptr; float* d_out = nullptr; int pts_cap = 0;
     cudaStream_t st = nullptr;
     // optional stage timing (pyramid build, tracker), same contract as sgs_extractor_set_profiling
-    bool profiling = false, pending = false; cudaEvent_t ev[3] = {nullptr, nullptr, nullptr}; double ms_acc[2] = {0, 0}; int calls = 0;
+    StageTimer timer{2};
 };
 
 namespace {
@@ -380,15 +384,8 @@ void build_pyramid(sgs_lk* k, const uint8_t* d_l0, int pitch0, int64_t fstride0,
 
 int run_lk(sgs_lk* k, const uint8_t* d_cur, const uint8_t* d_prev, const int32_t* d_prev_index, int nframes, size_t frame_stride, int pitch,
            const sgs_keypoint* d_kps, const float* d_pts, const int32_t* d_counts, int cap, float* d_out, cudaStream_t st) {
-    const bool prof = k->profiling;
-    if (prof && k->pending) {
-        if (cudaEventSynchronize(k->ev[2]) == cudaSuccess) {
-            for (int i = 0; i < 2; ++i) { float ms = 0; cudaEventElapsedTime(&ms, k->ev[i], k->ev[i + 1]); k->ms_acc[i] += ms; }
-            k->calls++;
-        }
-        k->pending = false;
-    }
-    if (prof) cudaEventRecord(k->ev[0], st);
+    k->timer.begin();
+    k->timer.mark(0, st);
     build_pyramid(k, d_cur, pitch, (int64_t)frame_stride, k->d_pyrI, k->d_der, nframes, st);
     const bool same_batch = d_prev_index != nullptr;     // previous images are other frames of the same batch: one pyramid serves both roles
     if (!same_batch) build_pyramid(k, d_prev, pitch, (int64_t)frame_stride, k->d_pyrJ, nullptr, nframes, st);
@@ -401,10 +398,10 @@ int run_lk(sgs_lk* k, const uint8_t* d_cur, const uint8_t* d_prev, const int32_t
             L.I[l] = k->d_pyrI + o; L.J[l] = (same_batch ? k->d_pyrI : k->d_pyrJ) + o; L.D[l] = k->d_der + o;
         } else { L.I[l] = L.J[l] = nullptr; L.D[l] = nullptr; L.w[l] = L.h[l] = L.pitch[l] = 0; L.fstride[l] = 0; }
     }
-    if (prof) cudaEventRecord(k->ev[1], st);
+    k->timer.mark(1, st);
     dim3 grid((cap + kLkWarps - 1) / kLkWarps, nframes);
     lk_track_kernel<<<grid, kLkWarps * 32, 0, st>>>(L, d_kps, reinterpret_cast<const float2*>(d_pts), d_counts, cap, d_prev_index, reinterpret_cast<float2*>(d_out));
-    if (prof) { cudaEventRecord(k->ev[2], st); k->pending = true; }
+    k->timer.end(st);
     SGS_CUDA_TRY(cudaGetLastError());
     return SGS_OK;
 }
@@ -415,36 +412,25 @@ extern "C" {
 SGS_API int sgs_lk_set_profiling(sgs_lk* k, int enable) {
     if (!k) return lk_bad("sgs_lk_set_profiling: NULL");
     SGS_CUDA_TRY(cudaSetDevice(k->device));
-    if (enable && !k->ev[0]) for (auto& e : k->ev) SGS_CUDA_TRY(cudaEventCreate(&e));
-    k->profiling = enable != 0; k->pending = false; k->ms_acc[0] = k->ms_acc[1] = 0; k->calls = 0;
+    SGS_CUDA_TRY(k->timer.enable(k->res, enable != 0));
     return SGS_OK;
 }
 
 SGS_API int sgs_lk_stage_times(sgs_lk* k, double* ms_total2, int* ncalls) {
     if (!k || !ms_total2 || !ncalls) return lk_bad("sgs_lk_stage_times: NULL");
-    if (k->pending && cudaEventSynchronize(k->ev[2]) == cudaSuccess) {
-        for (int i = 0; i < 2; ++i) { float ms = 0; cudaEventElapsedTime(&ms, k->ev[i], k->ev[i + 1]); k->ms_acc[i] += ms; }
-        k->calls++; k->pending = false;
-    }
-    ms_total2[0] = k->ms_acc[0]; ms_total2[1] = k->ms_acc[1]; *ncalls = k->calls;
+    k->timer.fold();        // a failed wait leaves the last call out of the totals
+    ms_total2[0] = k->timer.totals()[0]; ms_total2[1] = k->timer.totals()[1]; *ncalls = k->timer.calls();
     return SGS_OK;
 }
 
-SGS_API void sgs_lk_destroy(sgs_lk* k) {
-    if (!k) return;
-    cudaSetDevice(k->device);
-    for (auto& e : k->ev) if (e) cudaEventDestroy(e);
-    cudaFree(k->d_pyrI); cudaFree(k->d_pyrJ); cudaFree(k->d_der); cudaFree(k->d_img); cudaFree(k->d_pts); cudaFree(k->d_out);
-    if (k->st) cudaStreamDestroy(k->st);
-    delete k;
-}
+SGS_API void sgs_lk_destroy(sgs_lk* k) { delete k; }
 
 SGS_API int sgs_lk_create(int width, int height, int max_batch, int device, sgs_lk** out) {
     if (!out || width < 24 || height < 24 || max_batch < 1) return lk_bad("sgs_lk_create: bad argument");
     *out = nullptr;
     SGS_CUDA_TRY(cudaSetDevice(device));
-    sgs_lk* k = new sgs_lk();
-    k->device = device; k->w = width; k->h = height; k->max_batch = max_batch;
+    auto k = std::make_unique<sgs_lk>(device);
+    k->w = width; k->h = height; k->max_batch = max_batch;
     int64_t off = 0;
     k->max_level = 0;
     for (int l = 0; l <= kLkMaxLevel; ++l) {     // buildOpticalFlowPyramid stops when a level would not be larger than the window
@@ -461,13 +447,12 @@ SGS_API int sgs_lk_create(int width, int height, int max_batch, int device, sgs_
         off += k->lfs[l] * max_batch;
     }
     k->pyr_elems = off;
-    cudaError_t e = cudaStreamCreateWithFlags(&k->st, cudaStreamNonBlocking);
-    if (e == cudaSuccess) e = cudaMalloc(&k->d_pyrI, (size_t)off + 256);
-    if (e == cudaSuccess) e = cudaMalloc(&k->d_pyrJ, (size_t)off + 256);
-    if (e == cudaSuccess) e = cudaMalloc(&k->d_der, 4 * (size_t)off + 256);
-    if (e == cudaSuccess) e = cudaMemset(k->d_der, 0, 4 * (size_t)off + 256);        // the borders of the derivative planes are never written again
-    if (e != cudaSuccess) { set_error("sgs_lk_create: %s", cudaGetErrorString(e)); sgs_lk_destroy(k); return SGS_ERR_CUDA; }
-    *out = k;
+    SGS_CUDA_TRY_AT("sgs_lk_create", k->res.stream(&k->st));
+    SGS_CUDA_TRY_AT("sgs_lk_create", k->res.alloc(&k->d_pyrI, (size_t)off + 256));
+    SGS_CUDA_TRY_AT("sgs_lk_create", k->res.alloc(&k->d_pyrJ, (size_t)off + 256));
+    SGS_CUDA_TRY_AT("sgs_lk_create", k->res.alloc(&k->d_der, 4 * (size_t)off + 256));
+    SGS_CUDA_TRY_AT("sgs_lk_create", cudaMemset(k->d_der, 0, 4 * (size_t)off + 256));        // the borders of the derivative planes are never written again
+    *out = k.release();
     return SGS_OK;
 }
 
@@ -485,10 +470,11 @@ SGS_API int sgs_lk_track(sgs_lk* k, const uint8_t* cur, const uint8_t* prev, int
     if (n == 0) return SGS_OK;
     SGS_CUDA_TRY(cudaSetDevice(k->device));
     const int dp = (k->w + 15) & ~15;
-    if (!k->d_img) SGS_CUDA_TRY(cudaMalloc(&k->d_img, (size_t)2 * dp * k->h));
+    if (!k->d_img) SGS_CUDA_TRY(k->res.alloc(&k->d_img, (size_t)2 * dp * k->h));
     if (n > k->pts_cap) {
-        cudaFree(k->d_pts); cudaFree(k->d_out); k->d_pts = k->d_out = nullptr;
-        SGS_CUDA_TRY(cudaMalloc(&k->d_pts, 8 * (size_t)n)); SGS_CUDA_TRY(cudaMalloc(&k->d_out, 8 * (size_t)n));
+        k->pts_cap = 0;
+        SGS_CUDA_TRY(k->res.regrow(&k->d_pts, 8 * (size_t)n));
+        SGS_CUDA_TRY(k->res.regrow(&k->d_out, 8 * (size_t)n));
         k->pts_cap = n;
     }
     SGS_CUDA_TRY(cudaMemcpy2DAsync(k->d_img, dp, cur, pitch, k->w, k->h, cudaMemcpyHostToDevice, k->st));

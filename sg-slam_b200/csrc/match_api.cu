@@ -3,6 +3,7 @@
 #include <cuda_runtime.h>
 
 #include <cstring>
+#include <memory>
 #include <vector>
 
 #include "host_stage.cuh"
@@ -11,7 +12,9 @@
 using namespace sgs;
 
 struct sgs_matcher {
-    int device = 0, max_frames = 0, cur_cap = 0, point_cap = 0;
+    explicit sgs_matcher(int dev) : device(dev), res(dev) {}
+    int device, max_frames = 0, cur_cap = 0, point_cap = 0;
+    HandleResources res;
     PointPre* d_pre = nullptr;
     LocalPre* d_lpre = nullptr;
     int32_t* d_events = nullptr;
@@ -52,25 +55,17 @@ SGS_API int sgs_matcher_create(int device, int max_frames, int cur_cap, int poin
     if (cur_cap > 8192) { set_error("sgs_matcher_create: cur_cap %d exceeds the 8192 keypoints per frame the shared-memory grid supports", cur_cap); return SGS_ERR_UNSUPPORTED; }
     *out = nullptr;
     SGS_CUDA_TRY(cudaSetDevice(device));
-    sgs_matcher* m = new sgs_matcher();
-    m->device = device; m->max_frames = max_frames; m->cur_cap = cur_cap; m->point_cap = point_cap;
+    auto m = std::make_unique<sgs_matcher>(device);
+    m->max_frames = max_frames; m->cur_cap = cur_cap; m->point_cap = point_cap;
     const size_t np = (size_t)max_frames * point_cap;
-    if (cudaMalloc(&m->d_pre, np * sizeof(PointPre)) != cudaSuccess || cudaMalloc(&m->d_lpre, np * sizeof(LocalPre)) != cudaSuccess ||
-        cudaMalloc(&m->d_events, np * sizeof(int32_t)) != cudaSuccess) {
-        set_error("sgs_matcher_create: cudaMalloc failed: %s", cudaGetErrorString(cudaGetLastError()));
-        cudaFree(m->d_pre); cudaFree(m->d_lpre); cudaFree(m->d_events); delete m;
-        return SGS_ERR_CUDA;
-    }
-    *out = m;
+    SGS_CUDA_TRY_AT("sgs_matcher_create", m->res.alloc(&m->d_pre, np * sizeof(PointPre)));
+    SGS_CUDA_TRY_AT("sgs_matcher_create", m->res.alloc(&m->d_lpre, np * sizeof(LocalPre)));
+    SGS_CUDA_TRY_AT("sgs_matcher_create", m->res.alloc(&m->d_events, np * sizeof(int32_t)));
+    *out = m.release();
     return SGS_OK;
 }
 
-SGS_API void sgs_matcher_destroy(sgs_matcher* m) {
-    if (!m) return;
-    cudaSetDevice(m->device);
-    cudaFree(m->d_pre); cudaFree(m->d_lpre); cudaFree(m->d_events);
-    delete m;
-}
+SGS_API void sgs_matcher_destroy(sgs_matcher* m) { delete m; }
 
 SGS_API int sgs_match_project_lastframe_batch_device(sgs_matcher* m, const sgs_lastframe_batch* a, int nframes, void* stream) {
     if (!m || !a) { set_error("sgs_match_project_lastframe_batch_device: NULL"); return SGS_ERR_INVALID; }

@@ -37,6 +37,24 @@ def test_lk_against_golden(golden_dir):
         lk.close()
 
 
+def test_lk_point_buffers_regrow(golden_dir):
+    """sgs_lk_track on one handle with a small, a larger and again a small point count (the point buffers grow once): every result is what a
+    fresh handle returns."""
+    g = np.load(os.path.join(golden_dir, 'lk_320x240.npz'))
+    pts = g['pts']
+    lk = B.LK(320, 240)
+    try:
+        for sel in (pts[:40], pts, pts[-90:]):
+            fresh = B.LK(320, 240)
+            try:
+                want = fresh.track(g['cur'], g['prev'], sel)
+            finally:
+                fresh.close()
+            assert np.array_equal(lk.track(g['cur'], g['prev'], sel), want), len(sel)
+    finally:
+        lk.close()
+
+
 def test_lk_against_oracle_on_stream():
     frames, _ = synth.stream_s2(3, 640, 480, seed=2)
     lk = B.LK(640, 480)

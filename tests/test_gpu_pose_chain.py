@@ -101,9 +101,10 @@ def test_pose_chain_against_the_oracle_functions():
     ti['Tc'] = Tc
     o = dict(kps=np.zeros((nb, cap), B.KP_DTYPE), desc=np.zeros((nb, cap, 32), np.uint8), ur=np.zeros((nb, cap), np.float32), cnt=np.zeros(nb, np.int32),
              mp=np.zeros((nb, cap), np.int32), nm=np.zeros(nb, np.int32))
-    B.check(L.sgs_tracker_track_lk(trk.h, nb, P(ti['pidx']), P(ti['ur']), v(0), P(ti['boxes']), P(ti['nb']), P(ti['have']), P(ti['lxyz']), P(ti['ldesc']), P(ti['lflags']),
-                                   P(ti['loct']), P(ti['lang']), P(ti['ln']), P(Tc), P(ti['T']), C.c_float(TH), 0, 1, P(o['kps']), P(o['desc']), P(o['ur']), P(o['cnt']),
-                                   P(o['mp']), P(o['nm'])))
+    track_lk = lambda: B.check(L.sgs_tracker_track_lk(trk.h, nb, P(ti['pidx']), P(ti['ur']), v(0), P(ti['boxes']), P(ti['nb']), P(ti['have']), P(ti['lxyz']), P(ti['ldesc']),
+                                                      P(ti['lflags']), P(ti['loct']), P(ti['lang']), P(ti['ln']), P(Tc), P(ti['T']), C.c_float(TH), 0, 1, P(o['kps']),
+                                                      P(o['desc']), P(o['ur']), P(o['cnt']), P(o['mp']), P(o['nm'])))
+    track_lk()
     rng = np.random.default_rng(5)
     lms = [bench.make_local_map(f, o['kps'][f], o['desc'][f], int(o['cnt'][f]), ti, mcap, camd, sf, rng, W, H) for f in range(nb)]
     stack = lambda k, dt: np.ascontiguousarray(np.stack([m[k] for m in lms]).astype(dt))
@@ -122,6 +123,14 @@ def test_pose_chain_against_the_oracle_functions():
     a.th_local, a.nnratio_local = 3.0, 0.8
     for l in range(16): a.inv_level_sigma2[l] = float(isig[l])
     a.tcw_motion, a.tcw_final, a.f_mp, a.outlier, a.stats = outd['T1'].data_ptr(), outd['T2'].data_ptr(), outd['mp'].data_ptr(), outd['outl'].data_ptr(), outd['st'].data_ptr()
+    # a first chain with a smaller local-map capacity (it reads the first mp_cap rows of the local map): the checked call below runs on the scratch
+    # regrown for mcap and a recreated local-map matcher, after track_lk has restored the matches the first chain changed
+    a.mp_cap = 256
+    B.check(L.sgs_tracker_pose_chain_device(trk.h, C.byref(a), nb, v(0)))
+    first = {k: x.copy() for k, x in o.items()}
+    track_lk()
+    assert all(np.array_equal(o[k], first[k]) for k in o)
+    a.mp_cap = mcap
     B.check(L.sgs_tracker_pose_chain_device(trk.h, C.byref(a), nb, v(0)))
     torch.cuda.synchronize()
     g = {k: t.cpu().numpy() for k, t in outd.items()}
