@@ -1,9 +1,13 @@
 """ctypes binding of libsgs_cuda.so (include/sgs_abi.h) for the Python-side harness (tests, bench).
 
+lib() types every sgs_* function from the prototypes in sgs_abi.h, so ctypes converts the arguments (a Python float becomes a C float,
+an int a size_t or int64_t) and rejects one of the wrong type before the call.
+
 There is NO CPU fallback: loading fails loudly when the library has not been built, and every call fails with
 SGS_ERR_CUDA on a machine without a CUDA device."""
 import ctypes as C
 import os
+import re
 import subprocess
 
 import numpy as np
@@ -112,28 +116,39 @@ class LocalMapBatch(C.Structure):
                 ('f_mp', C.c_void_p), ('f_mp_obs', C.c_void_p), ('nmatches', C.c_void_p), ('ncand', C.c_void_p)]
 
 
-ABI_SYMBOLS = [
-    'sgs_tracker_pose_chain_device', 'sgs_detector_set_profiling', 'sgs_detector_kernel_times',
-    'sgs_abi_version', 'sgs_last_error', 'sgs_device_count', 'sgs_settings_load',
-    'sgs_extractor_create', 'sgs_extractor_destroy', 'sgs_extractor_tables', 'sgs_extractor_max_keypoints', 'sgs_extractor_level_info',
-    'sgs_extract', 'sgs_extract_batch', 'sgs_extract_batch_device', 'sgs_extractor_results_device', 'sgs_extractor_fetch', 'sgs_extractor_read_level',
-    'sgs_extractor_read_candidates',
-    'sgs_hamming_pairs', 'sgs_hamming_bf', 'sgs_hamming_bf_scratch_elems', 'sgs_hamming_bf_device',
-    'sgs_match_project_lastframe', 'sgs_match_project_localmap', 'sgs_matcher_create', 'sgs_matcher_destroy',
-    'sgs_match_project_lastframe_batch_device', 'sgs_match_project_localmap_batch_device',
-    'sgs_dynreject', 'sgs_dynreject_batch_device',
-    'sgs_tracker_create', 'sgs_tracker_destroy', 'sgs_tracker_max_keypoints', 'sgs_tracker_extract', 'sgs_tracker_track',
-    'sgs_tracker_extract_device', 'sgs_tracker_track_device', 'sgs_tracker_results_device', 'sgs_tracker_extractor',
-    'sgs_extractor_set_profiling', 'sgs_extractor_stage_times',
-    'sgs_lk_create', 'sgs_lk_destroy', 'sgs_lk_track', 'sgs_lk_track_batch_device', 'sgs_lk_read_level', 'sgs_lk_read_padded',
-    'sgs_tracker_lk_device', 'sgs_tracker_prev_xy_device', 'sgs_tracker_track_lk', 'sgs_extractor_level0_device', 'sgs_memcpy_d2h',
-    'sgs_lk_set_profiling', 'sgs_lk_stage_times', 'sgs_tracker_lk',
-    'sgs_pose_optimization_batch_device', 'sgs_pose_optimization', 'sgs_distinctive_descriptor_batch_device', 'sgs_fuse_search_batch_device', 'sgs_fuse_search', 'sgs_match_project_keyframe_batch_device', 'sgs_match_project_keyframe',
-    'sgs_tracker_detect_device', 'sgs_tracker_boxes_device', 'sgs_tracker_step', 'sgs_extractor_stream', 'sgs_vocabulary_create', 'sgs_vocabulary_create_device', 'sgs_vocabulary_destroy', 'sgs_vocabulary_parse_file', 'sgs_vocabulary_load', 'sgs_bow_transform_batch_device', 'sgs_match_bow_batch_device', 'sgs_bow_transform', 'sgs_match_bow', 'sgs_match_bow_keyframes', 'sgs_search_for_initialization_batch_device', 'sgs_search_for_initialization',
-    'sgs_stereo_from_depth_batch_device', 'sgs_frustum_batch_device', 'sgs_frustum', 'sgs_undistort_batch_device', 'sgs_undistort_points', 'sgs_image_bounds', 'sgs_tracker_stereo_device',
-    'sgs_fundamental_ransac', 'sgs_fundamental_batch_device', 'sgs_tracker_fundamental_device', 'sgs_tracker_fundamental_device_ptr',
-    'sgs_detector_create', 'sgs_detector_destroy', 'sgs_detector_info', 'sgs_detector_detect_device', 'sgs_detect', 'sgs_detector_describe', 'sgs_detector_blob',
-]
+_HEADER = os.path.join(os.path.dirname(_PKG), 'include', 'sgs_abi.h')
+_BY_VALUE = {'int': C.c_int32, 'int32_t': C.c_int32, 'int64_t': C.c_int64, 'size_t': C.c_size_t, 'float': C.c_float, 'double': C.c_double}
+_RETURNS = {'int': C.c_int, 'void': None}
+
+
+def _ctype(decl, fn, by_value):
+    """ctypes type of the C type `decl` in a prototype of `fn`: `const char*` is a byte string, every other pointer c_void_p, anything
+    else must be in `by_value` (never guessed)."""
+    t = ' '.join(decl.replace('*', ' * ').split()).replace(' *', '*')
+    if t == 'const char*':
+        return C.c_char_p
+    if t.endswith('*'):
+        return C.c_void_p
+    t = t.removeprefix('const ')
+    if t not in by_value:
+        raise TypeError('%s: no ctypes mapping for the C type %r' % (fn, t))
+    return by_value[t]
+
+
+def parse_abi(text):
+    """{name: (restype, argtypes)} of every SGS_API prototype in `text` (sgs_abi.h)."""
+    text = re.sub(r'^[ \t]*#.*$', '', re.sub(r'/\*.*?\*/|//[^\n]*', ' ', text, flags=re.S), flags=re.M)
+    protos = re.findall(r'SGS_API\s+([\w\s*]+?)\b(sgs_\w+)\s*\(([^)]*)\)\s*;', text)
+    if len(protos) != text.count('SGS_API'):
+        raise ValueError('sgs_abi.h: %d SGS_API declarations but %d prototypes parsed' % (text.count('SGS_API'), len(protos)))
+    return {name: (_ctype(ret, name, _RETURNS),
+                   [] if params.strip() == 'void' else [_ctype(re.sub(r'\w+\s*$', '', p), name, _BY_VALUE) for p in params.split(',')])
+            for ret, name, params in protos}
+
+
+with open(_HEADER) as f:
+    _SIGNATURES = parse_abi(f.read())
+ABI_SYMBOLS = sorted(_SIGNATURES)
 
 
 def build(force=False):
@@ -148,8 +163,11 @@ def lib():
     if _LIB is None:
         if not os.path.exists(LIB_PATH):
             raise RuntimeError('libsgs_cuda.so is not built (run __graft_entry__.build() or make -C sg-slam_b200/csrc); there is no CPU fallback')
-        _LIB = C.CDLL(LIB_PATH)
-        _LIB.sgs_last_error.restype = C.c_char_p
+        so = C.CDLL(LIB_PATH)
+        for name, (restype, argtypes) in _SIGNATURES.items():
+            fn = getattr(so, name)
+            fn.restype, fn.argtypes = restype, argtypes
+        _LIB = so
     return _LIB
 
 
@@ -162,27 +180,36 @@ def _p(a):
     return a.ctypes.data_as(C.c_void_p) if a is not None else None
 
 
+def _sized(fn, head, dtype, n_type=C.c_int, tail=()):
+    """The size-query protocol of the read-out accessors: fn(*head, NULL, 0, &n, *tail) reports the element count n (SGS_ERR_CAPACITY is that
+    answer, not a failure), then fn(*head, out, n, &n, *tail) fills out = zeros(n, dtype)."""
+    n = n_type()
+    rc = fn(*head, None, 0, C.byref(n), *tail)
+    if rc != SGS_ERR_CAPACITY:
+        check(rc)
+    out = np.zeros(n.value, dtype)
+    if n.value:
+        check(fn(*head, _p(out), n.value, C.byref(n), *tail))
+    return out
+
+
 def device_count():
     n = C.c_int()
     check(lib().sgs_device_count(C.byref(n)))
     return n.value
 
 
-class Extractor:
-    """ORB_SLAM2::ORBextractor on the GPU (sgs_extractor_* of include/sgs_abi.h)."""
+class _Handle:
+    """One sgs_* handle `h`: made by create(*args, &h), released once by destroy(h) on close() or garbage collection."""
 
-    def __init__(self, width, height, nfeatures=1000, scale=1.2, nlevels=8, ini=20, mn=7, max_batch=1, device=0):
-        self.params = OrbParams(nfeatures, scale, nlevels, ini, mn)
-        self.width, self.height, self.max_batch, self.device = width, height, max_batch, device
+    def __init__(self, create, destroy, *args):
         self.h = C.c_void_p()
-        check(lib().sgs_extractor_create(C.byref(self.params), width, height, max_batch, device, C.byref(self.h)))
-        cap = C.c_int()
-        check(lib().sgs_extractor_max_keypoints(self.h, C.byref(cap)))
-        self.cap = cap.value
+        self._destroy = destroy
+        check(create(*args, C.byref(self.h)))
 
     def close(self):
         if self.h:
-            lib().sgs_extractor_destroy(self.h)
+            self._destroy(self.h)
             self.h = C.c_void_p()
 
     def __del__(self):
@@ -190,6 +217,18 @@ class Extractor:
             self.close()
         except Exception:
             pass
+
+
+class Extractor(_Handle):
+    """ORB_SLAM2::ORBextractor on the GPU (sgs_extractor_* of include/sgs_abi.h)."""
+
+    def __init__(self, width, height, nfeatures=1000, scale=1.2, nlevels=8, ini=20, mn=7, max_batch=1, device=0):
+        self.params = OrbParams(nfeatures, scale, nlevels, ini, mn)
+        self.width, self.height, self.max_batch, self.device = width, height, max_batch, device
+        super().__init__(lib().sgs_extractor_create, lib().sgs_extractor_destroy, C.byref(self.params), width, height, max_batch, device)
+        cap = C.c_int()
+        check(lib().sgs_extractor_max_keypoints(self.h, C.byref(cap)))
+        self.cap = cap.value
 
     def tables(self):
         n = self.params.nlevels
@@ -219,15 +258,15 @@ class Extractor:
         kps = out_kps if out_kps is not None else np.zeros((F, self.cap), KP_DTYPE)
         desc = out_desc if out_desc is not None else np.zeros((F, self.cap, 32), np.uint8)
         n = out_n if out_n is not None else np.zeros(F, np.int32)
-        check(lib().sgs_extract_batch(self.h, _p(imgs), F, C.c_size_t(imgs.strides[0]), imgs.strides[1], _p(kps), _p(desc), self.cap, _p(n)))
+        check(lib().sgs_extract_batch(self.h, _p(imgs), F, imgs.strides[0], imgs.strides[1], _p(kps), _p(desc), self.cap, _p(n)))
         return kps, desc, n
 
     def extract_batch_device(self, d_ptr, nframes, frame_stride, pitch, stream=0):
-        check(lib().sgs_extract_batch_device(self.h, C.c_void_p(d_ptr), nframes, C.c_size_t(frame_stride), pitch, C.c_void_p(stream)))
+        check(lib().sgs_extract_batch_device(self.h, d_ptr, nframes, frame_stride, pitch, stream))
 
     def fetch(self, nframes, stream=0):
         kps = np.zeros((nframes, self.cap), KP_DTYPE); desc = np.zeros((nframes, self.cap, 32), np.uint8); n = np.zeros(nframes, np.int32)
-        check(lib().sgs_extractor_fetch(self.h, nframes, _p(kps), _p(desc), self.cap, _p(n), C.c_void_p(stream)))
+        check(lib().sgs_extractor_fetch(self.h, nframes, _p(kps), _p(desc), self.cap, _p(n), stream))
         return kps, desc, n
 
     def set_profiling(self, on=True):
@@ -251,14 +290,7 @@ class Extractor:
         return out
 
     def read_candidates(self, frame, level):
-        n = C.c_int()
-        code = lib().sgs_extractor_read_candidates(self.h, frame, level, None, 0, C.byref(n))
-        if code not in (SGS_OK, SGS_ERR_CAPACITY):
-            check(code)
-        out = np.zeros((max(n.value, 1), 3), np.int32)
-        if n.value:
-            check(lib().sgs_extractor_read_candidates(self.h, frame, level, _p(out), n.value, C.byref(n)))
-        return out[:n.value]
+        return _sized(lib().sgs_extractor_read_candidates, (self.h, frame, level), (np.int32, 3))
 
 
 def hamming_pairs(a, b, device=0):
@@ -282,8 +314,7 @@ def hamming_bf_scratch_elems(nq, nt):
 
 
 def hamming_bf_device(dq, nq, dt, nt, d_idx, d_best, d_second, d_scratch=0, stream=0):
-    check(lib().sgs_hamming_bf_device(C.c_void_p(dq), nq, C.c_void_p(dt), nt, C.c_void_p(d_idx), C.c_void_p(d_best), C.c_void_p(d_second),
-                                      C.c_void_p(d_scratch), C.c_void_p(stream)))
+    check(lib().sgs_hamming_bf_device(dq, nq, dt, nt, d_idx, d_best, d_second, d_scratch, stream))
 
 
 class HostFrame:
@@ -309,7 +340,7 @@ def match_project_lastframe(cur, Tcw_cur, Tcw_last, last_has_mp, last_xyz, last_
     mpo = None if cur_mp_obs is None else np.ascontiguousarray(cur_mp_obs, np.uint8)
     nm = C.c_int()
     check(lib().sgs_match_project_lastframe(C.byref(cur.c), _p(Tc), _p(Tl), n, _p(has), _p(xyz), _p(ld), _p(lo), _p(loct), _p(la),
-                                            C.c_float(th), int(mono), int(check_ori), _p(mp), _p(mpo), C.byref(nm), device))
+                                            th, int(mono), int(check_ori), _p(mp), _p(mpo), C.byref(nm), device))
     return nm.value, mp
 
 
@@ -321,8 +352,7 @@ def match_project_keyframe(cur, Tcw_cur, kf_valid, kf_xyz, kf_desc, kf_angle, mi
          np.ascontiguousarray(kf_angle, np.float32), np.ascontiguousarray(min_dist, np.float32), np.ascontiguousarray(max_dist, np.float32)]
     mp = np.full(cur.c.n, -1, np.int32) if cur_mp is None else np.ascontiguousarray(cur_mp, np.int32).copy()
     nm = C.c_int()
-    check(lib().sgs_match_project_keyframe(C.byref(cur.c), _p(Tc), n, *[_p(x) for x in a], C.c_float(th), int(orb_dist), int(check_ori), _p(mp), C.byref(nm),
-                                           device))
+    check(lib().sgs_match_project_keyframe(C.byref(cur.c), _p(Tc), n, *[_p(x) for x in a], th, int(orb_dist), int(check_ori), _p(mp), C.byref(nm), device))
     return nm.value, mp
 
 
@@ -333,8 +363,7 @@ def match_project_localmap(fr, inview, projx, projy, projxr, level, viewcos, mp_
          np.ascontiguousarray(mp_desc, np.uint8), np.ascontiguousarray(mp_obs, np.uint8)]
     mp = np.ascontiguousarray(f_mp, np.int32).copy(); mpo = np.ascontiguousarray(f_mp_obs, np.uint8).copy()
     nm = C.c_int()
-    check(lib().sgs_match_project_localmap(C.byref(fr.c), n, *[_p(x) for x in a], C.c_float(th), C.c_float(nnratio), id_base, _p(mp), _p(mpo),
-                                           C.byref(nm), device))
+    check(lib().sgs_match_project_localmap(C.byref(fr.c), n, *[_p(x) for x in a], th, nnratio, id_base, _p(mp), _p(mpo), C.byref(nm), device))
     return nm.value, mp, mpo
 
 
@@ -349,34 +378,21 @@ def dynreject(cur_xy, prev_xy, F, boxes, have_dyn, nfeatures, device=0):
     return nk.value, keep, dist, bool(rest.value)
 
 
-class Matcher:
+class Matcher(_Handle):
     def __init__(self, max_frames, cur_cap, point_cap, device=0):
-        self.h = C.c_void_p()
-        check(lib().sgs_matcher_create(device, max_frames, cur_cap, point_cap, C.byref(self.h)))
-
-    def close(self):
-        if self.h:
-            lib().sgs_matcher_destroy(self.h)
-            self.h = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
+        super().__init__(lib().sgs_matcher_create, lib().sgs_matcher_destroy, device, max_frames, cur_cap, point_cap)
 
     def lastframe_batch(self, args, nframes, stream=0):
-        check(lib().sgs_match_project_lastframe_batch_device(self.h, C.byref(args), nframes, C.c_void_p(stream)))
+        check(lib().sgs_match_project_lastframe_batch_device(self.h, C.byref(args), nframes, stream))
 
     def localmap_batch(self, args, nframes, stream=0):
-        check(lib().sgs_match_project_localmap_batch_device(self.h, C.byref(args), nframes, C.c_void_p(stream)))
+        check(lib().sgs_match_project_localmap_batch_device(self.h, C.byref(args), nframes, stream))
 
 
 def dynreject_batch_device(d_kps, d_desc, d_counts, cap, nframes, d_prev, d_F, d_boxes, d_nboxes, max_boxes, d_have, nfeatures,
                            d_kps_out, d_desc_out, d_counts_out, d_keep=0, stream=0):
-    v = C.c_void_p
-    check(lib().sgs_dynreject_batch_device(v(d_kps), v(d_desc), v(d_counts), cap, nframes, v(d_prev), v(d_F), v(d_boxes), v(d_nboxes), max_boxes,
-                                           v(d_have), nfeatures, v(d_kps_out), v(d_desc_out), v(d_counts_out), v(d_keep), v(stream)))
+    check(lib().sgs_dynreject_batch_device(d_kps, d_desc, d_counts, cap, nframes, d_prev, d_F, d_boxes, d_nboxes, max_boxes, d_have, nfeatures,
+                                           d_kps_out, d_desc_out, d_counts_out, d_keep, stream))
 
 
 def make_camera(w, h, cam, scale_factors):
@@ -389,59 +405,34 @@ def make_camera(w, h, cam, scale_factors):
     return c
 
 
-class Tracker:
+class Tracker(_Handle):
     """Batched front end with host buffers (sgs_tracker_* of include/sgs_abi.h)."""
 
     def __init__(self, width, height, camera, nfeatures=1000, scale=1.2, nlevels=8, ini=20, mn=7, max_batch=1, point_cap=1100, max_boxes=4, device=0):
         self.params = OrbParams(nfeatures, scale, nlevels, ini, mn)
-        self.h = C.c_void_p()
         self.cam = camera
-        check(lib().sgs_tracker_create(C.byref(self.params), width, height, max_batch, point_cap, max_boxes, C.byref(camera), device, C.byref(self.h)))
+        super().__init__(lib().sgs_tracker_create, lib().sgs_tracker_destroy, C.byref(self.params), width, height, max_batch, point_cap, max_boxes,
+                         C.byref(camera), device)
         cap = C.c_int()
         check(lib().sgs_tracker_max_keypoints(self.h, C.byref(cap)))
         self.cap, self.point_cap, self.max_boxes, self.max_batch = cap.value, point_cap, max_boxes, max_batch
 
-    def close(self):
-        if self.h:
-            lib().sgs_tracker_destroy(self.h)
-            self.h = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
     def extract(self, gray_ptr, nframes, frame_stride, pitch, kps_ptr, desc_ptr, n_ptr):
-        v = C.c_void_p
-        check(lib().sgs_tracker_extract(self.h, v(gray_ptr), nframes, C.c_size_t(frame_stride), pitch, v(kps_ptr), v(desc_ptr), self.cap, v(n_ptr)))
+        check(lib().sgs_tracker_extract(self.h, gray_ptr, nframes, frame_stride, pitch, kps_ptr, desc_ptr, self.cap, n_ptr))
 
     def track(self, nframes, ptrs, th, mono, check_ori, out_ptrs):
         """ptrs: prev_xy, u_right, F, boxes, nboxes, have_dyn, last_xyz, last_desc, last_flags, last_octave, last_angle, last_n, tcw_cur, tcw_last
         out_ptrs: kps, desc, u_right (or 0), counts, cur_mp, nmatches   (all raw host addresses)"""
-        v = C.c_void_p
-        check(lib().sgs_tracker_track(self.h, nframes, *[v(p) for p in ptrs], C.c_float(th), int(mono), int(check_ori), *[v(p) for p in out_ptrs]))
+        check(lib().sgs_tracker_track(self.h, nframes, *ptrs, th, int(mono), int(check_ori), *out_ptrs))
 
 
-class LK:
+class LK(_Handle):
     """cv::calcOpticalFlowPyrLK with the reference's parameters (sgs_lk_* of include/sgs_abi.h)."""
     PAD = 24            # border of every padded pyramid level (kLkPad)
 
     def __init__(self, width, height, max_batch=1, device=0):
-        self.h = C.c_void_p()
         self.width, self.height = width, height
-        check(lib().sgs_lk_create(width, height, max_batch, device, C.byref(self.h)))
-
-    def close(self):
-        if self.h:
-            lib().sgs_lk_destroy(self.h)
-            self.h = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
+        super().__init__(lib().sgs_lk_create, lib().sgs_lk_destroy, width, height, max_batch, device)
 
     def track(self, cur, prev, pts):
         cur = np.ascontiguousarray(cur, np.uint8); prev = np.ascontiguousarray(prev, np.uint8)
@@ -473,28 +464,25 @@ class LK:
 
     def track_batch_device(self, d_cur, d_prev, nframes, frame_stride, pitch, d_kps, d_counts, cap, d_prev_xy, stream=0, d_prev_index=0):
         """Previous images: d_prev [F], or frames of d_cur itself when d_prev_index [F] is given (then d_prev may be 0)."""
-        v = C.c_void_p
-        check(lib().sgs_lk_track_batch_device(self.h, v(d_cur), v(d_prev), v(d_prev_index), nframes, C.c_size_t(frame_stride), pitch, v(d_kps), v(d_counts),
-                                              cap, v(d_prev_xy), v(stream)))
+        check(lib().sgs_lk_track_batch_device(self.h, d_cur, d_prev, d_prev_index, nframes, frame_stride, pitch, d_kps, d_counts, cap, d_prev_xy, stream))
 
 
 def fundamental_ransac(pts1, pts2, thresh=1.0, confidence=0.99, max_iters=1000, device=0):
     """cv::findFundamentalMat(pts1, pts2, FM_RANSAC, thresh, confidence) on the GPU.  Returns (F 3x3 or None, mask, info[4])."""
     a = np.ascontiguousarray(pts1, np.float32).reshape(-1, 2); b = np.ascontiguousarray(pts2, np.float32).reshape(-1, 2)
     F = np.zeros(9, np.float64); mask = np.zeros(len(a), np.uint8); info = np.zeros(4, np.int32)
-    check(lib().sgs_fundamental_ransac(_p(a), _p(b), len(a), C.c_double(thresh), C.c_double(confidence), int(max_iters), _p(F), _p(mask), _p(info), device))
+    check(lib().sgs_fundamental_ransac(_p(a), _p(b), len(a), thresh, confidence, int(max_iters), _p(F), _p(mask), _p(info), device))
     return (None if np.isnan(F[0]) else F.reshape(3, 3)), mask, info
 
 
 def fundamental_batch_device(d_kps, d_prev_xy, d_counts, cap, nframes, d_boxes, d_nboxes, d_have, max_boxes, d_prev_index, d_F, d_info,
                              thresh=1.0, confidence=0.99, max_iters=1000, stream=0):
-    v = C.c_void_p
-    check(lib().sgs_fundamental_batch_device(v(d_kps), v(d_prev_xy), v(d_counts), cap, nframes, v(d_boxes), v(d_nboxes), v(d_have), max_boxes,
-                                             v(d_prev_index), C.c_double(thresh), C.c_double(confidence), int(max_iters), v(d_F), v(d_info), v(stream)))
+    check(lib().sgs_fundamental_batch_device(d_kps, d_prev_xy, d_counts, cap, nframes, d_boxes, d_nboxes, d_have, max_boxes, d_prev_index,
+                                             thresh, confidence, int(max_iters), d_F, d_info, stream))
 
 
 def memcpy_d2h(dst_array, d_ptr):
-    check(lib().sgs_memcpy_d2h(_p(dst_array), C.c_void_p(d_ptr), C.c_size_t(dst_array.nbytes)))
+    check(lib().sgs_memcpy_d2h(_p(dst_array), d_ptr, dst_array.nbytes))
     return dst_array
 
 
@@ -502,48 +490,29 @@ OBJ_DTYPE = np.dtype([('id', '<i4'), ('prob', '<f4'), ('x', '<f4'), ('y', '<f4')
 DET_DIAGNOSTIC, DET_PLAN_ONLY = 1, 2
 
 
-class Detector:
+class Detector(_Handle):
     """Detector2D (src/Detector2D.cc) on the GPU: sgs_detector_* of include/sgs_abi.h."""
 
     def __init__(self, param_path, bin_path, max_frames=1, det_thr=0.9, dyn_thr=0.01, flags=0, device=0):
-        self.h = C.c_void_p()
         self.flags = flags
-        check(lib().sgs_detector_create(os.fsencode(param_path), os.fsencode(bin_path), max_frames, C.c_float(det_thr), C.c_float(dyn_thr), flags, device,
-                                        C.byref(self.h)))
+        super().__init__(lib().sgs_detector_create, lib().sgs_detector_destroy, os.fsencode(param_path), os.fsencode(bin_path), max_frames, det_thr,
+                         dyn_thr, flags, device)
         r, t, nl, nk = C.c_int(), C.c_int(), C.c_int(), C.c_int()
         check(lib().sgs_detector_info(self.h, C.byref(r), C.byref(t), C.byref(nl), C.byref(nk)))
         self.rows_cap, self.input_size, self.num_layers, self.num_kernels = r.value, t.value, nl.value, nk.value
-
-    def close(self):
-        if self.h:
-            lib().sgs_detector_destroy(self.h)
-            self.h = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
     def set_profiling(self, enable):
         check(lib().sgs_detector_set_profiling(self.h, int(enable)))
 
     def kernel_times(self):
         """(ms_total per kernel [preprocess, the kernels of describe() in order, detout_class, detout_merge], completed calls)"""
-        nk, nc = C.c_int(), C.c_int()
-        check(lib().sgs_detector_kernel_times(self.h, None, 0, C.byref(nk), C.byref(nc)))
-        ms = (C.c_double * nk.value)()
-        check(lib().sgs_detector_kernel_times(self.h, ms, nk.value, C.byref(nk), C.byref(nc)))
-        return [ms[i] for i in range(nk.value)], nc.value
+        nc = C.c_int()
+        ms = _sized(lib().sgs_detector_kernel_times, (self.h,), np.float64, tail=(C.byref(nc),))
+        return ms.tolist(), nc.value
 
     def describe(self):
-        n = C.c_int64()
-        rc = lib().sgs_detector_describe(self.h, None, 0, C.byref(n))
-        if rc not in (SGS_OK, SGS_ERR_CAPACITY):
-            check(rc)
-        buf = C.create_string_buffer(n.value)
-        check(lib().sgs_detector_describe(self.h, buf, n.value, C.byref(n)))
-        return buf.value.decode()
+        text = _sized(lib().sgs_detector_describe, (self.h,), np.uint8, C.c_int64)
+        return text.tobytes().split(b'\0', 1)[0].decode()
 
     def detect(self, rgb):
         """One host frame (H x W x 3 uint8): accepted objects in detection order (OBJ_DTYPE)."""
@@ -554,16 +523,8 @@ class Detector:
 
     def detect_device(self, d_rgb, frame_stride, pitch, width, height, nframes, d_rows=0, d_nrows=0, d_objects=0, d_nobjects=0, d_dyn_map=0,
                       d_ndyn_map=0, d_dyn_rm=0, d_ndyn_rm=0, d_have_dyn_rm=0, max_boxes=0, d_status=0, stream=0):
-        v = C.c_void_p
-        check(lib().sgs_detector_detect_device(self.h, v(d_rgb), C.c_int64(frame_stride), pitch, width, height, nframes, v(d_rows), v(d_nrows), v(d_objects),
-                                               v(d_nobjects), v(d_dyn_map), v(d_ndyn_map), v(d_dyn_rm), v(d_ndyn_rm), v(d_have_dyn_rm), max_boxes, v(d_status),
-                                               v(stream)))
+        check(lib().sgs_detector_detect_device(self.h, d_rgb, frame_stride, pitch, width, height, nframes, d_rows, d_nrows, d_objects, d_nobjects,
+                                               d_dyn_map, d_ndyn_map, d_dyn_rm, d_ndyn_rm, d_have_dyn_rm, max_boxes, d_status, stream))
 
     def blob(self, name, frame=0):
-        n = C.c_int64()
-        rc = lib().sgs_detector_blob(self.h, name.encode(), frame, None, 0, C.byref(n))
-        if rc not in (SGS_OK, SGS_ERR_CAPACITY):
-            check(rc)
-        out = np.zeros(n.value, np.float32)
-        check(lib().sgs_detector_blob(self.h, name.encode(), frame, _p(out), out.size, C.byref(n)))
-        return out
+        return _sized(lib().sgs_detector_blob, (self.h, name.encode(), frame), np.float32, C.c_int64)

@@ -12,15 +12,11 @@ import scenarios as S  # noqa: E402
 from pysgs import binding as B  # noqa: E402
 
 
-class GpuVoc:
+class GpuVoc(B._Handle):
     def __init__(self, voc):
-        self.h = C.c_void_p()
         v = C.c_void_p
-        B.check(B.lib().sgs_vocabulary_create(0, voc['k'], voc['L'], len(voc['parent']), voc['parent'].ctypes.data_as(v), np.ascontiguousarray(voc['desc']).ctypes.data_as(v),
-                                              voc['weight'].ctypes.data_as(v), C.byref(self.h)))
-
-    def close(self):
-        B.lib().sgs_vocabulary_destroy(self.h)
+        super().__init__(B.lib().sgs_vocabulary_create, B.lib().sgs_vocabulary_destroy, 0, voc['k'], voc['L'], len(voc['parent']), voc['parent'].ctypes.data_as(v),
+                         np.ascontiguousarray(voc['desc']).ctypes.data_as(v), voc['weight'].ctypes.data_as(v))
 
 
 def _transform_gpu(gv, desc, counts, levelsup):
@@ -111,7 +107,7 @@ def test_host_variants():
         m = np.zeros(1000, np.int32); nm = C.c_int()
         P = lambda a: np.ascontiguousarray(a).ctypes.data_as(v)
         B.check(B.lib().sgs_match_bow(900, P(kn), P(kw), P(s['kf_valid']), P(s['kf_desc']), P(s['kf_angle']), 1000, P(fn), P(fw), P(s['f_desc']), P(s['f_angle']),
-                                      C.c_float(0.7), 1, m.ctypes.data_as(v), C.byref(nm), 0))
+                                      0.7, 1, m.ctypes.data_as(v), C.byref(nm), 0))
         onm, om = O.search_by_bow(kn, kw, s['kf_valid'], s['kf_desc'], s['kf_angle'], fn, fw, s['f_desc'], s['f_angle'], 0.7, True)
         assert nm.value == onm and np.array_equal(m, om)
         B.check(B.lib().sgs_bow_transform(gv.h, None, 0, 1, None, None, None))              # nothing to transform: no device work
@@ -125,7 +121,7 @@ def _match_bow_keyframes_host(mode, k1, k2, nnratio, ori, F12=None, epipole=None
     side = lambda k: [P(k['node'], np.int32), P(k['weight'], np.float64), P(k['valid'], np.uint8), P(k['desc'], np.uint8), P(k['angle'], np.float32)]
     n1, n2 = len(k1['desc']), len(k2['desc'])
     m = np.full(n1, 7, np.int32); nm = C.c_int(-1)
-    B.check(B.lib().sgs_match_bow_keyframes(mode, n1, *side(k1), n2, *side(k2), C.c_float(nnratio), int(ori), P(k1.get('stereo'), np.uint8), P(k2.get('stereo'), np.uint8),
+    B.check(B.lib().sgs_match_bow_keyframes(mode, n1, *side(k1), n2, *side(k2), nnratio, int(ori), P(k1.get('stereo'), np.uint8), P(k2.get('stereo'), np.uint8),
                                             P(k1.get('xy'), np.float32), P(k2.get('xy'), np.float32), P(k2.get('octave'), np.int32), P(F12, np.float32),
                                             P(epipole, np.float32), P(sigma2, np.float32), P(sf, np.float32), 0 if sf is None else len(sf), int(only_stereo),
                                             P(m), C.byref(nm), 0))

@@ -160,7 +160,7 @@ def test_large_pinned_batch_goes_up_in_chunks():
         pin = torch.from_numpy(frames).pin_memory()
         hk = torch.zeros((nf, ex.cap, 28), dtype=torch.uint8).pin_memory(); hd = torch.zeros((nf, ex.cap, 32), dtype=torch.uint8).pin_memory()
         n = np.zeros(nf, np.int32)
-        B.check(B.lib().sgs_extract_batch(ex.h, C.c_void_p(pin.data_ptr()), nf, C.c_size_t(640 * 480), 640, C.c_void_p(hk.data_ptr()), C.c_void_p(hd.data_ptr()), ex.cap,
+        B.check(B.lib().sgs_extract_batch(ex.h, C.c_void_p(pin.data_ptr()), nf, 640 * 480, 640, C.c_void_p(hk.data_ptr()), C.c_void_p(hd.data_ptr()), ex.cap,
                                           n.ctypes.data_as(C.c_void_p)))
         assert np.array_equal(n, ref_n)
         k = hk.numpy().reshape(nf, ex.cap * 28).view(B.KP_DTYPE).reshape(nf, ex.cap)

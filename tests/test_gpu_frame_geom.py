@@ -57,7 +57,7 @@ def test_frustum_golden(golden_dir):
     h = dict(inview=np.full(n, 7, np.uint8), proj_x=np.zeros(n, np.float32), proj_y=np.zeros(n, np.float32), proj_xr=np.zeros(n, np.float32),
              level=np.zeros(n, np.int32), view_cos=np.zeros(n, np.float32))
     P = lambda a: np.ascontiguousarray(a).ctypes.data_as(C.c_void_p)
-    B.check(B.lib().sgs_frustum(C.byref(cam), P(g['Tcw'].astype(np.float32)), n, P(g['xyz']), P(g['normal']), P(g['min_dist']), P(g['max_dist']), C.c_float(0.5),
+    B.check(B.lib().sgs_frustum(C.byref(cam), P(g['Tcw'].astype(np.float32)), n, P(g['xyz']), P(g['normal']), P(g['min_dist']), P(g['max_dist']), 0.5,
                                 *[P(h[k]) for k in ('inview', 'proj_x', 'proj_y', 'proj_xr', 'level', 'view_cos')], 0))
     _same(h, g, g['level_arg'])
 
@@ -126,8 +126,8 @@ def test_stereo_from_depth():
     dk = torch.from_numpy(kps.view(np.uint8).reshape(-1)).cuda(); dd = torch.from_numpy(depth).cuda(); dc = torch.from_numpy(counts).cuda()
     ur = torch.zeros((F, cap), device='cuda'); dz = torch.zeros((F, cap), device='cuda')
     v = C.c_void_p
-    B.check(B.lib().sgs_stereo_from_depth_batch_device(v(dk.data_ptr()), v(0), v(dc.data_ptr()), cap, F, v(dd.data_ptr()), C.c_size_t(640 * 480), 640,
-                                                       C.c_float(40.0), v(ur.data_ptr()), v(dz.data_ptr()), v(0)))
+    B.check(B.lib().sgs_stereo_from_depth_batch_device(v(dk.data_ptr()), v(0), v(dc.data_ptr()), cap, F, v(dd.data_ptr()), 640 * 480, 640,
+                                                       40.0, v(ur.data_ptr()), v(dz.data_ptr()), v(0)))
     torch.cuda.synchronize()
     ur = ur.cpu().numpy(); dz = dz.cpu().numpy()
     for f in range(F):
@@ -137,8 +137,8 @@ def test_stereo_from_depth():
         assert np.all(ur[f, n:] == -1)
     # one shared depth image (frame stride 0): every frame looks up frame 0's depth
     ur2 = torch.zeros((F, cap), device='cuda')
-    B.check(B.lib().sgs_stereo_from_depth_batch_device(v(dk.data_ptr()), v(0), v(dc.data_ptr()), cap, F, v(dd.data_ptr()), C.c_size_t(0), 640,
-                                                       C.c_float(40.0), v(ur2.data_ptr()), v(0), v(0)))
+    B.check(B.lib().sgs_stereo_from_depth_batch_device(v(dk.data_ptr()), v(0), v(dc.data_ptr()), cap, F, v(dd.data_ptr()), 0, 640,
+                                                       40.0, v(ur2.data_ptr()), v(0), v(0)))
     torch.cuda.synchronize()
     ru, _ = O.stereo_from_rgbd(kps[1, :counts[1]], depth[0], 40.0)
     assert ur2.cpu().numpy()[1, :counts[1]].tobytes() == ru.tobytes()
@@ -151,11 +151,11 @@ def test_undistort_and_image_bounds(golden_dir):
     for name in ('TUM1', 'TUM2'):
         K = g[name + '_K']; D = np.ascontiguousarray(g[name + '_D'], np.float32); pts = np.ascontiguousarray(g[name + '_pts'])
         out = np.zeros_like(pts)
-        B.check(B.lib().sgs_undistort_points(pts.ctypes.data_as(v), len(pts), C.c_float(K[0]), C.c_float(K[1]), C.c_float(K[2]), C.c_float(K[3]),
+        B.check(B.lib().sgs_undistort_points(pts.ctypes.data_as(v), len(pts), K[0], K[1], K[2], K[3],
                                              D.ctypes.data_as(v), out.ctypes.data_as(v), 0))
         assert out.tobytes() == g[name + '_und'].tobytes(), name
         b = np.zeros(4, np.float32)
-        B.check(B.lib().sgs_image_bounds(640, 480, C.c_float(K[0]), C.c_float(K[1]), C.c_float(K[2]), C.c_float(K[3]), D.ctypes.data_as(v), b.ctypes.data_as(v), 0))
+        B.check(B.lib().sgs_image_bounds(640, 480, K[0], K[1], K[2], K[3], D.ctypes.data_as(v), b.ctypes.data_as(v), 0))
         c = g[name + '_und'][-4:]          # corners (0,0) (w,0) (0,h) (w,h)
         assert b[0] == min(c[0, 0], c[2, 0]) and b[2] == max(c[1, 0], c[3, 0]) and b[1] == min(c[0, 1], c[1, 1]) and b[3] == max(c[2, 1], c[3, 1])
         # batched keypoint form: two frames, the second shorter; everything but pt is copied
@@ -163,12 +163,12 @@ def test_undistort_and_image_bounds(golden_dir):
         kps = np.zeros((2, cap), B.KP_DTYPE); kps['x'] = pts[:, 0]; kps['y'] = pts[:, 1]; kps['octave'] = 3; kps['angle'] = 42.0
         counts = np.array([cap, 100], np.int32)
         dk = torch.from_numpy(kps.view(np.uint8).reshape(-1)).cuda(); dc = torch.from_numpy(counts).cuda(); du = torch.zeros_like(dk)
-        B.check(B.lib().sgs_undistort_batch_device(v(dk.data_ptr()), v(dc.data_ptr()), cap, 2, C.c_float(K[0]), C.c_float(K[1]), C.c_float(K[2]), C.c_float(K[3]),
+        B.check(B.lib().sgs_undistort_batch_device(v(dk.data_ptr()), v(dc.data_ptr()), cap, 2, K[0], K[1], K[2], K[3],
                                                    D.ctypes.data_as(v), v(du.data_ptr()), v(0)))
         torch.cuda.synchronize()
         un = du.cpu().numpy().view(B.KP_DTYPE).reshape(2, cap)
         assert np.stack([un['x'][0], un['y'][0]], 1).tobytes() == g[name + '_und'].tobytes()
         assert np.array_equal(un['octave'][1, :100], kps['octave'][1, :100]) and np.array_equal(un['x'][1, :100], un['x'][0, :100])
     zero = np.zeros(5, np.float32); b = np.zeros(4, np.float32)
-    B.check(B.lib().sgs_image_bounds(640, 480, C.c_float(500), C.c_float(500), C.c_float(320), C.c_float(240), zero.ctypes.data_as(v), b.ctypes.data_as(v), 0))
+    B.check(B.lib().sgs_image_bounds(640, 480, 500, 500, 320, 240, zero.ctypes.data_as(v), b.ctypes.data_as(v), 0))
     assert list(b) == [0, 0, 640, 480]

@@ -251,7 +251,7 @@ def _fuse_search_host(fg, Tcw, Ow, s, nrm, th, inv_s2, sim3, xf, kf_matched):
     P = lambda a: None if a is None else np.ascontiguousarray(a).ctypes.data_as(C.c_void_p)
     bi = np.full(nmp, 7, np.int32); bd = np.full(nmp, 7, np.int32); nm = C.c_int(-1)
     B.check(B.lib().sgs_fuse_search(C.byref(fg.c), P(Tcw.astype(np.float32).reshape(16)), P(Ow.astype(np.float32)), nmp, P(s['kf_valid']), P(s['last_xyz']), P(nrm),
-                                    P(s['min_dist']), P(s['max_dist']), P(s['last_desc']), C.c_float(th), P(inv_s2), sim3, P(xf), P(bi), P(bd),
+                                    P(s['min_dist']), P(s['max_dist']), P(s['last_desc']), th, P(inv_s2), sim3, P(xf), P(bi), P(bd),
                                     P(kf_matched), C.byref(nm), 0))
     return nm.value, bi, bd
 
@@ -347,7 +347,7 @@ def test_search_for_initialization(window, ori):
     k1 = np.ascontiguousarray(s['k1']); k2 = np.ascontiguousarray(s['k2']); d1 = np.ascontiguousarray(s['d1']); d2 = np.ascontiguousarray(s['d2'])
     v1, v2 = view(k1, d1), view(k2, d2)
     prev = s['prev'].copy(); mo = np.zeros(n1, np.int32); nmo = C.c_int()
-    B.check(B.lib().sgs_search_for_initialization(C.byref(v1), C.byref(v2), prev.ctypes.data_as(C.c_void_p), window, C.c_float(0.9), int(ori), mo.ctypes.data_as(C.c_void_p), C.byref(nmo), 0))
+    B.check(B.lib().sgs_search_for_initialization(C.byref(v1), C.byref(v2), prev.ctypes.data_as(C.c_void_p), window, 0.9, int(ori), mo.ctypes.data_as(C.c_void_p), C.byref(nmo), 0))
     assert nmo.value == ref[0][0] and np.array_equal(mo, ref[0][1]) and np.array_equal(prev, ref[0][2])
 
 

@@ -83,7 +83,7 @@ def test_pose_chain_against_the_oracle_functions():
     L, v = B.lib(), C.c_void_p
     P = lambda a: a.ctypes.data_as(v)
     kps = np.zeros((nb, cap), B.KP_DTYPE); desc = np.zeros((nb, cap, 32), np.uint8); n = np.zeros(nb, np.int32)
-    B.check(L.sgs_tracker_extract(trk.h, P(frames), nb, C.c_size_t(W * H), W, P(kps), P(desc), cap, P(n)))
+    B.check(L.sgs_tracker_extract(trk.h, P(frames), nb, W * H, W, P(kps), P(desc), cap, P(n)))
     ti = bench.make_track_inputs(kps, desc, n, boxes, cap, pcap, pidx, W, H, camd)
     ti['lflags'][:, 9::23] |= 4                                         # some last-frame points are bad
     # poses: identity for most frames; two frames start with a yaw / pitch error of ~60 px (beyond every window at th = 15: 15 * 1.2^7 = 53.7 px, inside the
@@ -102,7 +102,7 @@ def test_pose_chain_against_the_oracle_functions():
     o = dict(kps=np.zeros((nb, cap), B.KP_DTYPE), desc=np.zeros((nb, cap, 32), np.uint8), ur=np.zeros((nb, cap), np.float32), cnt=np.zeros(nb, np.int32),
              mp=np.zeros((nb, cap), np.int32), nm=np.zeros(nb, np.int32))
     track_lk = lambda: B.check(L.sgs_tracker_track_lk(trk.h, nb, P(ti['pidx']), P(ti['ur']), v(0), P(ti['boxes']), P(ti['nb']), P(ti['have']), P(ti['lxyz']), P(ti['ldesc']),
-                                                      P(ti['lflags']), P(ti['loct']), P(ti['lang']), P(ti['ln']), P(Tc), P(ti['T']), C.c_float(TH), 0, 1, P(o['kps']),
+                                                      P(ti['lflags']), P(ti['loct']), P(ti['lang']), P(ti['ln']), P(Tc), P(ti['T']), TH, 0, 1, P(o['kps']),
                                                       P(o['desc']), P(o['ur']), P(o['cnt']), P(o['mp']), P(o['nm'])))
     track_lk()
     rng = np.random.default_rng(5)

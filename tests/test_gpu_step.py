@@ -39,7 +39,7 @@ def test_step_equals_the_stages_called_one_by_one(tmp_path):
     P = lambda a: a.ctypes.data_as(v)
     # 1. stage by stage: extract (host), detector (host frames one by one -> boxes by hand), track_lk with those boxes
     kps = np.zeros((nb, cap), B.KP_DTYPE); desc = np.zeros((nb, cap, 32), np.uint8); n = np.zeros(nb, np.int32)
-    B.check(L.sgs_tracker_extract(trk.h, P(frames), nb, C.c_size_t(W * H), W, P(kps), P(desc), cap, P(n)))
+    B.check(L.sgs_tracker_extract(trk.h, P(frames), nb, W * H, W, P(kps), P(desc), cap, P(n)))
     ti = _inputs(frames, gt, kps, desc, n, cap, trk.point_cap, pidx)
     import torch
     d_rgb = torch.from_numpy(rgb).cuda()
@@ -52,12 +52,12 @@ def test_step_equals_the_stages_called_one_by_one(tmp_path):
               mp=np.zeros((nb, cap), np.int32), nm=np.zeros(nb, np.int32))
     T = ti['T']
     B.check(L.sgs_tracker_track_lk(trk.h, nb, P(pidx), P(ti['ur']), v(0), P(bx), P(nbx), P(hv), P(ti['lxyz']), P(ti['ldesc']), P(ti['lflags']), P(ti['loct']), P(ti['lang']),
-                                   P(ti['ln']), P(T), P(T), C.c_float(TH), 0, 1, P(o1['kps']), P(o1['desc']), P(o1['ur']), P(o1['cnt']), P(o1['mp']), P(o1['nm'])))
+                                   P(ti['ln']), P(T), P(T), TH, 0, 1, P(o1['kps']), P(o1['desc']), P(o1['ur']), P(o1['cnt']), P(o1['mp']), P(o1['nm'])))
     # 2. one call
     o2 = {k: np.zeros_like(a) for k, a in o1.items()}
     bo = np.zeros((nb, 4, 4), np.float32); nbo = np.zeros(nb, np.int32); hvo = np.zeros(nb, np.uint8)
-    B.check(L.sgs_tracker_step(trk.h, det.h, P(frames), C.c_size_t(W * H), W, P(rgb), C.c_size_t(W * H * 3), W * 3, nb, P(pidx), P(ti['ur']), P(ti['lxyz']), P(ti['ldesc']),
-                               P(ti['lflags']), P(ti['loct']), P(ti['lang']), P(ti['ln']), P(T), P(T), C.c_float(TH), 0, 1, P(o2['kps']), P(o2['desc']), P(o2['ur']), P(o2['cnt']),
+    B.check(L.sgs_tracker_step(trk.h, det.h, P(frames), W * H, W, P(rgb), W * H * 3, W * 3, nb, P(pidx), P(ti['ur']), P(ti['lxyz']), P(ti['ldesc']),
+                               P(ti['lflags']), P(ti['loct']), P(ti['lang']), P(ti['ln']), P(T), P(T), TH, 0, 1, P(o2['kps']), P(o2['desc']), P(o2['ur']), P(o2['cnt']),
                                P(o2['mp']), P(o2['nm']), P(bo), P(nbo), P(hvo)))
     assert np.array_equal(nbo, nbx) and np.array_equal(hvo, hv)
     for f in range(nb):
@@ -71,7 +71,7 @@ def test_step_equals_the_stages_called_one_by_one(tmp_path):
     z = np.zeros_like(nbx); zh = np.zeros_like(hv)
     o3 = {k: np.zeros_like(a) for k, a in o1.items()}
     B.check(L.sgs_tracker_track_lk(trk.h, nb, P(pidx), P(ti['ur']), v(0), P(bx), P(z), P(zh), P(ti['lxyz']), P(ti['ldesc']), P(ti['lflags']), P(ti['loct']), P(ti['lang']),
-                                   P(ti['ln']), P(T), P(T), C.c_float(TH), 0, 1, P(o3['kps']), P(o3['desc']), P(o3['ur']), P(o3['cnt']), P(o3['mp']), P(o3['nm'])))
+                                   P(ti['ln']), P(T), P(T), TH, 0, 1, P(o3['kps']), P(o3['desc']), P(o3['ur']), P(o3['cnt']), P(o3['mp']), P(o3['nm'])))
     if hv.any():
         assert not np.array_equal(o3['cnt'], o1['cnt'])
     trk.close(); det.close()

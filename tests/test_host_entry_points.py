@@ -8,7 +8,7 @@ import pytest
 
 from pysgs import binding as B
 
-v, f32, f64 = C.c_void_p, C.c_float, C.c_double
+v = C.c_void_p
 
 
 def _p(a):
@@ -49,7 +49,7 @@ def lastframe(ncur=3, nlast=4, drop=None):
     nm = C.c_int(-5)
     P = {k: (None if k == drop else _p(x)) for k, x in a.items()}
     rc = B.lib().sgs_match_project_lastframe(C.byref(_view(ncur)), _p(T), _p(T), nlast, P['has'], P['xyz'], P['desc'], P['obs'], P['oct'], P['ang'],
-                                             f32(15.0), 0, 1, P['mp'], None, C.byref(nm), 0)
+                                             15.0, 0, 1, P['mp'], None, C.byref(nm), 0)
     return rc, dict(nmatches=nm.value)
 
 
@@ -58,7 +58,7 @@ def keyframe(ncur=3, nkf=4, drop=None):
              mx=_z(nkf, np.float32), mp=_f(ncur, -1, np.int32))
     nm = C.c_int(-5)
     P = {k: (None if k == drop else _p(x)) for k, x in a.items()}
-    rc = B.lib().sgs_match_project_keyframe(C.byref(_view(ncur)), _p(T), nkf, P['valid'], P['xyz'], P['desc'], P['ang'], P['mn'], P['mx'], f32(10.0), 100, 1,
+    rc = B.lib().sgs_match_project_keyframe(C.byref(_view(ncur)), _p(T), nkf, P['valid'], P['xyz'], P['desc'], P['ang'], P['mn'], P['mx'], 10.0, 100, 1,
                                             P['mp'], C.byref(nm), 0)
     return rc, dict(nmatches=nm.value)
 
@@ -69,7 +69,7 @@ def localmap(ncur=3, nmp=4, drop=None):
     nm = C.c_int(-5)
     P = {k: (None if k == drop else _p(x)) for k, x in a.items()}
     rc = B.lib().sgs_match_project_localmap(C.byref(_view(ncur)), nmp, P['inview'], P['px'], P['py'], P['pxr'], P['lvl'], P['vc'], P['desc'], P['obs'],
-                                            f32(1.0), f32(0.8), 0, P['mp'], P['mpo'], C.byref(nm), 0)
+                                            1.0, 0.8, 0, P['mp'], P['mpo'], C.byref(nm), 0)
     return rc, dict(nmatches=nm.value)
 
 
@@ -79,7 +79,7 @@ def fuse(nkf=3, nmp=4, drop=None):
     bi = _f(nmp, 7, np.int32); bd = _f(nmp, 7, np.int32); nm = C.c_int(-5)
     P = {k: (None if k == drop else _p(x)) for k, x in a.items()}
     rc = B.lib().sgs_fuse_search(C.byref(_view(nkf)), _p(T), _p(np.zeros(3, np.float32)), nmp, P['valid'], P['xyz'], P['nrm'], P['mn'], P['mx'], P['desc'],
-                                 f32(3.0), P['s2'], 0, None, _p(bi), _p(bd), None, C.byref(nm), 0)
+                                 3.0, P['s2'], 0, None, _p(bi), _p(bd), None, C.byref(nm), 0)
     return rc, dict(nmatches=nm.value, best_idx=bi, best_dist=bd)
 
 
@@ -87,7 +87,7 @@ def init(n1=3, n2=4, drop=None):
     a = dict(prev=_z(n1, np.float32, (2,)), m12=_f(n1, 7, np.int32))
     nm = C.c_int(-5)
     P = {k: (None if k == drop else _p(x)) for k, x in a.items()}
-    rc = B.lib().sgs_search_for_initialization(C.byref(_view(n1)), C.byref(_view(n2)), P['prev'], 100, f32(0.9), 1, P['m12'], C.byref(nm), 0)
+    rc = B.lib().sgs_search_for_initialization(C.byref(_view(n1)), C.byref(_view(n2)), P['prev'], 100, 0.9, 1, P['m12'], C.byref(nm), 0)
     return rc, dict(nmatches=nm.value, match12=a['m12'])
 
 
@@ -97,7 +97,7 @@ def bow_keyframes(n1=3, n2=4, drop=None, mode=1):
     nm = C.c_int(-5)
     P = {k: (None if k == drop else _p(x)) for k, x in a.items()}
     rc = B.lib().sgs_match_bow_keyframes(mode, n1, P['node1'], P['w1'], P['v1'], P['d1'], P['a1'], n2, P['node2'], P['w2'], P['v2'], P['d2'], P['a2'],
-                                         f32(0.75), 1, None, None, None, None, None, None, None, None, None, 8, 0, P['m12'], C.byref(nm), 0)
+                                         0.75, 1, None, None, None, None, None, None, None, None, None, 8, 0, P['m12'], C.byref(nm), 0)
     return rc, dict(nmatches=nm.value, match12=a['m12'])
 
 
@@ -106,7 +106,7 @@ def match_bow(nkf=3, nf=4, drop=None):
              fn=_z(nf, np.int32), fw=_z(nf, np.float64), fd=_z(nf, np.uint8, (32,)), fa=_z(nf, np.float32), mf=_f(nf, 7, np.int32))
     nm = C.c_int(-5)
     P = {k: (None if k == drop else _p(x)) for k, x in a.items()}
-    rc = B.lib().sgs_match_bow(nkf, P['kn'], P['kw'], P['kv'], P['kd'], P['ka'], nf, P['fn'], P['fw'], P['fd'], P['fa'], f32(0.7), 1, P['mf'], C.byref(nm), 0)
+    rc = B.lib().sgs_match_bow(nkf, P['kn'], P['kw'], P['kv'], P['kd'], P['ka'], nf, P['fn'], P['fw'], P['fd'], P['fa'], 0.7, 1, P['mf'], C.byref(nm), 0)
     return rc, dict(nmatches=nm.value, match_f=a['mf'])
 
 
@@ -125,7 +125,7 @@ def hamming_bf(nq=4, nt=4, drop=None):
 def undistort(n=4, drop=None):
     a = dict(xy=_z(n, np.float32, (2,)), k=np.array([0.1, 0, 0, 0, 0], np.float32), out=_z(n, np.float32, (2,)))
     P = {k: (None if k == drop else _p(x)) for k, x in a.items()}
-    return B.lib().sgs_undistort_points(P['xy'], n, f32(500), f32(500), f32(320), f32(240), P['k'], P['out'], 0), {}
+    return B.lib().sgs_undistort_points(P['xy'], n, 500, 500, 320, 240, P['k'], P['out'], 0), {}
 
 
 def frustum(n=4, drop=None):
@@ -133,7 +133,7 @@ def frustum(n=4, drop=None):
     a = dict(cam=None, xyz=_z(n, np.float32, (3,)), nrm=_z(n, np.float32, (3,)), mn=_z(n, np.float32), mx=_z(n, np.float32), iv=_z(n, np.uint8),
              px=_z(n, np.float32), py=_z(n, np.float32), pxr=_z(n, np.float32), lvl=_z(n, np.int32), vc=_z(n, np.float32))
     P = {k: (None if k == drop else (C.byref(cam) if k == 'cam' else _p(x))) for k, x in a.items()}
-    rc = B.lib().sgs_frustum(P['cam'], _p(T), n, P['xyz'], P['nrm'], P['mn'], P['mx'], f32(0.5), P['iv'], P['px'], P['py'], P['pxr'], P['lvl'], P['vc'], 0)
+    rc = B.lib().sgs_frustum(P['cam'], _p(T), n, P['xyz'], P['nrm'], P['mn'], P['mx'], 0.5, P['iv'], P['px'], P['py'], P['pxr'], P['lvl'], P['vc'], 0)
     return rc, {}
 
 
@@ -159,7 +159,7 @@ def dynreject(n=4, drop=None):
 def fundamental(n=8, drop=None):
     a = dict(p1=_z(n, np.float32, (2,)), p2=_z(n, np.float32, (2,)), F=_z(9, np.float64))
     P = {k: (None if k == drop else _p(x)) for k, x in a.items()}
-    return B.lib().sgs_fundamental_ransac(P['p1'], P['p2'], n, f64(1.0), f64(0.99), 200, P['F'], None, None, 0), {}
+    return B.lib().sgs_fundamental_ransac(P['p1'], P['p2'], n, 1.0, 0.99, 200, P['F'], None, None, 0), {}
 
 
 def _invalid(name, rc):

@@ -2,7 +2,6 @@
 (sgs_detector_describe): per kernel time, achieved GB/s and FP32-equivalent TFLOP/s of the 1x1-convolution GEMMs.  Usage: det_launch_table.py launches.csv [batch]"""
 import collections
 import csv
-import ctypes as C
 import os
 import re
 import sys
@@ -12,12 +11,9 @@ sys.path.insert(0, os.path.join(ROOT, 'sg-slam_b200'))
 from pysgs import binding as B  # noqa: E402
 
 path = sys.argv[1]; F = int(sys.argv[2]) if len(sys.argv) > 2 else 128
-L = B.lib(); h = C.c_void_p()
 m = os.path.join(ROOT, 'oracle', '_ref', 'ncnn_model', 'mobilenetv3_ssdlite_voc')
-B.check(L.sgs_detector_create((m + '.param').encode(), (m + '.bin').encode(), F, C.c_float(0.5), C.c_float(0.1), 2, 0, C.byref(h)))
-buf = C.create_string_buffer(1 << 20); n = C.c_int64()
-L.sgs_detector_describe(h, buf, C.c_int64(1 << 20), C.byref(n))
-ops = [o for o in buf.value.decode().split('\n')[1:] if o]
+plan = B.Detector(m + '.param', m + '.bin', max_frames=F, det_thr=0.5, dyn_thr=0.1, flags=B.DET_PLAN_ONLY)
+ops = [o for o in plan.describe().split('\n')[1:] if o]
 rows = [r for r in csv.reader(open(path)) if len(r) > 5]
 for i, r in enumerate(rows):
     if 'Kernel Name' in r:

@@ -35,10 +35,9 @@ def build(nh):
         d_frames = torch.from_numpy(frames[sl]).cuda(); d_pidx = torch.from_numpy(np.ascontiguousarray(pidx[sl] - i * hb)).cuda()
         # inputs of the track stage: dummy last-frame points (zeros are fine for timing shape? no: use real ones from a set-up pass)
         hk = np.zeros((hb, cap), B.KP_DTYPE); hd = np.zeros((hb, cap, 32), np.uint8); hn = np.zeros(hb, np.int32)
-        L.sgs_tracker_extractor.restype = C.c_void_p
-        exh = v(L.sgs_tracker_extractor(trk.h))
-        B.check(L.sgs_tracker_extract_device(trk.h, v(d_frames.data_ptr()), hb, C.c_size_t(W * H), W, v(st.cuda_stream)))
-        B.check(L.sgs_extractor_fetch(exh, hb, hk.ctypes.data_as(v), hd.ctypes.data_as(v), cap, hn.ctypes.data_as(v), v(st.cuda_stream)))
+        exh = L.sgs_tracker_extractor(trk.h)
+        B.check(L.sgs_tracker_extract_device(trk.h, d_frames.data_ptr(), hb, W * H, W, st.cuda_stream))
+        B.check(L.sgs_extractor_fetch(exh, hb, hk.ctypes.data_as(v), hd.ctypes.data_as(v), cap, hn.ctypes.data_as(v), st.cuda_stream))
         ti = BN.make_track_inputs(hk, hd, hn, boxes[sl], None, cap, NF + 64, pidx[sl] - i * hb)
         dv = {k: torch.from_numpy(np.ascontiguousarray(ti[k])).cuda() for k in ('ur', 'boxes', 'nb', 'have', 'lxyz', 'ldesc', 'lflags', 'loct', 'lang', 'ln', 'T')}
         hs.append(dict(trk=trk, st=st, d_frames=d_frames, d_pidx=d_pidx, dv=dv, hb=hb))
@@ -47,12 +46,12 @@ def build(nh):
 
 def step(h):
     trk, st, hb, dv = h['trk'], h['st'], h['hb'], h['dv']
-    B.check(L.sgs_tracker_extract_device(trk.h, v(h['d_frames'].data_ptr()), hb, C.c_size_t(W * H), W, v(st.cuda_stream)))
-    B.check(L.sgs_tracker_lk_device(trk.h, v(h['d_frames'].data_ptr()), hb, C.c_size_t(W * H), W, v(h['d_pidx'].data_ptr()), v(st.cuda_stream)))
-    B.check(L.sgs_tracker_fundamental_device(trk.h, hb, v(dv['boxes'].data_ptr()), v(dv['nb'].data_ptr()), v(dv['have'].data_ptr()), v(h['d_pidx'].data_ptr()), v(st.cuda_stream)))
-    B.check(L.sgs_tracker_stereo_device(trk.h, hb, v(d_depth.data_ptr()), C.c_size_t(0), W, v(st.cuda_stream)))
+    B.check(L.sgs_tracker_extract_device(trk.h, h['d_frames'].data_ptr(), hb, W * H, W, st.cuda_stream))
+    B.check(L.sgs_tracker_lk_device(trk.h, h['d_frames'].data_ptr(), hb, W * H, W, h['d_pidx'].data_ptr(), st.cuda_stream))
+    B.check(L.sgs_tracker_fundamental_device(trk.h, hb, dv['boxes'].data_ptr(), dv['nb'].data_ptr(), dv['have'].data_ptr(), h['d_pidx'].data_ptr(), st.cuda_stream))
+    B.check(L.sgs_tracker_stereo_device(trk.h, hb, d_depth.data_ptr(), 0, W, st.cuda_stream))
     ptrs = [0, 0] + [dv[k].data_ptr() for k in ('boxes', 'nb', 'have', 'lxyz', 'ldesc', 'lflags', 'loct', 'lang', 'ln', 'T', 'T')]
-    B.check(L.sgs_tracker_track_device(trk.h, hb, v(0), *[v(p) for p in ptrs], C.c_float(TH), 0, 1, v(st.cuda_stream)))
+    B.check(L.sgs_tracker_track_device(trk.h, hb, 0, *ptrs, TH, 0, 1, st.cuda_stream))
 
 
 for nh in (1, 2, 4):
