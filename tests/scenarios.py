@@ -198,17 +198,18 @@ def bow_pair_scenario(seed, voc, n_kf=1000, n_f=1000, flips=40):
     return dict(kf_desc=kf_desc, f_desc=f_desc, kf_angle=kf_angle, f_angle=f_angle, kf_valid=kf_valid)
 
 
-def pose_scenario(seed, n=800, outlier_frac=0.15, noise=0.5, mono_frac=0.2, pose_err=(0.02, 0.05)):
+def pose_scenario(seed, n=800, outlier_frac=0.15, noise=0.5, mono_frac=0.2, pose_err=(0.02, 0.05), nlevels=8):
     """Motion-only BA input: map points seen from a true pose, keypoints = projections + noise (a fraction is gross outliers), some without
-    depth (monocular observations); the initial pose is the true pose perturbed by pose_err = (rotation rad, translation m)."""
+    depth (monocular observations); the initial pose is the true pose perturbed by pose_err = (rotation rad, translation m).  Octaves are
+    drawn from the `nlevels` levels of a 1.2 pyramid."""
     rng = np.random.RandomState(seed)
     cam = dict(synth.TUM3)
-    sf = scale_factors().astype(np.float32)
+    sf = scale_factors(nlevels).astype(np.float32)
     T_true = pose(0.03, -0.02, 0.01, (0.1, -0.05, 0.2))
     Xc = np.c_[rng.uniform(-1.5, 1.5, n), rng.uniform(-1.0, 1.0, n), rng.uniform(1.0, 6.0, n)]
     R = T_true[:3, :3].astype(np.float64); t = T_true[:3, 3].astype(np.float64)
     Xw = ((Xc - t) @ R).astype(np.float32)
-    octave = rng.randint(0, 8, n).astype(np.int32)
+    octave = rng.randint(0, nlevels, n).astype(np.int32)
     u = cam['fx'] * Xc[:, 0] / Xc[:, 2] + cam['cx']; v = cam['fy'] * Xc[:, 1] / Xc[:, 2] + cam['cy']
     sig = noise * sf[octave]
     xy = np.stack([u + rng.normal(0, 1, n) * sig, v + rng.normal(0, 1, n) * sig], 1)

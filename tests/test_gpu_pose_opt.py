@@ -1,6 +1,7 @@
 """GPU Optimizer::PoseOptimization through the C ABI against the CPU restatement (tests/test_pose_opt.py explains why g2o itself is not the
-reference here).  Tolerance: pose entries 1e-6 absolute (both sides are FP64 with different summation orders, results stored as float32);
-outlier flags and inlier counts identical."""
+reference here).  Tolerance: pose entries within one float32 ulp (both sides are FP64 with different summation orders, ~1e-12 apart on the double
+pose; rounding that to float32 can add one ulp, no more); outlier flags and inlier counts identical.  tests/test_gpu_pose_opt_cases.py runs the
+full case set."""
 import ctypes as C
 
 import numpy as np
@@ -9,6 +10,7 @@ import pytest
 pytestmark = pytest.mark.gpu
 
 import oracle as O  # noqa: E402
+import pose_cases as PC  # noqa: E402
 import scenarios as S  # noqa: E402
 from pysgs import binding as B  # noqa: E402
 
@@ -72,7 +74,7 @@ def _scenarios():
 def _check(f, s, T, outl, nin):
     c = s['cam']; m = len(s['xy'])
     rn, rT, ro = O.pose_optimization(s['T0'], s['has'], s['xyz'], s['xy'], s['octave'], s['uright'], s['inv_s2'], c['fx'], c['fy'], c['cx'], c['cy'], c['bf'])
-    assert np.abs(T - rT).max() <= 1e-6, (f, np.abs(T - rT).max())
+    assert PC.ulp_distance(T, rT).max() <= 1, (f, int(PC.ulp_distance(T, rT).max()), np.abs(T - rT).max())
     used = s['has'] == 1
     assert np.array_equal(outl[:m][used], ro[used]), (f, int((outl[:m][used] != ro[used]).sum()))
     assert nin == rn, (f, nin, rn)

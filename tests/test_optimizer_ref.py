@@ -3,7 +3,8 @@ file compiled unmodified from the reference tree; see oracle/Makefile, target re
 stand-in of oracle/g2o_shim/Eigen (eager evaluation of Eigen's published formulas): what is pinned is the control flow and arithmetic of Optimizer.cc and g2o --
 graph set-up, Levenberg with its lambda schedule and rejected trials, the Huber kernel, the four rounds with their chi-square re-classification, the early exits --
 not Eigen's instruction order.  The oracle's sgo_pose_optimization (oracle/pose_opt.cpp, the checker of the GPU's pose_opt_kernel) must return the same inlier
-count and the same outlier flags; the pose (float32 on both sides) must agree within 1e-6 -- on every case below it is in fact identical.  No device needed."""
+count and the same outlier flags; the pose (float32 on both sides) must agree within 1e-6 -- on every case below it is in fact identical.  The frames are
+pose_cases.reference_cases(), shared with the device kernel's tests.  No device needed."""
 import ctypes as C
 import os
 
@@ -11,7 +12,7 @@ import numpy as np
 import pytest
 
 import oracle as O
-import scenarios as S
+import pose_cases as PC
 
 LIB = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), 'oracle', '_ref', 'liboptimizer_ref.so')
 pytestmark = pytest.mark.skipif(not os.path.exists(LIB), reason='oracle/_ref/liboptimizer_ref.so not built (reference tree absent)')
@@ -46,45 +47,41 @@ def _same(s, tag):
     return rn, bool(np.array_equal(rT, oT))
 
 
+def _family(*fams):
+    return [(name, s) for fam, name, s in PC.reference_cases() if fam in fams]
+
+
 def test_tracking_like_frames():
     identical = 0
-    for seed in range(1, 25):
-        n, same = _same(S.pose_scenario(seed), ('plain', seed))
+    for name, s in _family('plain'):
+        n, same = _same(s, name)
         assert n > 300
         identical += same
     assert identical >= 20                                  # in practice all of them: both sides round the same double pose to float32
 
 
 def test_hard_frames_rejected_trials_many_outliers_and_noise():
-    for seed in range(30, 42):
-        _same(S.pose_scenario(seed, outlier_frac=0.45, noise=1.5, pose_err=(0.08, 0.3)), ('hard', seed))
-    for seed in range(42, 48):                              # a start far from the optimum: Levenberg rejects trials and raises lambda
-        _same(S.pose_scenario(seed, n=300, outlier_frac=0.3, noise=1.0, pose_err=(0.25, 0.8)), ('far', seed))
+    for name, s in _family('hard', 'far'):                  # 45 % outliers and 1.5 px noise; starts 0.25 rad / 0.8 m away (rejected trials)
+        _same(s, name)
 
 
 def test_monocular_only_and_stereo_only():
-    for seed in (50, 51, 52):
-        _same(S.pose_scenario(seed, mono_frac=1.0), ('mono', seed))
-        _same(S.pose_scenario(seed, mono_frac=0.0), ('stereo', seed))
+    for name, s in _family('mono', 'stereo'):
+        _same(s, name)
 
 
 def test_early_exits():
-    s = S.pose_scenario(5, outlier_frac=0.0, noise=0.2)
-    for k in (0, 1, 2):                                     # fewer than three correspondences: pose untouched, 0 returned (src/Optimizer.cc:338-339)
-        s2 = dict(s); s2['has'] = np.zeros_like(s['has']); s2['has'][:k] = 1
-        n, same = _same(s2, ('few', k))
+    for name, s in _family('few'):                          # fewer than three correspondences: pose untouched, 0 returned (src/Optimizer.cc:338-339)
+        n, same = _same(s, name)
         assert n == 0 and same
-    for k in (3, 4, 6, 9, 10, 11, 14):                      # fewer than ten edges: a single round (:427-428); ten and more: four
-        s3 = dict(s); s3['has'] = np.zeros_like(s['has']); s3['has'][:k] = 1
-        _same(s3, ('edges', k))
-    s4 = S.pose_scenario(7, n=12, outlier_frac=0.5, noise=2.0)           # tiny graphs with outliers
-    s4['has'][:] = 1
-    _same(s4, ('tiny', 7))
+    for name, s in _family('edges', 'tiny'):                # fewer than ten edges: a single round (:427-428); ten and more: four; a tiny graph with outliers
+        _same(s, name)
 
 
 def test_points_behind_the_camera_and_exact_start():
-    s = S.pose_scenario(9)
-    s['xyz'][:40] *= -1                                     # negative depth: huge residuals, flagged in the first round
-    _same(s, ('behind', 9))
-    s = S.pose_scenario(11, outlier_frac=0.0, noise=0.0, pose_err=(0.0, 0.0))   # already at the optimum: tiny gradient, Levenberg's stop rules
-    _same(s, ('exact', 11))
+    for name, s in _family('behind', 'exact'):              # negative depth (flagged in the first round); a start at the optimum (Levenberg's stop rules)
+        _same(s, name)
+
+
+def test_case_set_holds_the_61_reference_frames():
+    assert len(PC.reference_cases()) == 61
