@@ -692,6 +692,55 @@ SGS_API int sgs_tracker_step(sgs_tracker* t, sgs_detector* det, const uint8_t* g
                              const int32_t* last_n, const float* tcw_cur, const float* tcw_last, float th, int mono, int check_orientation,
                              sgs_keypoint* kps_out, uint8_t* desc_out, float* u_right_out, int32_t* counts_out, int32_t* cur_mp_out,
                              int32_t* nmatches_out, sgs_rect* boxes_out, int32_t* nboxes_out, uint8_t* have_out);
+
+/* ------------------------------------------------------------------------------------------------------------------------------
+ * RGB-D frames as the camera delivers them: Tracking::GrabImageRGBD (src/Tracking.cc:206-251) + the RGB-D Frame constructor (src/Frame.cc:129-198)
+ * + TrackWithMotionModel's matcher call (src/Tracking.cc:906-924).  The format block is filled from the sgs_settings the caller loads:
+ *   rgb              Camera.RGB: != 0 -> cvtColor(CV_RGB2GRAY) (byte 0 gets the R weight), 0 -> CV_BGR2GRAY.  Followed literally: a caller that
+ *                    reads BGR files (imread) with a settings file saying RGB: 1 gets what the reference computes on those bytes.
+ *   depth_type       0: uint16 raw depth, 1: float32 (anything else is SGS_ERR_INVALID)
+ *   depth_map_factor mDepthMapFactor (sgs_settings.depth_map_factor): depth = (float)raw * depth_map_factor; finite and > 0
+ *   dist_coef        k1 k2 p1 p2 k3 of Frame::UndistortKeyPoints (k1 == 0: mvKeysUn = mvKeys)
+ * The intrinsics are the handle's sgs_camera (its image bounds come from sgs_image_bounds with the same coefficients).
+ * ------------------------------------------------------------------------------------------------------------------------------ */
+typedef struct sgs_rgbd_format {
+    int32_t rgb;
+    int32_t depth_type;
+    float depth_map_factor;
+    float dist_coef[5];
+} sgs_rgbd_format;
+/* The two conversions alone, on device frames (all pitches and frame strides in bytes):
+ *   gray  [F] = cvtColor(rgb [F], RGB2GRAY / BGR2GRAY) of interleaved 8-bit 3-channel frames: Y = (9798 R + 19235 G + 3735 B + 2^14) >> 15
+ *   depth_out [F] = raw depth [F] converted to float32 metres, (float)raw * depth_map_factor
+ * d_rgb / d_gray may both be NULL (depth only), d_depth / d_depth_out may both be NULL (gray only).  One launch on `stream`. */
+SGS_API int sgs_grab_rgbd_batch_device(const uint8_t* d_rgb, size_t rgb_stride, int rgb_pitch, const void* d_depth, size_t depth_stride, int depth_pitch,
+                                       const sgs_rgbd_format* fmt, int width, int height, int nframes, uint8_t* d_gray, size_t gray_stride, int gray_pitch,
+                                       float* d_depth_out, size_t depth_out_stride, int depth_out_pitch, void* stream);
+/* The whole RGB-D front end on device frames, enqueued on `stream` (NULL: the tracker's stream) without synchronising:
+ *   colour frames -> detector (the tracker's detector stream) -------------------------------------------------------------\
+ *   colour + raw depth -> gray (into the extractor's level 0) + float depth -> ORB extract -> LK -> join -> findFundamentalMat ->
+ *   UndistortKeyPoints -> ComputeStereoFromRGBD (depth at mvKeys, uRight from mvKeysUn.x) -> dyn-reject + ordered compaction of keypoints,
+ *   descriptors, mvKeysUn, mvuRight and mvDepth -> SearchByProjection(cur, last) on mvKeysUn.
+ * d_rgb: interleaved 8-bit frames, d_depth: uint16 or float32 frames (pitches / strides in bytes, multiples of the depth element size); a float32 depth
+ * with factor 1 is read in place.  d_prev_index [F] (device; values in [0, nframes), not checked) and the last-frame arrays are those of
+ * sgs_tracker_lk_device / sgs_tracker_track_device.  The results are those of sgs_tracker_results_device (u_right = mvuRight of the kept keypoints) and
+ * sgs_tracker_frame_device; the next sgs_tracker_pose_chain_device reads mvKeysUn. */
+SGS_API int sgs_tracker_step_rgbd_device(sgs_tracker* t, sgs_detector* det, const uint8_t* d_rgb, size_t rgb_stride, int rgb_pitch, const void* d_depth,
+                                         size_t depth_stride, int depth_pitch, const sgs_rgbd_format* fmt, int nframes, const int32_t* d_prev_index,
+                                         const float* last_xyz, const uint8_t* last_desc, const uint8_t* last_flags, const int32_t* last_octave,
+                                         const float* last_angle, const int32_t* last_n, const float* tcw_cur, const float* tcw_last, float th, int mono,
+                                         int check_orientation, void* stream);
+/* The same step from HOST buffers: each colour frame is uploaded once (detector and gray conversion read the same copy), the raw depth as given;
+ * outputs as sgs_tracker_step plus kps_un_out [F][cap] (mvKeysUn) and depth_out [F][cap] (mvDepth), each of which may be NULL.  Synchronises. */
+SGS_API int sgs_tracker_step_rgbd(sgs_tracker* t, sgs_detector* det, const uint8_t* rgb, size_t rgb_stride, int rgb_pitch, const void* depth,
+                                  size_t depth_stride, int depth_pitch, const sgs_rgbd_format* fmt, int nframes, const int32_t* prev_index,
+                                  const float* last_xyz, const uint8_t* last_desc, const uint8_t* last_flags, const int32_t* last_octave,
+                                  const float* last_angle, const int32_t* last_n, const float* tcw_cur, const float* tcw_last, float th, int mono,
+                                  int check_orientation, sgs_keypoint* kps_out, uint8_t* desc_out, float* u_right_out, int32_t* counts_out,
+                                  int32_t* cur_mp_out, int32_t* nmatches_out, sgs_rect* boxes_out, int32_t* nboxes_out, uint8_t* have_out,
+                                  sgs_keypoint* kps_un_out, float* depth_out);
+/* Device pointers to the compacted mvKeysUn [F][cap] and mvDepth [F][cap] (-1 without depth) of the last RGB-D step; SGS_ERR_INVALID before the first. */
+SGS_API int sgs_tracker_frame_device(const sgs_tracker* t, const sgs_keypoint** d_kps_un, const float** d_depth);
 /* Text listing of the kernel list: one line per kernel with its fused element-wise tail and activation-pool buffers.  SGS_ERR_CAPACITY
  * with *n = bytes required (terminator included) when cap is too small. */
 SGS_API int sgs_detector_describe(const sgs_detector* d, char* out, int64_t cap, int64_t* n);

@@ -4,9 +4,12 @@
 //   sgs_tracker_track   : dyn-reject verdicts + ordered compaction (src/Frame.cc:560-604) followed by
 //                         ORBmatcher::SearchByProjection(cur, last, th, mono) (src/ORBmatcher.cc:1332-1472, called from
 //                         Tracking::TrackWithMotionModel, src/Tracking.cc:924), on the device-resident extraction results.
+//   sgs_tracker_step / sgs_tracker_step_rgbd(_device): the whole front end with the detector on its own stream; the RGB-D step starts from the
+//                         colour and raw depth frames (grab.cu) and adds UndistortKeyPoints + ComputeStereoFromRGBD (one shared body, enqueue_step).
 // One H2D of the frames, one H2D of the per-frame track inputs, one D2H of the compacted results + matches.
 #include <cuda_runtime.h>
 
+#include <cmath>
 #include <cstring>
 #include <memory>
 #include <vector>
@@ -38,9 +41,14 @@ struct sgs_tracker {
     sgs_keypoint* d_kps2 = nullptr; uint8_t* d_desc2 = nullptr; int32_t* d_cnt2 = nullptr; uint8_t* d_keep = nullptr; float* d_uright2 = nullptr;
     int32_t* d_mp = nullptr; int32_t* d_nm = nullptr; unsigned long long* d_ncand = nullptr;
     int last_nframes = 0;
+    const sgs_keypoint* keys_un = nullptr;      // mvKeysUn of the last track call: d_kps2, or d_kpsun2 after an RGB-D step
     // detector inside the step (sgs_tracker_step / sgs_tracker_detect_device): RGB staging, its own stream, the join events
     uint8_t* d_rgb = nullptr; size_t d_rgb_cap = 0; int32_t* d_det_status = nullptr;
     cudaStream_t det_st = nullptr; cudaEvent_t det_ev = nullptr; cudaEvent_t ex_ev = nullptr;
+    cudaEvent_t rgb_ev = nullptr;               // the colour frames of a step are on the device
+    // RGB-D steps, sized on first use: raw depth staging (host entry point), float depth, mvKeysUn / mvDepth before and after the compaction
+    uint8_t* d_depth_raw = nullptr; size_t d_depth_raw_cap = 0; float* d_depthf = nullptr;
+    sgs_keypoint* d_kpsun = nullptr; float* d_dz = nullptr; sgs_keypoint* d_kpsun2 = nullptr; float* d_dz2 = nullptr;
     // sgs_tracker_pose_chain_device: scratch sized on first use for (max_batch, mp_cap)
     int chain_mp_cap = 0;
     Child<sgs_matcher> mt_local{nullptr, sgs_matcher_destroy};
@@ -51,9 +59,12 @@ struct sgs_tracker {
 };
 
 namespace sgs {
-// ordered compaction of the per-keypoint u_right side array with the verdicts of the dyn-reject kernel
+// ordered compaction of the per-keypoint side arrays (u_right; after an RGB-D step also mvKeysUn and mvDepth, kun_in / dz_in may be NULL) with the
+// verdicts of the dyn-reject kernel
 __global__ void compact_uright_kernel(const float* __restrict__ ur_in, const uint8_t* __restrict__ keep, const int32_t* __restrict__ n_in,
-                                      const int32_t* __restrict__ n_out, int cap, float* __restrict__ ur_out, int32_t* __restrict__ mp) {
+                                      const int32_t* __restrict__ n_out, int cap, float* __restrict__ ur_out, int32_t* __restrict__ mp,
+                                      const sgs_keypoint* __restrict__ kun_in, sgs_keypoint* __restrict__ kun_out, const float* __restrict__ dz_in,
+                                      float* __restrict__ dz_out) {
     __shared__ int s_warp[8];
     __shared__ int s_carry;
     const int f = blockIdx.x;
@@ -71,7 +82,11 @@ __global__ void compact_uright_kernel(const float* __restrict__ ur_in, const uin
         __syncthreads();
         int off = s_carry;
         for (int w = 0; w < warp; ++w) off += s_warp[w];
-        if (ok) ur_out[base + off + __popc(m & ((1u << lane) - 1))] = ur_in[base + i];
+        if (ok) {
+            const int64_t o = base + off + __popc(m & ((1u << lane) - 1));
+            ur_out[o] = ur_in[base + i];
+            if (kun_in) { kun_out[o] = kun_in[base + i]; dz_out[o] = dz_in[base + i]; }
+        }
         __syncthreads();
         if (threadIdx.x == 0) { int t = 0; for (int w = 0; w < 8; ++w) t += s_warp[w]; s_carry += t; }
         __syncthreads();
@@ -169,12 +184,13 @@ using namespace sgs;
 namespace {
 int bad(const char* m) { set_error("%s", m); return SGS_ERR_INVALID; }
 
-// the per-frame inputs of the last-frame search, host -> device on `s`
+// the per-frame inputs of the last-frame search, host -> device on `s` (u_right NULL: computed on the device by an RGB-D step)
 int upload_track_inputs(sgs_tracker* t, size_t B, const float* u_right, const float* last_xyz, const uint8_t* last_desc, const uint8_t* last_flags,
                         const int32_t* last_octave, const float* last_angle, const int32_t* last_n, const float* tcw_cur, const float* tcw_last, cudaStream_t s) {
     const size_t K = t->cap, M = t->point_cap;
     auto h2d = [s](void* dst, const void* src, size_t bytes) { return cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, s); };
-    SGS_CUDA_TRY(h2d(t->d_uright_in, u_right, B * K * 4)); SGS_CUDA_TRY(h2d(t->d_lxyz, last_xyz, B * M * 12)); SGS_CUDA_TRY(h2d(t->d_ldesc, last_desc, B * M * 32));
+    if (u_right) SGS_CUDA_TRY(h2d(t->d_uright_in, u_right, B * K * 4));
+    SGS_CUDA_TRY(h2d(t->d_lxyz, last_xyz, B * M * 12)); SGS_CUDA_TRY(h2d(t->d_ldesc, last_desc, B * M * 32));
     SGS_CUDA_TRY(h2d(t->d_lflags, last_flags, B * M)); SGS_CUDA_TRY(h2d(t->d_loct, last_octave, B * M * 4)); SGS_CUDA_TRY(h2d(t->d_lang, last_angle, B * M * 4));
     SGS_CUDA_TRY(h2d(t->d_ln, last_n, B * 4)); SGS_CUDA_TRY(h2d(t->d_tc, tcw_cur, B * 64)); SGS_CUDA_TRY(h2d(t->d_tl, tcw_last, B * 64));
     return SGS_OK;
@@ -188,6 +204,172 @@ int download_track_results(const sgs_tracker* t, size_t B, sgs_keypoint* kps_out
     SGS_CUDA_TRY(d2h(kps_out, t->d_kps2, B * K * sizeof(sgs_keypoint))); SGS_CUDA_TRY(d2h(desc_out, t->d_desc2, B * K * 32)); SGS_CUDA_TRY(d2h(counts_out, t->d_cnt2, B * 4));
     if (u_right_out) SGS_CUDA_TRY(d2h(u_right_out, t->d_uright2, B * K * 4));
     SGS_CUDA_TRY(d2h(cur_mp_out, t->d_mp, B * K * 4)); SGS_CUDA_TRY(d2h(nmatches_out, t->d_nm, B * 4));
+    return SGS_OK;
+}
+
+// dyn-reject + compaction + SearchByProjection(cur, last) on `st` (body of sgs_tracker_track_device).  kun / dz (RGB-D step, else NULL): mvKeysUn and
+// mvDepth of the extracted keypoints, compacted beside them; the search then runs on the compacted mvKeysUn.
+int enqueue_track(sgs_tracker* t, int nframes, const float* prev_xy, const float* u_right, const double* F, const sgs_rect* boxes, const int32_t* nboxes,
+                  const uint8_t* have_dyn, const float* last_xyz, const uint8_t* last_desc, const uint8_t* last_flags, const int32_t* last_octave,
+                  const float* last_angle, const int32_t* last_n, const float* tcw_cur, const float* tcw_last, float th, int mono, int check_orientation,
+                  const sgs_keypoint* kun, const float* dz, cudaStream_t st) {
+    const sgs_keypoint* d_kps; const uint8_t* d_desc; const int32_t* d_cnt; int cap = 0;
+    sgs_extractor_results_device(t->ex.get(), &d_kps, &d_desc, &d_cnt, &cap);
+    int rc = sgs_dynreject_batch_device(d_kps, d_desc, d_cnt, cap, nframes, prev_xy, F, boxes, nboxes, t->max_boxes, have_dyn,
+                                        t->nfeatures, t->d_kps2, t->d_desc2, t->d_cnt2, t->d_keep, st);
+    if (rc != SGS_OK) return rc;
+    compact_uright_kernel<<<nframes, 256, 0, st>>>(u_right, t->d_keep, d_cnt, t->d_cnt2, cap, t->d_uright2, t->d_mp, kun, t->d_kpsun2, dz, t->d_dz2);
+    t->keys_un = kun ? t->d_kpsun2 : t->d_kps2;
+    SGS_CUDA_TRY(cudaMemsetAsync(t->d_ncand, 0, (size_t)nframes * 8, st));
+    sgs_lastframe_batch a;
+    std::memset(&a, 0, sizeof a);
+    a.cam = t->cam;
+    a.cur_kps = t->keys_un; a.cur_desc = t->d_desc2; a.cur_uright = t->d_uright2; a.cur_n = t->d_cnt2;
+    a.last_xyz = last_xyz; a.last_desc = last_desc; a.last_flags = last_flags; a.last_octave = last_octave; a.last_angle = last_angle; a.last_n = last_n;
+    a.tcw_cur = tcw_cur; a.tcw_last = tcw_last; a.th = th; a.mono = mono; a.check_orientation = check_orientation;
+    a.cur_mp = t->d_mp; a.cur_mp_obs_in = nullptr; a.nmatches = t->d_nm; a.ncand = (uint64_t*)t->d_ncand;
+    return sgs_match_project_lastframe_batch_device(t->mt.get(), &a, nframes, st);
+}
+
+// device buffers of the RGB-D steps, sized for max_batch frames on first use (raw_bytes: one raw depth frame, staged by the host entry point)
+int ensure_rgbd_buffers(sgs_tracker* t, size_t raw_bytes) {
+    HandleResources& R = t->res;
+    const size_t B = t->max_batch, K = t->cap, px = (size_t)t->width * t->height;
+    if (!t->d_kpsun2) {     // allocated last: a failed first attempt is repeated whole by the next call
+        SGS_CUDA_TRY(R.regrow(&t->d_depthf, B * px * 4 + 16)); SGS_CUDA_TRY(R.regrow(&t->d_kpsun, B * K * sizeof(sgs_keypoint) + 16));
+        SGS_CUDA_TRY(R.regrow(&t->d_dz, B * K * 4 + 16)); SGS_CUDA_TRY(R.regrow(&t->d_dz2, B * K * 4 + 16)); SGS_CUDA_TRY(R.regrow(&t->d_kpsun2, B * K * sizeof(sgs_keypoint) + 16));
+    }
+    if (t->d_depth_raw_cap < raw_bytes * B) {
+        t->d_depth_raw_cap = 0;
+        SGS_CUDA_TRY(R.regrow(&t->d_depth_raw, raw_bytes * B));
+        t->d_depth_raw_cap = raw_bytes * B;
+    }
+    return SGS_OK;
+}
+
+// colour frames host -> the tracker's dense staging buffer (pitch width * 3) on the detector stream
+int upload_rgb(sgs_tracker* t, const uint8_t* rgb, size_t rgb_stride, int rgb_pitch, size_t B) {
+    const size_t rgb_bytes = (size_t)t->width * 3 * t->height;
+    if (t->d_rgb_cap < rgb_bytes * (size_t)t->max_batch) {
+        t->d_rgb_cap = 0;
+        SGS_CUDA_TRY(t->res.regrow(&t->d_rgb, rgb_bytes * (size_t)t->max_batch));
+        t->d_rgb_cap = rgb_bytes * (size_t)t->max_batch;
+    }
+    if (rgb_stride == (size_t)rgb_pitch * t->height) {
+        SGS_CUDA_TRY(cudaMemcpy2DAsync(t->d_rgb, (size_t)t->width * 3, rgb, rgb_pitch, (size_t)t->width * 3, (size_t)t->height * B, cudaMemcpyHostToDevice, t->det_st));
+    } else {
+        for (size_t f = 0; f < B; ++f)
+            SGS_CUDA_TRY(cudaMemcpy2DAsync(t->d_rgb + f * rgb_bytes, (size_t)t->width * 3, rgb + f * rgb_stride, rgb_pitch, (size_t)t->width * 3, t->height, cudaMemcpyHostToDevice, t->det_st));
+    }
+    return SGS_OK;
+}
+
+// Where the frames of a step come from.  The colour frames are on the device (ready in the order of rgb_st).  The gray frames either come from host
+// memory (sgs_tracker_step) or, with gray == NULL, are converted from the colour frames together with the raw depth (RGB-D steps).
+struct StepFrames {
+    const uint8_t* d_rgb; size_t rgb_stride; int rgb_pitch; cudaStream_t rgb_st;
+    const uint8_t* gray; size_t gray_stride; int gray_pitch;
+    const void* d_depth; size_t depth_stride; int depth_pitch; const sgs_rgbd_format* fmt;
+};
+// The per-frame inputs of the search: host pointers, uploaded on the copy stream while the kernels run, or device pointers.  u_right: the step's
+// host input (sgs_tracker_step); NULL in RGB-D steps, which compute it.
+struct StepInputs {
+    bool host; const int32_t* prev_index; const float* u_right;
+    const float* last_xyz; const uint8_t* last_desc; const uint8_t* last_flags; const int32_t* last_octave; const float* last_angle; const int32_t* last_n;
+    const float* tcw_cur; const float* tcw_last;
+};
+
+// The stream and event choreography of every step: the detector on its own stream beside extract -> LK on `st`, joined before findFundamentalMat;
+// an RGB-D step converts gray and depth on `st` and adds UndistortKeyPoints + ComputeStereoFromRGBD before the rejection.
+int enqueue_step(sgs_tracker* t, sgs_detector* det, const StepFrames& fr, int nframes, const StepInputs& in, float th, int mono, int check_orientation,
+                 cudaStream_t st) {
+    const size_t B = nframes;
+    const bool rgbd = fr.gray == nullptr;
+    // ---- detector branch: network on the colour frames, boxes into the tracker's arrays
+    if (fr.rgb_st != t->det_st || (rgbd && fr.rgb_st != st)) SGS_CUDA_TRY(cudaEventRecord(t->rgb_ev, fr.rgb_st));
+    if (fr.rgb_st != t->det_st) SGS_CUDA_TRY(cudaStreamWaitEvent(t->det_st, t->rgb_ev, 0));
+    int rc = sgs_tracker_detect_device(t, det, fr.d_rgb, (int64_t)fr.rgb_stride, fr.rgb_pitch, t->width, t->height, nframes, t->det_st);
+    if (rc != SGS_OK) return rc;
+    SGS_CUDA_TRY(cudaEventRecord(t->det_ev, t->det_st));
+    // ---- tracking branch: gray frames into the extractor's level 0 + ORB extraction, then LK on `st`
+    const uint8_t* d_frames; int pitch; size_t fstride;
+    sgs_extractor_level0_device(t->ex.get(), &d_frames, &pitch, &fstride);
+    const float* depth = nullptr; size_t depth_fstride = 0; int depth_pitch = 0;      // float depth, in elements
+    if (!rgbd) {
+        rc = sgs_extract_batch(t->ex.get(), fr.gray, nframes, fr.gray_stride, fr.gray_pitch, nullptr, nullptr, 0, nullptr);
+        if (rc != SGS_OK) return rc;
+        SGS_CUDA_TRY(cudaEventRecord(t->ex_ev, (cudaStream_t)sgs_extractor_stream(t->ex.get())));
+        SGS_CUDA_TRY(cudaStreamWaitEvent(st, t->ex_ev, 0));
+    } else {
+        if (fr.rgb_st != st) SGS_CUDA_TRY(cudaStreamWaitEvent(st, t->rgb_ev, 0));
+        const sgs_rgbd_format& fm = *fr.fmt;
+        const bool in_place = fm.depth_type == 1 && fm.depth_map_factor == 1.0f;      // Tracking.cc:229-230 converts iff factor != 1 or not CV_32F
+        const size_t wpitch = (size_t)t->width * 4;
+        rc = sgs_grab_rgbd_batch_device(fr.d_rgb, fr.rgb_stride, fr.rgb_pitch, in_place ? nullptr : fr.d_depth, fr.depth_stride, fr.depth_pitch, &fm, t->width,
+                                        t->height, nframes, const_cast<uint8_t*>(d_frames), fstride, pitch, in_place ? nullptr : t->d_depthf,
+                                        wpitch * t->height, (int)wpitch, st);
+        if (rc != SGS_OK) return rc;
+        if (in_place) { depth = (const float*)fr.d_depth; depth_fstride = fr.depth_stride / 4; depth_pitch = fr.depth_pitch / 4; }
+        else { depth = t->d_depthf; depth_fstride = (size_t)t->width * t->height; depth_pitch = t->width; }
+        rc = sgs_extract_batch_device(t->ex.get(), d_frames, nframes, fstride, pitch, st);
+        if (rc != SGS_OK) return rc;
+    }
+    t->last_nframes = nframes;
+    const int32_t* d_pidx = in.prev_index;
+    const float *lxyz = in.last_xyz, *lang = in.last_angle, *tc = in.tcw_cur, *tl = in.tcw_last;
+    const uint8_t *ldesc = in.last_desc, *lfl = in.last_flags;
+    const int32_t *loct = in.last_octave, *ln = in.last_n;
+    if (in.host) {
+        SGS_CUDA_TRY(cudaMemcpyAsync(t->d_pidx, in.prev_index, sizeof(int32_t) * B, cudaMemcpyHostToDevice, st));
+        rc = upload_track_inputs(t, B, in.u_right, in.last_xyz, in.last_desc, in.last_flags, in.last_octave, in.last_angle, in.last_n, in.tcw_cur, in.tcw_last, t->copy_st);
+        if (rc != SGS_OK) return rc;
+        SGS_CUDA_TRY(cudaEventRecord(t->copy_ev, t->copy_st));
+        d_pidx = t->d_pidx;
+        lxyz = t->d_lxyz; ldesc = t->d_ldesc; lfl = t->d_lflags; loct = t->d_loct; lang = t->d_lang; ln = t->d_ln; tc = t->d_tc; tl = t->d_tl;
+    }
+    rc = sgs_tracker_lk_device(t, d_frames, nframes, fstride, pitch, d_pidx, st);
+    if (rc != SGS_OK) return rc;
+    SGS_CUDA_TRY(cudaStreamWaitEvent(st, t->det_ev, 0));                  // the join of src/Frame.cc:478-481: boxes of every frame of the batch are there
+    rc = sgs_tracker_fundamental_device(t, nframes, nullptr, nullptr, nullptr, d_pidx, st);
+    if (rc != SGS_OK) return rc;
+    if (rgbd) {     // Frame.cc:146-174 undistorts and looks the depth up after the rejection; both are per point, so doing them first gives the same values
+        const sgs_keypoint* d_kps; const int32_t* d_cnt; int cap = 0;
+        sgs_extractor_results_device(t->ex.get(), &d_kps, nullptr, &d_cnt, &cap);
+        rc = sgs_undistort_batch_device(d_kps, d_cnt, cap, nframes, t->cam.fx, t->cam.fy, t->cam.cx, t->cam.cy, fr.fmt->dist_coef, t->d_kpsun, st);
+        if (rc != SGS_OK) return rc;
+        rc = sgs_stereo_from_depth_batch_device(d_kps, t->d_kpsun, d_cnt, cap, nframes, depth, depth_fstride, depth_pitch, t->cam.bf, t->d_uright_in, t->d_dz, st);
+        if (rc != SGS_OK) return rc;
+    }
+    if (in.host) SGS_CUDA_TRY(cudaStreamWaitEvent(st, t->copy_ev, 0));
+    return enqueue_track(t, nframes, t->d_prev, t->d_uright_in, t->d_Fgpu, t->d_boxes, t->d_nboxes, t->d_have, lxyz, ldesc, lfl,
+                         loct, lang, ln, tc, tl, th, mono, check_orientation, rgbd ? t->d_kpsun : nullptr, rgbd ? t->d_dz : nullptr, st);
+}
+
+// the outputs of a step, device -> host on the tracker's stream, then the one synchronisation of the call (every pointer but the first six may be NULL)
+int download_step(sgs_tracker* t, size_t B, sgs_keypoint* kps_out, uint8_t* desc_out, float* u_right_out, int32_t* counts_out, int32_t* cur_mp_out,
+                  int32_t* nmatches_out, sgs_rect* boxes_out, int32_t* nboxes_out, uint8_t* have_out, sgs_keypoint* kps_un_out, float* depth_out) {
+    cudaStream_t st = t->st;
+    int rc = download_track_results(t, B, kps_out, desc_out, u_right_out, counts_out, cur_mp_out, nmatches_out, st);
+    if (rc != SGS_OK) return rc;
+    if (boxes_out) SGS_CUDA_TRY(cudaMemcpyAsync(boxes_out, t->d_boxes, B * t->max_boxes * sizeof(sgs_rect), cudaMemcpyDeviceToHost, st));
+    if (nboxes_out) SGS_CUDA_TRY(cudaMemcpyAsync(nboxes_out, t->d_nboxes, B * 4, cudaMemcpyDeviceToHost, st));
+    if (have_out) SGS_CUDA_TRY(cudaMemcpyAsync(have_out, t->d_have, B, cudaMemcpyDeviceToHost, st));
+    if (kps_un_out) SGS_CUDA_TRY(cudaMemcpyAsync(kps_un_out, t->d_kpsun2, B * t->cap * sizeof(sgs_keypoint), cudaMemcpyDeviceToHost, st));
+    if (depth_out) SGS_CUDA_TRY(cudaMemcpyAsync(depth_out, t->d_dz2, B * t->cap * 4, cudaMemcpyDeviceToHost, st));
+    SGS_CUDA_TRY(cudaStreamSynchronize(st));
+    return SGS_OK;
+}
+
+// argument checks shared by the two RGB-D steps, before anything is enqueued (byte pitches and frame strides)
+int check_rgbd_args(const sgs_tracker* t, const char* fn, const sgs_rgbd_format* fmt, int nframes, size_t rgb_stride, int rgb_pitch, size_t depth_stride,
+                    int depth_pitch, const void* depth) {
+    if (nframes < 1 || nframes > t->max_batch) { set_error("%s: nframes outside [1,max_batch]", fn); return SGS_ERR_INVALID; }
+    if (fmt->depth_type != 0 && fmt->depth_type != 1) { set_error("%s: depth_type is neither 0 (uint16) nor 1 (float32)", fn); return SGS_ERR_INVALID; }
+    if (!std::isfinite(fmt->depth_map_factor) || !(fmt->depth_map_factor > 0.f)) { set_error("%s: depth_map_factor is not a finite positive number", fn); return SGS_ERR_INVALID; }
+    const size_t esz = fmt->depth_type == 0 ? 2 : 4;
+    if (rgb_pitch < t->width * 3 || rgb_stride < (size_t)rgb_pitch * t->height) { set_error("%s: rgb pitch / stride too small", fn); return SGS_ERR_INVALID; }
+    if ((size_t)depth_pitch < esz * t->width || depth_stride < (size_t)depth_pitch * t->height) { set_error("%s: depth pitch / stride too small", fn); return SGS_ERR_INVALID; }
+    if (depth_pitch % esz || depth_stride % esz || (uintptr_t)depth % esz) { set_error("%s: depth pitch, stride or pointer not a multiple of the element size", fn); return SGS_ERR_INVALID; }
     return SGS_OK;
 }
 }  // namespace
@@ -223,6 +405,7 @@ SGS_API int sgs_tracker_create(const sgs_orb_params* params, int width, int heig
     const size_t B = max_batch, K = t->cap, M = point_cap;
     SGS_CUDA_TRY_AT(fn, R.stream(&t->st)); SGS_CUDA_TRY_AT(fn, R.stream(&t->copy_st)); SGS_CUDA_TRY_AT(fn, R.event(&t->copy_ev, cudaEventDisableTiming));
     SGS_CUDA_TRY_AT(fn, R.stream(&t->det_st)); SGS_CUDA_TRY_AT(fn, R.event(&t->det_ev, cudaEventDisableTiming)); SGS_CUDA_TRY_AT(fn, R.event(&t->ex_ev, cudaEventDisableTiming));
+    SGS_CUDA_TRY_AT(fn, R.event(&t->rgb_ev, cudaEventDisableTiming));
     // every array below has 16 bytes of slack past its end
     SGS_CUDA_TRY_AT(fn, R.alloc(&t->d_prev, B * K * 8 + 16)); SGS_CUDA_TRY_AT(fn, R.alloc(&t->d_uright_in, B * K * 4 + 16)); SGS_CUDA_TRY_AT(fn, R.alloc(&t->d_F, B * 72 + 16));
     SGS_CUDA_TRY_AT(fn, R.alloc(&t->d_boxes, B * t->max_boxes * sizeof(sgs_rect) + 16)); SGS_CUDA_TRY_AT(fn, R.alloc(&t->d_nboxes, B * 4 + 16)); SGS_CUDA_TRY_AT(fn, R.alloc(&t->d_have, B + 16));
@@ -233,6 +416,7 @@ SGS_API int sgs_tracker_create(const sgs_orb_params* params, int width, int heig
     SGS_CUDA_TRY_AT(fn, R.alloc(&t->d_uright2, B * K * 4 + 16)); SGS_CUDA_TRY_AT(fn, R.alloc(&t->d_mp, B * K * 4 + 16)); SGS_CUDA_TRY_AT(fn, R.alloc(&t->d_nm, B * 4 + 16));
     SGS_CUDA_TRY_AT(fn, R.alloc(&t->d_ncand, B * 8 + 16)); SGS_CUDA_TRY_AT(fn, R.alloc(&t->d_Fgpu, B * 72 + 16)); SGS_CUDA_TRY_AT(fn, R.alloc(&t->d_finfo, B * 16 + 16));
     SGS_CUDA_TRY_AT(fn, R.alloc(&t->d_det_status, B * 4 + 16));
+    t->keys_un = t->d_kps2;
     *out = t.release();
     return SGS_OK;
 }
@@ -271,22 +455,8 @@ SGS_API int sgs_tracker_track_device(sgs_tracker* t, int nframes, const float* p
     if (!F) F = t->d_Fgpu;                  // filled by sgs_tracker_fundamental_device
     if (nframes < 1 || nframes > t->last_nframes) return bad("sgs_tracker_track_device: nframes exceeds the last extract call");
     if (!prev_xy) prev_xy = t->d_prev;      // filled by sgs_tracker_lk_device
-    cudaStream_t st = stream ? (cudaStream_t)stream : t->st;
-    const sgs_keypoint* d_kps; const uint8_t* d_desc; const int32_t* d_cnt; int cap = 0;
-    sgs_extractor_results_device(t->ex.get(), &d_kps, &d_desc, &d_cnt, &cap);
-    int rc = sgs_dynreject_batch_device(d_kps, d_desc, d_cnt, cap, nframes, prev_xy, F, boxes ? boxes : t->d_boxes, nboxes, t->max_boxes, have_dyn,
-                                        t->nfeatures, t->d_kps2, t->d_desc2, t->d_cnt2, t->d_keep, st);
-    if (rc != SGS_OK) return rc;
-    compact_uright_kernel<<<nframes, 256, 0, st>>>(u_right, t->d_keep, d_cnt, t->d_cnt2, cap, t->d_uright2, t->d_mp);
-    SGS_CUDA_TRY(cudaMemsetAsync(t->d_ncand, 0, (size_t)nframes * 8, st));
-    sgs_lastframe_batch a;
-    std::memset(&a, 0, sizeof a);
-    a.cam = t->cam;
-    a.cur_kps = t->d_kps2; a.cur_desc = t->d_desc2; a.cur_uright = t->d_uright2; a.cur_n = t->d_cnt2;
-    a.last_xyz = last_xyz; a.last_desc = last_desc; a.last_flags = last_flags; a.last_octave = last_octave; a.last_angle = last_angle; a.last_n = last_n;
-    a.tcw_cur = tcw_cur; a.tcw_last = tcw_last; a.th = th; a.mono = mono; a.check_orientation = check_orientation;
-    a.cur_mp = t->d_mp; a.cur_mp_obs_in = nullptr; a.nmatches = t->d_nm; a.ncand = (uint64_t*)t->d_ncand;
-    return sgs_match_project_lastframe_batch_device(t->mt.get(), &a, nframes, st);
+    return enqueue_track(t, nframes, prev_xy, u_right, F, boxes ? boxes : t->d_boxes, nboxes, have_dyn, last_xyz, last_desc, last_flags, last_octave, last_angle,
+                         last_n, tcw_cur, tcw_last, th, mono, check_orientation, nullptr, nullptr, stream ? (cudaStream_t)stream : t->st);
 }
 
 // device pointers to the results of the last track call: kps [B][cap], desc, u_right, counts [B], cur_mp [B][cap], nmatches [B], ncand [B]
@@ -450,7 +620,7 @@ SGS_API int sgs_tracker_pose_chain_device(sgs_tracker* t, const sgs_posechain_ba
     sgs_lastframe_batch lf;
     std::memset(&lf, 0, sizeof lf);
     lf.cam = t->cam;
-    lf.cur_kps = t->d_kps2; lf.cur_desc = t->d_desc2; lf.cur_uright = t->d_uright2; lf.cur_n = t->d_cnt2;
+    lf.cur_kps = t->keys_un; lf.cur_desc = t->d_desc2; lf.cur_uright = t->d_uright2; lf.cur_n = t->d_cnt2;
     lf.last_xyz = a->last_xyz; lf.last_desc = a->last_desc; lf.last_flags = a->last_flags; lf.last_octave = a->last_octave; lf.last_angle = a->last_angle; lf.last_n = a->last_n;
     lf.tcw_cur = a->tcw_cur; lf.tcw_last = a->tcw_last; lf.th = 2.f * a->th; lf.mono = a->mono; lf.check_orientation = a->check_orientation;
     lf.cur_mp = t->d_mp; lf.nmatches = t->d_nm2; lf.ncand = (uint64_t*)t->d_ncand2; lf.frame_enable = t->d_enable;
@@ -463,7 +633,7 @@ SGS_API int sgs_tracker_pose_chain_device(sgs_tracker* t, const sgs_posechain_ba
     SGS_CUDA_TRY(cudaMemsetAsync(a->outlier, 0, (size_t)F * cap, st));
     sgs_poseopt_batch po;
     std::memset(&po, 0, sizeof po);
-    po.cam = t->cam; po.tcw_in = a->tcw_cur; po.kps = t->d_kps2; po.uright = t->d_uright2; po.n = t->d_cnt2; po.cap = cap;
+    po.cam = t->cam; po.tcw_in = a->tcw_cur; po.kps = t->keys_un; po.uright = t->d_uright2; po.n = t->d_cnt2; po.cap = cap;
     po.mp_index = t->d_mp; po.points_xyz = a->last_xyz; po.point_cap = t->point_cap;
     for (int l = 0; l < 16; ++l) po.inv_level_sigma2[l] = a->inv_level_sigma2[l];
     po.tcw_out = a->tcw_motion; po.outlier = a->outlier; po.ninliers = t->d_ninl; po.scratch_err = t->d_po_err; po.scratch_level = t->d_po_level;
@@ -483,7 +653,7 @@ SGS_API int sgs_tracker_pose_chain_device(sgs_tracker* t, const sgs_posechain_ba
     chain_mask_kernel<<<F, 256, 0, st>>>(a->mp_n, a->mp_cap, a->mp_valid, t->d_seen, t->d_inview, a->stats);
     sgs_localmap_batch lm;
     std::memset(&lm, 0, sizeof lm);
-    lm.cam = t->cam; lm.cur_kps = t->d_kps2; lm.cur_desc = t->d_desc2; lm.cur_uright = t->d_uright2; lm.cur_n = t->d_cnt2;
+    lm.cam = t->cam; lm.cur_kps = t->keys_un; lm.cur_desc = t->d_desc2; lm.cur_uright = t->d_uright2; lm.cur_n = t->d_cnt2;
     lm.mp_inview = t->d_inview; lm.proj_x = t->d_projx; lm.proj_y = t->d_projy; lm.proj_xr = t->d_projxr; lm.level = t->d_level; lm.view_cos = t->d_viewcos;
     lm.mp_desc = a->mp_desc; lm.mp_obs = a->mp_obs; lm.mp_n = a->mp_n; lm.th = a->th_local; lm.nnratio = a->nnratio_local; lm.id_base = t->point_cap;
     lm.f_mp = t->d_mp; lm.f_mp_obs = t->d_obs; lm.nmatches = t->d_nml; lm.ncand = (uint64_t*)t->d_ncand2;
@@ -535,50 +705,74 @@ SGS_API int sgs_tracker_step(sgs_tracker* t, sgs_detector* det, const uint8_t* g
     for (int f = 0; f < nframes; ++f) if (prev_index[f] < 0 || prev_index[f] >= nframes) return bad("sgs_tracker_step: prev_index out of range");
     SGS_CUDA_TRY(cudaSetDevice(t->device));
     const size_t B = nframes;
-    // ---- detector branch: colour frames up, network, boxes into the tracker's arrays
-    const size_t rgb_bytes = (size_t)t->width * 3 * t->height;
-    if (t->d_rgb_cap < rgb_bytes * (size_t)t->max_batch) {
-        t->d_rgb_cap = 0;
-        SGS_CUDA_TRY(t->res.regrow(&t->d_rgb, rgb_bytes * (size_t)t->max_batch));
-        t->d_rgb_cap = rgb_bytes * (size_t)t->max_batch;
-    }
-    if (rgb_stride == (size_t)rgb_pitch * t->height) {
-        SGS_CUDA_TRY(cudaMemcpy2DAsync(t->d_rgb, (size_t)t->width * 3, rgb, rgb_pitch, (size_t)t->width * 3, (size_t)t->height * B, cudaMemcpyHostToDevice, t->det_st));
+    int rc = upload_rgb(t, rgb, rgb_stride, rgb_pitch, B);
+    if (rc != SGS_OK) return rc;
+    const StepFrames fr{t->d_rgb, (size_t)t->width * 3 * t->height, t->width * 3, t->det_st, gray, gray_stride, gray_pitch, nullptr, 0, 0, nullptr};
+    const StepInputs in{true, prev_index, u_right, last_xyz, last_desc, last_flags, last_octave, last_angle, last_n, tcw_cur, tcw_last};
+    rc = enqueue_step(t, det, fr, nframes, in, th, mono, check_orientation, t->st);
+    if (rc != SGS_OK) return rc;
+    return download_step(t, B, kps_out, desc_out, u_right_out, counts_out, cur_mp_out, nmatches_out, boxes_out, nboxes_out, have_out, nullptr, nullptr);
+}
+
+// The RGB-D front end (Tracking::GrabImageRGBD + the RGB-D Frame constructor + the first matcher call) on device frames; see sgs_abi.h.
+SGS_API int sgs_tracker_step_rgbd_device(sgs_tracker* t, sgs_detector* det, const uint8_t* d_rgb, size_t rgb_stride, int rgb_pitch, const void* d_depth,
+                                         size_t depth_stride, int depth_pitch, const sgs_rgbd_format* fmt, int nframes, const int32_t* d_prev_index,
+                                         const float* last_xyz, const uint8_t* last_desc, const uint8_t* last_flags, const int32_t* last_octave,
+                                         const float* last_angle, const int32_t* last_n, const float* tcw_cur, const float* tcw_last, float th, int mono,
+                                         int check_orientation, void* stream) {
+    const char* const fn = "sgs_tracker_step_rgbd_device";
+    if (!t || !det || !d_rgb || !d_depth || !fmt || !d_prev_index || !last_xyz || !last_desc || !last_flags || !last_octave || !last_angle || !last_n ||
+        !tcw_cur || !tcw_last) return bad("sgs_tracker_step_rgbd_device: NULL argument");
+    int rc = check_rgbd_args(t, fn, fmt, nframes, rgb_stride, rgb_pitch, depth_stride, depth_pitch, d_depth);
+    if (rc != SGS_OK) return rc;
+    SGS_CUDA_TRY(cudaSetDevice(t->device));
+    rc = ensure_rgbd_buffers(t, 0);
+    if (rc != SGS_OK) return rc;
+    cudaStream_t st = stream ? (cudaStream_t)stream : t->st;
+    const StepFrames fr{d_rgb, rgb_stride, rgb_pitch, st, nullptr, 0, 0, d_depth, depth_stride, depth_pitch, fmt};
+    const StepInputs in{false, d_prev_index, nullptr, last_xyz, last_desc, last_flags, last_octave, last_angle, last_n, tcw_cur, tcw_last};
+    return enqueue_step(t, det, fr, nframes, in, th, mono, check_orientation, st);
+}
+
+// The same from host buffers: one upload of the colour frames (detector and gray conversion read it), the raw depth as given, one synchronisation.
+SGS_API int sgs_tracker_step_rgbd(sgs_tracker* t, sgs_detector* det, const uint8_t* rgb, size_t rgb_stride, int rgb_pitch, const void* depth,
+                                  size_t depth_stride, int depth_pitch, const sgs_rgbd_format* fmt, int nframes, const int32_t* prev_index,
+                                  const float* last_xyz, const uint8_t* last_desc, const uint8_t* last_flags, const int32_t* last_octave,
+                                  const float* last_angle, const int32_t* last_n, const float* tcw_cur, const float* tcw_last, float th, int mono,
+                                  int check_orientation, sgs_keypoint* kps_out, uint8_t* desc_out, float* u_right_out, int32_t* counts_out,
+                                  int32_t* cur_mp_out, int32_t* nmatches_out, sgs_rect* boxes_out, int32_t* nboxes_out, uint8_t* have_out,
+                                  sgs_keypoint* kps_un_out, float* depth_out) {
+    const char* const fn = "sgs_tracker_step_rgbd";
+    if (!t || !det || !rgb || !depth || !fmt || !prev_index || !last_xyz || !last_desc || !last_flags || !last_octave || !last_angle || !last_n || !tcw_cur ||
+        !tcw_last || !kps_out || !desc_out || !counts_out || !cur_mp_out || !nmatches_out) return bad("sgs_tracker_step_rgbd: NULL argument");
+    int rc = check_rgbd_args(t, fn, fmt, nframes, rgb_stride, rgb_pitch, depth_stride, depth_pitch, depth);
+    if (rc != SGS_OK) return rc;
+    for (int f = 0; f < nframes; ++f) if (prev_index[f] < 0 || prev_index[f] >= nframes) return bad("sgs_tracker_step_rgbd: prev_index out of range");
+    SGS_CUDA_TRY(cudaSetDevice(t->device));
+    const size_t B = nframes, row = (size_t)t->width * (fmt->depth_type == 0 ? 2 : 4);
+    rc = ensure_rgbd_buffers(t, row * t->height);
+    if (rc != SGS_OK) return rc;
+    rc = upload_rgb(t, rgb, rgb_stride, rgb_pitch, B);
+    if (rc != SGS_OK) return rc;
+    if (depth_stride == (size_t)depth_pitch * t->height) {
+        SGS_CUDA_TRY(cudaMemcpy2DAsync(t->d_depth_raw, row, depth, depth_pitch, row, (size_t)t->height * B, cudaMemcpyHostToDevice, t->st));
     } else {
         for (size_t f = 0; f < B; ++f)
-            SGS_CUDA_TRY(cudaMemcpy2DAsync(t->d_rgb + f * rgb_bytes, (size_t)t->width * 3, rgb + f * rgb_stride, rgb_pitch, (size_t)t->width * 3, t->height, cudaMemcpyHostToDevice, t->det_st));
+            SGS_CUDA_TRY(cudaMemcpy2DAsync(t->d_depth_raw + f * row * t->height, row, (const uint8_t*)depth + f * depth_stride, depth_pitch, row, t->height,
+                                           cudaMemcpyHostToDevice, t->st));
     }
-    int rc = sgs_tracker_detect_device(t, det, t->d_rgb, (int64_t)rgb_bytes, t->width * 3, t->width, t->height, nframes, t->det_st);
+    const StepFrames fr{t->d_rgb, (size_t)t->width * 3 * t->height, t->width * 3, t->det_st, nullptr, 0, 0, t->d_depth_raw, row * t->height, (int)row, fmt};
+    const StepInputs in{true, prev_index, nullptr, last_xyz, last_desc, last_flags, last_octave, last_angle, last_n, tcw_cur, tcw_last};
+    rc = enqueue_step(t, det, fr, nframes, in, th, mono, check_orientation, t->st);
     if (rc != SGS_OK) return rc;
-    SGS_CUDA_TRY(cudaEventRecord(t->det_ev, t->det_st));
-    // ---- tracking branch: gray frames up + ORB extraction (the extractor's streams), then LK on the tracker's stream
-    rc = sgs_extract_batch(t->ex.get(), gray, nframes, gray_stride, gray_pitch, nullptr, nullptr, 0, nullptr);
-    if (rc != SGS_OK) return rc;
-    t->last_nframes = nframes;
-    cudaStream_t st = t->st;
-    SGS_CUDA_TRY(cudaEventRecord(t->ex_ev, (cudaStream_t)sgs_extractor_stream(t->ex.get())));
-    SGS_CUDA_TRY(cudaStreamWaitEvent(st, t->ex_ev, 0));
-    SGS_CUDA_TRY(cudaMemcpyAsync(t->d_pidx, prev_index, sizeof(int32_t) * B, cudaMemcpyHostToDevice, st));
-    rc = upload_track_inputs(t, B, u_right, last_xyz, last_desc, last_flags, last_octave, last_angle, last_n, tcw_cur, tcw_last, t->copy_st);
-    if (rc != SGS_OK) return rc;
-    SGS_CUDA_TRY(cudaEventRecord(t->copy_ev, t->copy_st));
-    const uint8_t* d_frames; int pitch; size_t fstride;
-    sgs_extractor_level0_device(t->ex.get(), &d_frames, &pitch, &fstride);
-    rc = sgs_tracker_lk_device(t, d_frames, nframes, fstride, pitch, t->d_pidx, st);
-    if (rc != SGS_OK) return rc;
-    SGS_CUDA_TRY(cudaStreamWaitEvent(st, t->det_ev, 0));                  // the join of src/Frame.cc:478-481: boxes of every frame of the batch are there
-    rc = sgs_tracker_fundamental_device(t, nframes, nullptr, nullptr, nullptr, t->d_pidx, st);
-    if (rc != SGS_OK) return rc;
-    SGS_CUDA_TRY(cudaStreamWaitEvent(st, t->copy_ev, 0));
-    rc = sgs_tracker_track_device(t, nframes, nullptr, t->d_uright_in, nullptr, nullptr, nullptr, nullptr, t->d_lxyz, t->d_ldesc, t->d_lflags, t->d_loct, t->d_lang, t->d_ln,
-                                  t->d_tc, t->d_tl, th, mono, check_orientation, st);
-    if (rc != SGS_OK) return rc;
-    rc = download_track_results(t, B, kps_out, desc_out, u_right_out, counts_out, cur_mp_out, nmatches_out, st);
-    if (rc != SGS_OK) return rc;
-    if (boxes_out) SGS_CUDA_TRY(cudaMemcpyAsync(boxes_out, t->d_boxes, B * t->max_boxes * sizeof(sgs_rect), cudaMemcpyDeviceToHost, st));
-    if (nboxes_out) SGS_CUDA_TRY(cudaMemcpyAsync(nboxes_out, t->d_nboxes, B * 4, cudaMemcpyDeviceToHost, st));
-    if (have_out) SGS_CUDA_TRY(cudaMemcpyAsync(have_out, t->d_have, B, cudaMemcpyDeviceToHost, st));
-    SGS_CUDA_TRY(cudaStreamSynchronize(st));
+    return download_step(t, B, kps_out, desc_out, u_right_out, counts_out, cur_mp_out, nmatches_out, boxes_out, nboxes_out, have_out, kps_un_out, depth_out);
+}
+
+SGS_API int sgs_tracker_frame_device(const sgs_tracker* t, const sgs_keypoint** d_kps_un, const float** d_depth) {
+    if (!t) return bad("sgs_tracker_frame_device: NULL handle");
+    if (!t->d_kpsun2) return bad("sgs_tracker_frame_device: no RGB-D step has run on this handle");
+    if (d_kps_un) *d_kps_un = t->d_kpsun2;
+    if (d_depth) *d_depth = t->d_dz2;
     return SGS_OK;
 }
 

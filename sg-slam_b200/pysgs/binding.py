@@ -40,6 +40,21 @@ class Settings(C.Structure):
                 ('dynamic_detection_confidence_threshold', C.c_float)]
 
 
+class RgbdFormat(C.Structure):          # sgs_rgbd_format
+    _fields_ = [('rgb', C.c_int32), ('depth_type', C.c_int32), ('depth_map_factor', C.c_float), ('dist_coef', C.c_float * 5)]
+
+
+DEPTH_U16, DEPTH_F32 = 0, 1
+
+
+def rgbd_format(settings, depth_type=DEPTH_U16):
+    """The sgs_rgbd_format of a loaded Settings: Camera.RGB, mDepthMapFactor and k1 k2 p1 p2 k3."""
+    f = RgbdFormat(settings.rgb, depth_type, settings.depth_map_factor)
+    for i, k in enumerate(('k1', 'k2', 'p1', 'p2', 'k3')):
+        f.dist_coef[i] = getattr(settings, k)
+    return f
+
+
 class FrameView(C.Structure):
     _fields_ = [('n', C.c_int32), ('keys_un', C.c_void_p), ('u_right', C.c_void_p), ('desc', C.c_void_p),
                 ('min_x', C.c_float), ('min_y', C.c_float), ('max_x', C.c_float), ('max_y', C.c_float),

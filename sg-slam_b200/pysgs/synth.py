@@ -90,6 +90,19 @@ def stream_s2(nframes=16, w=640, h=480, seed=2, tex_w=1024, tex_h=768, person=Tr
     return frames, boxes
 
 
+def stream_s2_rgbd(nframes=16, w=640, h=480, seed=2, **kw):
+    """Colour RGB-D variant of S2: the S2 frames of `seed` in three channels that differ -- c0 = frame + N(0,3), c1 = frame + N(0,3),
+    c2 = 255 - frame + N(0,3), so that the two channel orders give different gray images -- and the S1 depth plane stored TUM-style as
+    uint16 = round(d * 5000) for every frame.  Returns (colour u8 [n,h,w,3], depth u16 [n,h,w], boxes [n,4])."""
+    frames, boxes = stream_s2(nframes, w, h, seed=seed, **kw)
+    rng = np.random.RandomState(seed + 31)
+    g = frames.astype(np.float64)
+    ch = [g, g, 255.0 - g]
+    rgb = np.stack([np.clip(np.rint(c + rng.normal(0, 3, g.shape)), 0, 255) for c in ch], -1).astype(np.uint8)
+    depth = np.rint(depth_s1(w, h).astype(np.float64) * 5000).astype(np.uint16)
+    return rgb, np.ascontiguousarray(np.broadcast_to(depth, (nframes, h, w))), boxes
+
+
 def descriptors_s5(n, seed=5):
     """S5: uniform random 256-bit descriptors [n,32] u8."""
     rng = np.random.RandomState(seed)
