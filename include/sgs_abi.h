@@ -489,15 +489,18 @@ SGS_API int sgs_fundamental_batch_device(const sgs_keypoint* d_kps, const float*
 /* ------------------------------------------------------------------------------------
  * Batched front end with HOST buffers: the part of Frame::Frame (RGB-D ctor, src/Frame.cc:129-198) and
  * Tracking::TrackWithMotionModel (src/Tracking.cc:906-931) that runs on the GPU, for `nframes` independent frames.
- *   sgs_tracker_extract : ExtractORB (src/Frame.cc:146).  Keypoints/descriptors return to the host, which runs
- *                         calcOpticalFlowPyrLK + findFundamentalMat (src/Frame.cc:445-472) -- not on the GPU in this round.
+ *   sgs_tracker_extract : ExtractORB (src/Frame.cc:146).  Keypoints/descriptors also return to the host.
+ *                         calcOpticalFlowPyrLK + findFundamentalMat (src/Frame.cc:445-472) run on the device in sgs_tracker_track_lk
+ *                         and sgs_tracker_step; sgs_tracker_track takes their results (prev_xy, F) from the caller instead.
  *   sgs_tracker_track   : dyn-reject verdicts + ordered compaction of keypoints, descriptors and u_right
  *                         (src/Frame.cc:560-604) on the device-resident extraction results, then
  *                         SearchByProjection(cur, last, th, mono) (src/ORBmatcher.cc:1332-1472).
  * Array shapes: prev_xy [F][cap][2], u_right [F][cap] (mvuRight of the UNfiltered keypoints), F [F][9] (NaN in F[0] ==
  * empty matrix), boxes [F][max_boxes], last_* [F][point_cap](..), tcw_* [F][16]; outputs kps_out [F][cap],
  * desc_out [F][cap][32], u_right_out [F][cap] (may be NULL), counts_out [F], cur_mp_out [F][cap], nmatches_out [F].
- * Pinned host memory is copied without staging.
+ * Pinned host memory is copied without staging.  The host-buffer calls (sgs_tracker_track, _track_lk, _step, _step_rgbd)
+ * upload u_right and the last-frame arrays on a copy stream of the tracker that is not ordered after work still pending
+ * from the device-pointer calls below: synchronise their stream before a host-buffer call on the same tracker.
  * ------------------------------------------------------------------------------------ */
 typedef struct sgs_tracker sgs_tracker;
 SGS_API int sgs_tracker_create(const sgs_orb_params* params, int width, int height, int max_batch, int point_cap,

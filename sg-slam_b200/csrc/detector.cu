@@ -716,7 +716,7 @@ struct sgs_detector {
     float* d_prior = nullptr; float* d_var = nullptr;
     unsigned long long* d_picked = nullptr; int32_t* d_picked_n = nullptr;
     // host-call scratch
-    uint8_t* d_img = nullptr; int64_t d_img_cap = 0;
+    uint8_t* d_img = nullptr; size_t d_img_cap = 0;
     int* d_pre_tab = nullptr; int pre_w = 0, pre_h = 0;       // resize coefficient table of the last source geometry (preprocess_table_kernel)
     sgs_object2d* d_obj = nullptr; int32_t* d_cnt = nullptr;
     int last_frames = 0;
@@ -1325,7 +1325,7 @@ int sgs_detect(sgs_detector* D, const uint8_t* rgb, int width, int height, int p
     if (!D || !rgb || !n || (cap > 0 && !objects) || width < 2 || height < 2 || pitch < width * 3) { set_error("sgs_detect: bad argument"); return SGS_ERR_INVALID; }
     SGS_CUDA_TRY(cudaSetDevice(D->device));
     const int64_t bytes = (int64_t)pitch * height;
-    if (bytes > D->d_img_cap) { D->d_img_cap = 0; SGS_CUDA_TRY(D->res.regrow(&D->d_img, (size_t)bytes)); D->d_img_cap = bytes; }
+    SGS_CUDA_TRY(D->res.grow(&D->d_img, &D->d_img_cap, (size_t)bytes));
     SGS_CUDA_TRY(cudaMemcpy(D->d_img, rgb, (size_t)bytes, cudaMemcpyHostToDevice));
     int rc = sgs_detector_detect_device(D, D->d_img, bytes, pitch, width, height, 1, nullptr, nullptr, D->d_obj, D->d_cnt, nullptr, nullptr, nullptr, nullptr, nullptr, 0,
                                         nullptr, nullptr);

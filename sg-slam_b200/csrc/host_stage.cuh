@@ -101,6 +101,14 @@ public:
             if (r->p == *p) { r->release(r->p); held_.erase(r); break; }
         return alloc(p, bytes);
     }
+    // a buffer grown on demand: regrows *p when *cap < bytes; *cap is 0 after a failed grow, so the next call tries again
+    template <class T> cudaError_t grow(T** p, size_t* cap, size_t bytes) {
+        if (*cap >= bytes) return cudaSuccess;
+        *cap = 0;
+        const cudaError_t e = regrow(p, bytes);
+        if (e == cudaSuccess) *cap = bytes;
+        return e;
+    }
 
 private:
     struct Held { void* p; cudaError_t (*release)(void*); };

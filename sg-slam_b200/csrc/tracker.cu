@@ -1,6 +1,6 @@
 // tracker.cu -- batched front end of the tracking thread's per-frame hot path with HOST buffers at the boundary:
 //   sgs_tracker_extract : Frame::ExtractORB (src/Frame.cc:274-280) for a batch of frames; keypoints go back to the host
-//                         (the host runs LK + findFundamentalMat on them, src/Frame.cc:445-472 -- not on the GPU yet);
+//                         (LK + findFundamentalMat, src/Frame.cc:445-472, run on the device in sgs_tracker_track_lk and the steps);
 //   sgs_tracker_track   : dyn-reject verdicts + ordered compaction (src/Frame.cc:560-604) followed by
 //                         ORBmatcher::SearchByProjection(cur, last, th, mono) (src/ORBmatcher.cc:1332-1472, called from
 //                         Tracking::TrackWithMotionModel, src/Tracking.cc:924), on the device-resident extraction results.
@@ -31,7 +31,9 @@ struct sgs_tracker {
     int32_t* d_pidx = nullptr;
     double* d_Fgpu = nullptr; int32_t* d_finfo = nullptr;     // findFundamentalMat on the device
     cudaStream_t st = nullptr;
-    cudaStream_t copy_st = nullptr; cudaEvent_t copy_ev = nullptr;      // input uploads of sgs_tracker_track_lk run beside the LK kernels
+    // the bulk host uploads of every host track call and step run on copy_st beside the kernels, joined by copy_ev before the rejection;
+    // copy_st is not ordered after work still pending on `st` from the device entry points
+    cudaStream_t copy_st = nullptr; cudaEvent_t copy_ev = nullptr;
     // device inputs of track()
     float* d_prev = nullptr; float* d_uright_in = nullptr; double* d_F = nullptr; sgs_rect* d_boxes = nullptr; int32_t* d_nboxes = nullptr;
     uint8_t* d_have = nullptr;
@@ -182,52 +184,141 @@ __global__ void __launch_bounds__(256) chain_final_kernel(const int32_t* __restr
 using namespace sgs;
 
 namespace {
-int bad(const char* m) { set_error("%s", m); return SGS_ERR_INVALID; }
+int bad(const char* fn, const char* why) { set_error("%s: %s", fn, why); return SGS_ERR_INVALID; }
 
-// the per-frame inputs of the last-frame search, host -> device on `s` (u_right NULL: computed on the device by an RGB-D step)
-int upload_track_inputs(sgs_tracker* t, size_t B, const float* u_right, const float* last_xyz, const uint8_t* last_desc, const uint8_t* last_flags,
-                        const int32_t* last_octave, const float* last_angle, const int32_t* last_n, const float* tcw_cur, const float* tcw_last, cudaStream_t s) {
+// The argument checks of the entry points: each returns false after set_error("<fn>: ...") on a refusal, which the entry point returns as
+// SGS_ERR_INVALID before it enqueues anything.
+// nframes in [1, limit] (the frames of the last extract call, or max_batch for the calls that bring their own frames); prev_index [nframes]
+// (host, NULL: none to check): each frame's previous frame is a row of the batch
+bool frames_ok(const char* fn, int nframes, int limit, const int32_t* prev_index = nullptr) {
+    if (nframes < 1 || nframes > limit) { set_error("%s: nframes = %d outside [1,%d]", fn, nframes, limit); return false; }
+    for (int f = 0; prev_index && f < nframes; ++f)
+        if (prev_index[f] < 0 || prev_index[f] >= nframes) { set_error("%s: prev_index out of range", fn); return false; }
+    return true;
+}
+
+// colour frames: interleaved 8-bit RGB, byte pitch and frame stride
+bool rgb_layout_ok(const sgs_tracker* t, const char* fn, size_t rgb_stride, int rgb_pitch) {
+    if (rgb_pitch >= t->width * 3 && rgb_stride >= (size_t)rgb_pitch * t->height) return true;
+    set_error("%s: rgb pitch / stride too small", fn);
+    return false;
+}
+
+// the depth format and layout of the RGB-D steps (byte pitch and frame stride)
+bool depth_args_ok(const sgs_tracker* t, const char* fn, const sgs_rgbd_format* fmt, size_t depth_stride, int depth_pitch, const void* depth) {
+    const char* why = nullptr;
+    const size_t esz = fmt->depth_type == 0 ? 2 : 4;
+    if (fmt->depth_type != 0 && fmt->depth_type != 1) why = "depth_type is neither 0 (uint16) nor 1 (float32)";
+    else if (!std::isfinite(fmt->depth_map_factor) || !(fmt->depth_map_factor > 0.f)) why = "depth_map_factor is not a finite positive number";
+    else if ((size_t)depth_pitch < esz * t->width || depth_stride < (size_t)depth_pitch * t->height) why = "depth pitch / stride too small";
+    else if (depth_pitch % esz || depth_stride % esz || (uintptr_t)depth % esz) why = "depth pitch, stride or pointer not a multiple of the element size";
+    if (why) set_error("%s: %s", fn, why);
+    return why == nullptr;
+}
+
+// the extraction results of the last extract call, on the device: keypoints [F][cap], descriptors [F][cap][32], counts [F]
+struct Extracted { const sgs_keypoint* kps; const uint8_t* desc; const int32_t* n; int cap; };
+Extracted extracted(const sgs_tracker* t) {
+    Extracted e{};
+    sgs_extractor_results_device(t->ex.get(), &e.kps, &e.desc, &e.n, &e.cap);
+    return e;
+}
+
+// The eight per-frame arrays SearchByProjection(cur, last) reads about the last frame: [F][point_cap](..) and the poses [F][16], host or device
+// pointers (the last_* fields of sgs_posechain_batch and the arguments of the track calls).
+struct LastFrame {
+    const float* xyz = nullptr; const uint8_t* desc = nullptr; const uint8_t* flags = nullptr; const int32_t* octave = nullptr;
+    const float* angle = nullptr; const int32_t* n = nullptr; const float* tcw_cur = nullptr; const float* tcw_last = nullptr;
+
+    bool complete() const { return xyz && desc && flags && octave && angle && n && tcw_cur && tcw_last; }
+};
+// the tracker's device copies, filled by stage_host_inputs
+LastFrame device_last(const sgs_tracker* t) {
+    LastFrame l;
+    l.xyz = t->d_lxyz; l.desc = t->d_ldesc; l.flags = t->d_lflags; l.octave = t->d_loct; l.angle = t->d_lang; l.n = t->d_ln; l.tcw_cur = t->d_tc; l.tcw_last = t->d_tl;
+    return l;
+}
+
+// SearchByProjection(cur, last, th, mono) of the tracker's compacted current frame into its cur_mp / nmatches / ncand
+sgs_lastframe_batch lastframe_search(const sgs_tracker* t, const LastFrame& l, float th, int mono, int check_orientation) {
+    sgs_lastframe_batch a;
+    std::memset(&a, 0, sizeof a);
+    a.cam = t->cam;
+    a.cur_kps = t->keys_un; a.cur_desc = t->d_desc2; a.cur_uright = t->d_uright2; a.cur_n = t->d_cnt2;
+    a.last_xyz = l.xyz; a.last_desc = l.desc; a.last_flags = l.flags; a.last_octave = l.octave; a.last_angle = l.angle; a.last_n = l.n;
+    a.tcw_cur = l.tcw_cur; a.tcw_last = l.tcw_last; a.th = th; a.mono = mono; a.check_orientation = check_orientation;
+    a.cur_mp = t->d_mp; a.nmatches = t->d_nm; a.ncand = (uint64_t*)t->d_ncand;
+    return a;
+}
+
+// The per-frame inputs of a track call.  NULL: not given -- computed on the device (u_right of an RGB-D step, F), or the tracker's own
+// array as it is (boxes).  prev_xy replaces prev_index in sgs_tracker_track, which runs no LK.
+struct TrackInputs {
+    LastFrame last;
+    const float* u_right = nullptr;
+    const int32_t* prev_index = nullptr; const float* prev_xy = nullptr; const double* F = nullptr;
+    const sgs_rect* boxes = nullptr; const int32_t* nboxes = nullptr; const uint8_t* have_dyn = nullptr;
+};
+
+// Host inputs -> the tracker's device arrays.  What LK and the F estimate read goes first, on the tracker's stream; the bulk (u_right, the
+// last-frame arrays) goes on the copy stream beside those kernels, and copy_ev marks its end for the wait before the rejection.
+int stage_host_inputs(sgs_tracker* t, size_t B, const TrackInputs& in) {
     const size_t K = t->cap, M = t->point_cap;
-    auto h2d = [s](void* dst, const void* src, size_t bytes) { return cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, s); };
-    if (u_right) SGS_CUDA_TRY(h2d(t->d_uright_in, u_right, B * K * 4));
-    SGS_CUDA_TRY(h2d(t->d_lxyz, last_xyz, B * M * 12)); SGS_CUDA_TRY(h2d(t->d_ldesc, last_desc, B * M * 32));
-    SGS_CUDA_TRY(h2d(t->d_lflags, last_flags, B * M)); SGS_CUDA_TRY(h2d(t->d_loct, last_octave, B * M * 4)); SGS_CUDA_TRY(h2d(t->d_lang, last_angle, B * M * 4));
-    SGS_CUDA_TRY(h2d(t->d_ln, last_n, B * 4)); SGS_CUDA_TRY(h2d(t->d_tc, tcw_cur, B * 64)); SGS_CUDA_TRY(h2d(t->d_tl, tcw_last, B * 64));
+    auto h2d = [](void* dst, const void* src, size_t bytes, cudaStream_t s) { return cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, s); };
+    const cudaStream_t st = t->st, cs = t->copy_st;
+    if (in.prev_index) SGS_CUDA_TRY(h2d(t->d_pidx, in.prev_index, sizeof(int32_t) * B, st));
+    if (in.prev_xy) SGS_CUDA_TRY(h2d(t->d_prev, in.prev_xy, B * K * 8, st));
+    if (in.F) SGS_CUDA_TRY(h2d(t->d_F, in.F, B * 72, st));
+    if (in.boxes) SGS_CUDA_TRY(h2d(t->d_boxes, in.boxes, B * t->max_boxes * sizeof(sgs_rect), st));
+    if (in.nboxes) SGS_CUDA_TRY(h2d(t->d_nboxes, in.nboxes, B * 4, st));
+    if (in.have_dyn) SGS_CUDA_TRY(h2d(t->d_have, in.have_dyn, B, st));
+    const LastFrame& l = in.last;
+    if (in.u_right) SGS_CUDA_TRY(h2d(t->d_uright_in, in.u_right, B * K * 4, cs));
+    SGS_CUDA_TRY(h2d(t->d_lxyz, l.xyz, B * M * 12, cs)); SGS_CUDA_TRY(h2d(t->d_ldesc, l.desc, B * M * 32, cs));
+    SGS_CUDA_TRY(h2d(t->d_lflags, l.flags, B * M, cs)); SGS_CUDA_TRY(h2d(t->d_loct, l.octave, B * M * 4, cs)); SGS_CUDA_TRY(h2d(t->d_lang, l.angle, B * M * 4, cs));
+    SGS_CUDA_TRY(h2d(t->d_ln, l.n, B * 4, cs)); SGS_CUDA_TRY(h2d(t->d_tc, l.tcw_cur, B * 64, cs)); SGS_CUDA_TRY(h2d(t->d_tl, l.tcw_last, B * 64, cs));
+    SGS_CUDA_TRY(cudaEventRecord(t->copy_ev, cs));
     return SGS_OK;
 }
 
-// the results of the last-frame search, device -> host on `s` (u_right_out may be NULL)
-int download_track_results(const sgs_tracker* t, size_t B, sgs_keypoint* kps_out, uint8_t* desc_out, float* u_right_out, int32_t* counts_out,
-                           int32_t* cur_mp_out, int32_t* nmatches_out, cudaStream_t s) {
+// Where a host entry point's results go: the arrays of sgs_tracker_track, then the extras of the steps.  u_right and the extras may be NULL.
+struct HostOutputs {
+    sgs_keypoint* kps = nullptr; uint8_t* desc = nullptr; float* u_right = nullptr; int32_t* counts = nullptr; int32_t* cur_mp = nullptr;
+    int32_t* nmatches = nullptr; sgs_rect* boxes = nullptr; int32_t* nboxes = nullptr; uint8_t* have = nullptr; sgs_keypoint* kps_un = nullptr; float* depth = nullptr;
+
+    bool complete() const { return kps && desc && counts && cur_mp && nmatches; }
+};
+
+// the results, device -> host on the tracker's stream, then the one synchronisation of the call
+int download_results(sgs_tracker* t, size_t B, const HostOutputs& o) {
     const size_t K = t->cap;
-    auto d2h = [s](void* dst, const void* src, size_t bytes) { return cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, s); };
-    SGS_CUDA_TRY(d2h(kps_out, t->d_kps2, B * K * sizeof(sgs_keypoint))); SGS_CUDA_TRY(d2h(desc_out, t->d_desc2, B * K * 32)); SGS_CUDA_TRY(d2h(counts_out, t->d_cnt2, B * 4));
-    if (u_right_out) SGS_CUDA_TRY(d2h(u_right_out, t->d_uright2, B * K * 4));
-    SGS_CUDA_TRY(d2h(cur_mp_out, t->d_mp, B * K * 4)); SGS_CUDA_TRY(d2h(nmatches_out, t->d_nm, B * 4));
+    const cudaStream_t st = t->st;
+    auto d2h = [st](void* dst, const void* src, size_t bytes) { return cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, st); };
+    SGS_CUDA_TRY(d2h(o.kps, t->d_kps2, B * K * sizeof(sgs_keypoint))); SGS_CUDA_TRY(d2h(o.desc, t->d_desc2, B * K * 32)); SGS_CUDA_TRY(d2h(o.counts, t->d_cnt2, B * 4));
+    if (o.u_right) SGS_CUDA_TRY(d2h(o.u_right, t->d_uright2, B * K * 4));
+    SGS_CUDA_TRY(d2h(o.cur_mp, t->d_mp, B * K * 4)); SGS_CUDA_TRY(d2h(o.nmatches, t->d_nm, B * 4));
+    if (o.boxes) SGS_CUDA_TRY(d2h(o.boxes, t->d_boxes, B * t->max_boxes * sizeof(sgs_rect)));
+    if (o.nboxes) SGS_CUDA_TRY(d2h(o.nboxes, t->d_nboxes, B * 4));
+    if (o.have) SGS_CUDA_TRY(d2h(o.have, t->d_have, B));
+    if (o.kps_un) SGS_CUDA_TRY(d2h(o.kps_un, t->d_kpsun2, B * K * sizeof(sgs_keypoint)));
+    if (o.depth) SGS_CUDA_TRY(d2h(o.depth, t->d_dz2, B * K * 4));
+    SGS_CUDA_TRY(cudaStreamSynchronize(st));
     return SGS_OK;
 }
 
 // dyn-reject + compaction + SearchByProjection(cur, last) on `st` (body of sgs_tracker_track_device).  kun / dz (RGB-D step, else NULL): mvKeysUn and
 // mvDepth of the extracted keypoints, compacted beside them; the search then runs on the compacted mvKeysUn.
 int enqueue_track(sgs_tracker* t, int nframes, const float* prev_xy, const float* u_right, const double* F, const sgs_rect* boxes, const int32_t* nboxes,
-                  const uint8_t* have_dyn, const float* last_xyz, const uint8_t* last_desc, const uint8_t* last_flags, const int32_t* last_octave,
-                  const float* last_angle, const int32_t* last_n, const float* tcw_cur, const float* tcw_last, float th, int mono, int check_orientation,
-                  const sgs_keypoint* kun, const float* dz, cudaStream_t st) {
-    const sgs_keypoint* d_kps; const uint8_t* d_desc; const int32_t* d_cnt; int cap = 0;
-    sgs_extractor_results_device(t->ex.get(), &d_kps, &d_desc, &d_cnt, &cap);
-    int rc = sgs_dynreject_batch_device(d_kps, d_desc, d_cnt, cap, nframes, prev_xy, F, boxes, nboxes, t->max_boxes, have_dyn,
+                  const uint8_t* have_dyn, const LastFrame& last, float th, int mono, int check_orientation, const sgs_keypoint* kun, const float* dz,
+                  cudaStream_t st) {
+    const Extracted ex = extracted(t);
+    int rc = sgs_dynreject_batch_device(ex.kps, ex.desc, ex.n, ex.cap, nframes, prev_xy, F, boxes, nboxes, t->max_boxes, have_dyn,
                                         t->nfeatures, t->d_kps2, t->d_desc2, t->d_cnt2, t->d_keep, st);
     if (rc != SGS_OK) return rc;
-    compact_uright_kernel<<<nframes, 256, 0, st>>>(u_right, t->d_keep, d_cnt, t->d_cnt2, cap, t->d_uright2, t->d_mp, kun, t->d_kpsun2, dz, t->d_dz2);
+    compact_uright_kernel<<<nframes, 256, 0, st>>>(u_right, t->d_keep, ex.n, t->d_cnt2, ex.cap, t->d_uright2, t->d_mp, kun, t->d_kpsun2, dz, t->d_dz2);
     t->keys_un = kun ? t->d_kpsun2 : t->d_kps2;
     SGS_CUDA_TRY(cudaMemsetAsync(t->d_ncand, 0, (size_t)nframes * 8, st));
-    sgs_lastframe_batch a;
-    std::memset(&a, 0, sizeof a);
-    a.cam = t->cam;
-    a.cur_kps = t->keys_un; a.cur_desc = t->d_desc2; a.cur_uright = t->d_uright2; a.cur_n = t->d_cnt2;
-    a.last_xyz = last_xyz; a.last_desc = last_desc; a.last_flags = last_flags; a.last_octave = last_octave; a.last_angle = last_angle; a.last_n = last_n;
-    a.tcw_cur = tcw_cur; a.tcw_last = tcw_last; a.th = th; a.mono = mono; a.check_orientation = check_orientation;
-    a.cur_mp = t->d_mp; a.cur_mp_obs_in = nullptr; a.nmatches = t->d_nm; a.ncand = (uint64_t*)t->d_ncand;
+    const sgs_lastframe_batch a = lastframe_search(t, last, th, mono, check_orientation);
     return sgs_match_project_lastframe_batch_device(t->mt.get(), &a, nframes, st);
 }
 
@@ -239,28 +330,24 @@ int ensure_rgbd_buffers(sgs_tracker* t, size_t raw_bytes) {
         SGS_CUDA_TRY(R.regrow(&t->d_depthf, B * px * 4 + 16)); SGS_CUDA_TRY(R.regrow(&t->d_kpsun, B * K * sizeof(sgs_keypoint) + 16));
         SGS_CUDA_TRY(R.regrow(&t->d_dz, B * K * 4 + 16)); SGS_CUDA_TRY(R.regrow(&t->d_dz2, B * K * 4 + 16)); SGS_CUDA_TRY(R.regrow(&t->d_kpsun2, B * K * sizeof(sgs_keypoint) + 16));
     }
-    if (t->d_depth_raw_cap < raw_bytes * B) {
-        t->d_depth_raw_cap = 0;
-        SGS_CUDA_TRY(R.regrow(&t->d_depth_raw, raw_bytes * B));
-        t->d_depth_raw_cap = raw_bytes * B;
-    }
+    SGS_CUDA_TRY(R.grow(&t->d_depth_raw, &t->d_depth_raw_cap, raw_bytes * B));
     return SGS_OK;
+}
+
+// B host frames of `rows` rows of row_bytes (byte pitch, frame stride) -> dense device frames on `s`: one copy when the host frames are dense too
+cudaError_t upload_frames(uint8_t* dst, const void* src, size_t stride, int pitch, size_t row_bytes, int rows, size_t B, cudaStream_t s) {
+    if (stride == (size_t)pitch * rows) return cudaMemcpy2DAsync(dst, row_bytes, src, pitch, row_bytes, (size_t)rows * B, cudaMemcpyHostToDevice, s);
+    for (size_t f = 0; f < B; ++f)
+        if (const cudaError_t e = cudaMemcpy2DAsync(dst + f * row_bytes * rows, row_bytes, (const uint8_t*)src + f * stride, pitch, row_bytes, rows,
+                                                    cudaMemcpyHostToDevice, s)) return e;
+    return cudaSuccess;
 }
 
 // colour frames host -> the tracker's dense staging buffer (pitch width * 3) on the detector stream
 int upload_rgb(sgs_tracker* t, const uint8_t* rgb, size_t rgb_stride, int rgb_pitch, size_t B) {
-    const size_t rgb_bytes = (size_t)t->width * 3 * t->height;
-    if (t->d_rgb_cap < rgb_bytes * (size_t)t->max_batch) {
-        t->d_rgb_cap = 0;
-        SGS_CUDA_TRY(t->res.regrow(&t->d_rgb, rgb_bytes * (size_t)t->max_batch));
-        t->d_rgb_cap = rgb_bytes * (size_t)t->max_batch;
-    }
-    if (rgb_stride == (size_t)rgb_pitch * t->height) {
-        SGS_CUDA_TRY(cudaMemcpy2DAsync(t->d_rgb, (size_t)t->width * 3, rgb, rgb_pitch, (size_t)t->width * 3, (size_t)t->height * B, cudaMemcpyHostToDevice, t->det_st));
-    } else {
-        for (size_t f = 0; f < B; ++f)
-            SGS_CUDA_TRY(cudaMemcpy2DAsync(t->d_rgb + f * rgb_bytes, (size_t)t->width * 3, rgb + f * rgb_stride, rgb_pitch, (size_t)t->width * 3, t->height, cudaMemcpyHostToDevice, t->det_st));
-    }
+    const size_t row = (size_t)t->width * 3;
+    SGS_CUDA_TRY(t->res.grow(&t->d_rgb, &t->d_rgb_cap, row * t->height * t->max_batch));
+    SGS_CUDA_TRY(upload_frames(t->d_rgb, rgb, rgb_stride, rgb_pitch, row, t->height, B, t->det_st));
     return SGS_OK;
 }
 
@@ -268,21 +355,17 @@ int upload_rgb(sgs_tracker* t, const uint8_t* rgb, size_t rgb_stride, int rgb_pi
 // memory (sgs_tracker_step) or, with gray == NULL, are converted from the colour frames together with the raw depth (RGB-D steps).
 struct StepFrames {
     const uint8_t* d_rgb; size_t rgb_stride; int rgb_pitch; cudaStream_t rgb_st;
-    const uint8_t* gray; size_t gray_stride; int gray_pitch;
-    const void* d_depth; size_t depth_stride; int depth_pitch; const sgs_rgbd_format* fmt;
+    const uint8_t* gray = nullptr; size_t gray_stride = 0; int gray_pitch = 0;
+    const void* d_depth = nullptr; size_t depth_stride = 0; int depth_pitch = 0; const sgs_rgbd_format* fmt = nullptr;
 };
-// The per-frame inputs of the search: host pointers, uploaded on the copy stream while the kernels run, or device pointers.  u_right: the step's
-// host input (sgs_tracker_step); NULL in RGB-D steps, which compute it.
-struct StepInputs {
-    bool host; const int32_t* prev_index; const float* u_right;
-    const float* last_xyz; const uint8_t* last_desc; const uint8_t* last_flags; const int32_t* last_octave; const float* last_angle; const int32_t* last_n;
-    const float* tcw_cur; const float* tcw_last;
-};
+// the colour frames staged by upload_rgb
+StepFrames staged_rgb(const sgs_tracker* t) { return {t->d_rgb, (size_t)t->width * 3 * t->height, t->width * 3, t->det_st}; }
 
 // The stream and event choreography of every step: the detector on its own stream beside extract -> LK on `st`, joined before findFundamentalMat;
-// an RGB-D step converts gray and depth on `st` and adds UndistortKeyPoints + ComputeStereoFromRGBD before the rejection.
-int enqueue_step(sgs_tracker* t, sgs_detector* det, const StepFrames& fr, int nframes, const StepInputs& in, float th, int mono, int check_orientation,
-                 cudaStream_t st) {
+// an RGB-D step converts gray and depth on `st` and adds UndistortKeyPoints + ComputeStereoFromRGBD before the rejection.  host_inputs: `in`
+// holds host pointers, staged by stage_host_inputs while the kernels run; else device pointers.
+int enqueue_step(sgs_tracker* t, sgs_detector* det, const StepFrames& fr, int nframes, const TrackInputs& in, bool host_inputs, float th, int mono,
+                 int check_orientation, cudaStream_t st) {
     const size_t B = nframes;
     const bool rgbd = fr.gray == nullptr;
     // ---- detector branch: network on the colour frames, boxes into the tracker's arrays
@@ -316,16 +399,11 @@ int enqueue_step(sgs_tracker* t, sgs_detector* det, const StepFrames& fr, int nf
     }
     t->last_nframes = nframes;
     const int32_t* d_pidx = in.prev_index;
-    const float *lxyz = in.last_xyz, *lang = in.last_angle, *tc = in.tcw_cur, *tl = in.tcw_last;
-    const uint8_t *ldesc = in.last_desc, *lfl = in.last_flags;
-    const int32_t *loct = in.last_octave, *ln = in.last_n;
-    if (in.host) {
-        SGS_CUDA_TRY(cudaMemcpyAsync(t->d_pidx, in.prev_index, sizeof(int32_t) * B, cudaMemcpyHostToDevice, st));
-        rc = upload_track_inputs(t, B, in.u_right, in.last_xyz, in.last_desc, in.last_flags, in.last_octave, in.last_angle, in.last_n, in.tcw_cur, in.tcw_last, t->copy_st);
+    LastFrame last = in.last;
+    if (host_inputs) {
+        rc = stage_host_inputs(t, B, in);
         if (rc != SGS_OK) return rc;
-        SGS_CUDA_TRY(cudaEventRecord(t->copy_ev, t->copy_st));
-        d_pidx = t->d_pidx;
-        lxyz = t->d_lxyz; ldesc = t->d_ldesc; lfl = t->d_lflags; loct = t->d_loct; lang = t->d_lang; ln = t->d_ln; tc = t->d_tc; tl = t->d_tl;
+        d_pidx = t->d_pidx; last = device_last(t);
     }
     rc = sgs_tracker_lk_device(t, d_frames, nframes, fstride, pitch, d_pidx, st);
     if (rc != SGS_OK) return rc;
@@ -333,44 +411,15 @@ int enqueue_step(sgs_tracker* t, sgs_detector* det, const StepFrames& fr, int nf
     rc = sgs_tracker_fundamental_device(t, nframes, nullptr, nullptr, nullptr, d_pidx, st);
     if (rc != SGS_OK) return rc;
     if (rgbd) {     // Frame.cc:146-174 undistorts and looks the depth up after the rejection; both are per point, so doing them first gives the same values
-        const sgs_keypoint* d_kps; const int32_t* d_cnt; int cap = 0;
-        sgs_extractor_results_device(t->ex.get(), &d_kps, nullptr, &d_cnt, &cap);
-        rc = sgs_undistort_batch_device(d_kps, d_cnt, cap, nframes, t->cam.fx, t->cam.fy, t->cam.cx, t->cam.cy, fr.fmt->dist_coef, t->d_kpsun, st);
+        const Extracted ex = extracted(t);
+        rc = sgs_undistort_batch_device(ex.kps, ex.n, ex.cap, nframes, t->cam.fx, t->cam.fy, t->cam.cx, t->cam.cy, fr.fmt->dist_coef, t->d_kpsun, st);
         if (rc != SGS_OK) return rc;
-        rc = sgs_stereo_from_depth_batch_device(d_kps, t->d_kpsun, d_cnt, cap, nframes, depth, depth_fstride, depth_pitch, t->cam.bf, t->d_uright_in, t->d_dz, st);
+        rc = sgs_stereo_from_depth_batch_device(ex.kps, t->d_kpsun, ex.n, ex.cap, nframes, depth, depth_fstride, depth_pitch, t->cam.bf, t->d_uright_in, t->d_dz, st);
         if (rc != SGS_OK) return rc;
     }
-    if (in.host) SGS_CUDA_TRY(cudaStreamWaitEvent(st, t->copy_ev, 0));
-    return enqueue_track(t, nframes, t->d_prev, t->d_uright_in, t->d_Fgpu, t->d_boxes, t->d_nboxes, t->d_have, lxyz, ldesc, lfl,
-                         loct, lang, ln, tc, tl, th, mono, check_orientation, rgbd ? t->d_kpsun : nullptr, rgbd ? t->d_dz : nullptr, st);
-}
-
-// the outputs of a step, device -> host on the tracker's stream, then the one synchronisation of the call (every pointer but the first six may be NULL)
-int download_step(sgs_tracker* t, size_t B, sgs_keypoint* kps_out, uint8_t* desc_out, float* u_right_out, int32_t* counts_out, int32_t* cur_mp_out,
-                  int32_t* nmatches_out, sgs_rect* boxes_out, int32_t* nboxes_out, uint8_t* have_out, sgs_keypoint* kps_un_out, float* depth_out) {
-    cudaStream_t st = t->st;
-    int rc = download_track_results(t, B, kps_out, desc_out, u_right_out, counts_out, cur_mp_out, nmatches_out, st);
-    if (rc != SGS_OK) return rc;
-    if (boxes_out) SGS_CUDA_TRY(cudaMemcpyAsync(boxes_out, t->d_boxes, B * t->max_boxes * sizeof(sgs_rect), cudaMemcpyDeviceToHost, st));
-    if (nboxes_out) SGS_CUDA_TRY(cudaMemcpyAsync(nboxes_out, t->d_nboxes, B * 4, cudaMemcpyDeviceToHost, st));
-    if (have_out) SGS_CUDA_TRY(cudaMemcpyAsync(have_out, t->d_have, B, cudaMemcpyDeviceToHost, st));
-    if (kps_un_out) SGS_CUDA_TRY(cudaMemcpyAsync(kps_un_out, t->d_kpsun2, B * t->cap * sizeof(sgs_keypoint), cudaMemcpyDeviceToHost, st));
-    if (depth_out) SGS_CUDA_TRY(cudaMemcpyAsync(depth_out, t->d_dz2, B * t->cap * 4, cudaMemcpyDeviceToHost, st));
-    SGS_CUDA_TRY(cudaStreamSynchronize(st));
-    return SGS_OK;
-}
-
-// argument checks shared by the two RGB-D steps, before anything is enqueued (byte pitches and frame strides)
-int check_rgbd_args(const sgs_tracker* t, const char* fn, const sgs_rgbd_format* fmt, int nframes, size_t rgb_stride, int rgb_pitch, size_t depth_stride,
-                    int depth_pitch, const void* depth) {
-    if (nframes < 1 || nframes > t->max_batch) { set_error("%s: nframes outside [1,max_batch]", fn); return SGS_ERR_INVALID; }
-    if (fmt->depth_type != 0 && fmt->depth_type != 1) { set_error("%s: depth_type is neither 0 (uint16) nor 1 (float32)", fn); return SGS_ERR_INVALID; }
-    if (!std::isfinite(fmt->depth_map_factor) || !(fmt->depth_map_factor > 0.f)) { set_error("%s: depth_map_factor is not a finite positive number", fn); return SGS_ERR_INVALID; }
-    const size_t esz = fmt->depth_type == 0 ? 2 : 4;
-    if (rgb_pitch < t->width * 3 || rgb_stride < (size_t)rgb_pitch * t->height) { set_error("%s: rgb pitch / stride too small", fn); return SGS_ERR_INVALID; }
-    if ((size_t)depth_pitch < esz * t->width || depth_stride < (size_t)depth_pitch * t->height) { set_error("%s: depth pitch / stride too small", fn); return SGS_ERR_INVALID; }
-    if (depth_pitch % esz || depth_stride % esz || (uintptr_t)depth % esz) { set_error("%s: depth pitch, stride or pointer not a multiple of the element size", fn); return SGS_ERR_INVALID; }
-    return SGS_OK;
+    if (host_inputs) SGS_CUDA_TRY(cudaStreamWaitEvent(st, t->copy_ev, 0));
+    return enqueue_track(t, nframes, t->d_prev, t->d_uright_in, t->d_Fgpu, t->d_boxes, t->d_nboxes, t->d_have, last, th, mono, check_orientation,
+                         rgbd ? t->d_kpsun : nullptr, rgbd ? t->d_dz : nullptr, st);
 }
 }  // namespace
 
@@ -380,7 +429,7 @@ SGS_API void sgs_tracker_destroy(sgs_tracker* t) { delete t; }
 
 SGS_API int sgs_tracker_create(const sgs_orb_params* params, int width, int height, int max_batch, int point_cap, int max_boxes,
                                const sgs_camera* cam, int device, sgs_tracker** out) {
-    if (!params || !cam || !out || point_cap < 1 || max_boxes < 0) return bad("sgs_tracker_create: bad argument");
+    if (!params || !cam || !out || point_cap < 1 || max_boxes < 0) return bad("sgs_tracker_create", "bad argument");
     *out = nullptr;
     auto t = std::make_unique<sgs_tracker>(device);
     t->max_batch = max_batch; t->point_cap = point_cap; t->max_boxes = max_boxes > 0 ? max_boxes : 1; t->cam = *cam;
@@ -422,21 +471,21 @@ SGS_API int sgs_tracker_create(const sgs_orb_params* params, int width, int heig
 }
 
 SGS_API int sgs_tracker_max_keypoints(const sgs_tracker* t, int* cap) {
-    if (!t || !cap) return bad("sgs_tracker_max_keypoints: NULL");
+    if (!t || !cap) return bad("sgs_tracker_max_keypoints", "NULL");
     *cap = t->cap;
     return SGS_OK;
 }
 
 SGS_API int sgs_tracker_extract(sgs_tracker* t, const uint8_t* gray, int nframes, size_t frame_stride, int pitch, sgs_keypoint* kps, uint8_t* desc,
                                 int cap, int* n) {
-    if (!t) return bad("sgs_tracker_extract: NULL handle");
+    if (!t) return bad("sgs_tracker_extract", "NULL handle");
     int rc = sgs_extract_batch(t->ex.get(), gray, nframes, frame_stride, pitch, kps, desc, cap, n);
     if (rc == SGS_OK) t->last_nframes = nframes;
     return rc;
 }
 
 SGS_API int sgs_tracker_extract_device(sgs_tracker* t, const uint8_t* d_gray, int nframes, size_t frame_stride, int pitch, void* stream) {
-    if (!t) return bad("sgs_tracker_extract_device: NULL handle");
+    if (!t) return bad("sgs_tracker_extract_device", "NULL handle");
     int rc = sgs_extract_batch_device(t->ex.get(), d_gray, nframes, frame_stride, pitch, stream ? stream : (void*)t->st);
     if (rc == SGS_OK) t->last_nframes = nframes;
     return rc;
@@ -447,22 +496,23 @@ SGS_API int sgs_tracker_track_device(sgs_tracker* t, int nframes, const float* p
                                      const int32_t* nboxes, const uint8_t* have_dyn, const float* last_xyz, const uint8_t* last_desc,
                                      const uint8_t* last_flags, const int32_t* last_octave, const float* last_angle, const int32_t* last_n,
                                      const float* tcw_cur, const float* tcw_last, float th, int mono, int check_orientation, void* stream) {
-    if (!t || !last_xyz || !last_desc || !last_flags || !last_octave || !last_angle ||
-        !last_n || !tcw_cur || !tcw_last) return bad("sgs_tracker_track_device: NULL argument");
-    if (!nboxes) nboxes = t->d_nboxes;           // boxes / nboxes / have_dyn == NULL: the tracker's own arrays, filled by sgs_tracker_detect_device
-    if (!have_dyn) have_dyn = t->d_have;
-    if (!u_right) u_right = t->d_uright_in;      // filled by sgs_tracker_stereo_device
-    if (!F) F = t->d_Fgpu;                  // filled by sgs_tracker_fundamental_device
-    if (nframes < 1 || nframes > t->last_nframes) return bad("sgs_tracker_track_device: nframes exceeds the last extract call");
-    if (!prev_xy) prev_xy = t->d_prev;      // filled by sgs_tracker_lk_device
-    return enqueue_track(t, nframes, prev_xy, u_right, F, boxes ? boxes : t->d_boxes, nboxes, have_dyn, last_xyz, last_desc, last_flags, last_octave, last_angle,
-                         last_n, tcw_cur, tcw_last, th, mono, check_orientation, nullptr, nullptr, stream ? (cudaStream_t)stream : t->st);
+    const char* const fn = "sgs_tracker_track_device";
+    LastFrame last;
+    last.xyz = last_xyz; last.desc = last_desc; last.flags = last_flags; last.octave = last_octave; last.angle = last_angle; last.n = last_n;
+    last.tcw_cur = tcw_cur; last.tcw_last = tcw_last;
+    if (!t || !last.complete()) return bad(fn, "NULL argument");
+    if (!frames_ok(fn, nframes, t->last_nframes)) return SGS_ERR_INVALID;
+    // NULL: the tracker's own arrays, filled by sgs_tracker_lk_device (prev_xy), sgs_tracker_stereo_device (u_right), sgs_tracker_fundamental_device
+    // (F) and sgs_tracker_detect_device (boxes, nboxes, have_dyn)
+    return enqueue_track(t, nframes, prev_xy ? prev_xy : t->d_prev, u_right ? u_right : t->d_uright_in, F ? F : t->d_Fgpu, boxes ? boxes : t->d_boxes,
+                         nboxes ? nboxes : t->d_nboxes, have_dyn ? have_dyn : t->d_have, last, th, mono, check_orientation, nullptr, nullptr,
+                         stream ? (cudaStream_t)stream : t->st);
 }
 
 // device pointers to the results of the last track call: kps [B][cap], desc, u_right, counts [B], cur_mp [B][cap], nmatches [B], ncand [B]
 SGS_API int sgs_tracker_results_device(const sgs_tracker* t, const sgs_keypoint** kps, const uint8_t** desc, const float** u_right,
                                        const int32_t** counts, const int32_t** cur_mp, const int32_t** nmatches, const uint64_t** ncand) {
-    if (!t) return bad("sgs_tracker_results_device: NULL handle");
+    if (!t) return bad("sgs_tracker_results_device", "NULL handle");
     if (kps) *kps = t->d_kps2;
     if (desc) *desc = t->d_desc2;
     if (u_right) *u_right = t->d_uright2;
@@ -478,25 +528,24 @@ SGS_API int sgs_tracker_track(sgs_tracker* t, int nframes, const float* prev_xy,
                               const uint8_t* last_flags, const int32_t* last_octave, const float* last_angle, const int32_t* last_n,
                               const float* tcw_cur, const float* tcw_last, float th, int mono, int check_orientation, sgs_keypoint* kps_out,
                               uint8_t* desc_out, float* u_right_out, int32_t* counts_out, int32_t* cur_mp_out, int32_t* nmatches_out) {
-    if (!t || !prev_xy || !u_right || !F || !nboxes || !have_dyn || !last_xyz || !last_desc || !last_flags || !last_octave || !last_angle ||
-        !last_n || !tcw_cur || !tcw_last || !kps_out || !desc_out || !counts_out || !cur_mp_out || !nmatches_out)
-        return bad("sgs_tracker_track: NULL argument");
-    if (nframes < 1 || nframes > t->last_nframes) return bad("sgs_tracker_track: nframes exceeds the last sgs_tracker_extract call");
+    const char* const fn = "sgs_tracker_track";
+    LastFrame last;
+    last.xyz = last_xyz; last.desc = last_desc; last.flags = last_flags; last.octave = last_octave; last.angle = last_angle; last.n = last_n;
+    last.tcw_cur = tcw_cur; last.tcw_last = tcw_last;
+    HostOutputs out;
+    out.kps = kps_out; out.desc = desc_out; out.u_right = u_right_out; out.counts = counts_out; out.cur_mp = cur_mp_out; out.nmatches = nmatches_out;
+    if (!t || !prev_xy || !u_right || !F || !nboxes || !have_dyn || !last.complete() || !out.complete()) return bad(fn, "NULL argument");
+    if (!frames_ok(fn, nframes, t->last_nframes)) return SGS_ERR_INVALID;
     SGS_CUDA_TRY(cudaSetDevice(t->device));
-    const size_t B = nframes, K = t->cap;
-    cudaStream_t st = t->st;
-    SGS_CUDA_TRY(cudaMemcpyAsync(t->d_prev, prev_xy, B * K * 8, cudaMemcpyHostToDevice, st)); SGS_CUDA_TRY(cudaMemcpyAsync(t->d_F, F, B * 72, cudaMemcpyHostToDevice, st));
-    if (boxes) SGS_CUDA_TRY(cudaMemcpyAsync(t->d_boxes, boxes, B * t->max_boxes * sizeof(sgs_rect), cudaMemcpyHostToDevice, st));
-    SGS_CUDA_TRY(cudaMemcpyAsync(t->d_nboxes, nboxes, B * 4, cudaMemcpyHostToDevice, st)); SGS_CUDA_TRY(cudaMemcpyAsync(t->d_have, have_dyn, B, cudaMemcpyHostToDevice, st));
-    int rc = upload_track_inputs(t, B, u_right, last_xyz, last_desc, last_flags, last_octave, last_angle, last_n, tcw_cur, tcw_last, st);
+    TrackInputs in{last};
+    in.u_right = u_right; in.prev_xy = prev_xy; in.F = F; in.boxes = boxes; in.nboxes = nboxes; in.have_dyn = have_dyn;
+    int rc = stage_host_inputs(t, nframes, in);
     if (rc != SGS_OK) return rc;
-    rc = sgs_tracker_track_device(t, nframes, t->d_prev, t->d_uright_in, t->d_F, t->d_boxes, t->d_nboxes, t->d_have, t->d_lxyz, t->d_ldesc,
-                                  t->d_lflags, t->d_loct, t->d_lang, t->d_ln, t->d_tc, t->d_tl, th, mono, check_orientation, st);
+    SGS_CUDA_TRY(cudaStreamWaitEvent(t->st, t->copy_ev, 0));
+    rc = enqueue_track(t, nframes, t->d_prev, t->d_uright_in, t->d_F, t->d_boxes, t->d_nboxes, t->d_have, device_last(t), th, mono, check_orientation,
+                       nullptr, nullptr, t->st);
     if (rc != SGS_OK) return rc;
-    rc = download_track_results(t, B, kps_out, desc_out, u_right_out, counts_out, cur_mp_out, nmatches_out, st);
-    if (rc != SGS_OK) return rc;
-    SGS_CUDA_TRY(cudaStreamSynchronize(st));
-    return SGS_OK;
+    return download_results(t, nframes, out);
 }
 
 SGS_API sgs_extractor* sgs_tracker_extractor(sgs_tracker* t) { return t ? t->ex.get() : nullptr; }
@@ -504,45 +553,45 @@ SGS_API sgs_lk* sgs_tracker_lk(sgs_tracker* t) { return t ? t->lk.get() : nullpt
 
 SGS_API int sgs_tracker_lk_device(sgs_tracker* t, const uint8_t* d_frames, int nframes, size_t frame_stride, int pitch, const int32_t* d_prev_index,
                                   void* stream) {
-    if (!t || !d_frames || !d_prev_index) return bad("sgs_tracker_lk_device: NULL argument");
-    if (nframes < 1 || nframes > t->last_nframes) return bad("sgs_tracker_lk_device: nframes exceeds the last extract call");
-    const sgs_keypoint* d_kps; const uint8_t* d_desc; const int32_t* d_cnt; int cap = 0;
-    sgs_extractor_results_device(t->ex.get(), &d_kps, &d_desc, &d_cnt, &cap);
-    return sgs_lk_track_batch_device(t->lk.get(), d_frames, nullptr, d_prev_index, nframes, frame_stride, pitch, d_kps, d_cnt, cap, t->d_prev,
+    const char* const fn = "sgs_tracker_lk_device";
+    if (!t || !d_frames || !d_prev_index) return bad(fn, "NULL argument");
+    if (!frames_ok(fn, nframes, t->last_nframes)) return SGS_ERR_INVALID;
+    const Extracted ex = extracted(t);
+    return sgs_lk_track_batch_device(t->lk.get(), d_frames, nullptr, d_prev_index, nframes, frame_stride, pitch, ex.kps, ex.n, ex.cap, t->d_prev,
                                      stream ? stream : (void*)t->st);
 }
 
 SGS_API int sgs_tracker_fundamental_device(sgs_tracker* t, int nframes, const sgs_rect* d_boxes, const int32_t* d_nboxes, const uint8_t* d_have_dyn,
                                            const int32_t* d_prev_index, void* stream) {
-    if (!t || !d_prev_index) return bad("sgs_tracker_fundamental_device: NULL argument");
-    if (!d_nboxes) d_nboxes = t->d_nboxes;       // NULL: the tracker's own arrays, filled by sgs_tracker_detect_device
-    if (!d_have_dyn) d_have_dyn = t->d_have;
-    if (nframes < 1 || nframes > t->last_nframes) return bad("sgs_tracker_fundamental_device: nframes exceeds the last extract call");
-    const sgs_keypoint* d_kps; const uint8_t* d_desc; const int32_t* d_cnt; int cap = 0;
-    sgs_extractor_results_device(t->ex.get(), &d_kps, &d_desc, &d_cnt, &cap);
-    // parameters of the reference call: FM_RANSAC, 1.0, 0.99 (src/Frame.cc:470,472); OpenCV's default of 1000 iterations
-    return sgs_fundamental_batch_device(d_kps, t->d_prev, d_cnt, cap, nframes, d_boxes ? d_boxes : t->d_boxes, d_nboxes, d_have_dyn, t->max_boxes,
-                                        d_prev_index, 1.0, 0.99, 1000, t->d_Fgpu, t->d_finfo, stream ? stream : (void*)t->st);
+    const char* const fn = "sgs_tracker_fundamental_device";
+    if (!t || !d_prev_index) return bad(fn, "NULL argument");
+    if (!frames_ok(fn, nframes, t->last_nframes)) return SGS_ERR_INVALID;
+    const Extracted ex = extracted(t);
+    // NULL boxes: the tracker's own arrays, filled by sgs_tracker_detect_device.  Parameters of the reference call: FM_RANSAC, 1.0, 0.99
+    // (src/Frame.cc:470,472); OpenCV's default of 1000 iterations
+    return sgs_fundamental_batch_device(ex.kps, t->d_prev, ex.n, ex.cap, nframes, d_boxes ? d_boxes : t->d_boxes, d_nboxes ? d_nboxes : t->d_nboxes,
+                                        d_have_dyn ? d_have_dyn : t->d_have, t->max_boxes, d_prev_index, 1.0, 0.99, 1000, t->d_Fgpu, t->d_finfo,
+                                        stream ? stream : (void*)t->st);
 }
 
 SGS_API int sgs_tracker_stereo_device(sgs_tracker* t, int nframes, const float* d_depth, size_t depth_frame_stride, int depth_pitch, void* stream) {
-    if (!t || !d_depth) return bad("sgs_tracker_stereo_device: NULL argument");
-    if (nframes < 1 || nframes > t->last_nframes) return bad("sgs_tracker_stereo_device: nframes exceeds the last extract call");
-    const sgs_keypoint* d_kps; const uint8_t* d_desc; const int32_t* d_cnt; int cap = 0;
-    sgs_extractor_results_device(t->ex.get(), &d_kps, &d_desc, &d_cnt, &cap);
-    return sgs_stereo_from_depth_batch_device(d_kps, nullptr, d_cnt, cap, nframes, d_depth, depth_frame_stride, depth_pitch, t->cam.bf, t->d_uright_in, nullptr,
+    const char* const fn = "sgs_tracker_stereo_device";
+    if (!t || !d_depth) return bad(fn, "NULL argument");
+    if (!frames_ok(fn, nframes, t->last_nframes)) return SGS_ERR_INVALID;
+    const Extracted ex = extracted(t);
+    return sgs_stereo_from_depth_batch_device(ex.kps, nullptr, ex.n, ex.cap, nframes, d_depth, depth_frame_stride, depth_pitch, t->cam.bf, t->d_uright_in, nullptr,
                                               stream ? stream : (void*)t->st);
 }
 
 SGS_API int sgs_tracker_fundamental_device_ptr(const sgs_tracker* t, const double** d_F, const int32_t** d_info) {
-    if (!t) return bad("sgs_tracker_fundamental_device_ptr: NULL");
+    if (!t) return bad("sgs_tracker_fundamental_device_ptr", "NULL");
     if (d_F) *d_F = t->d_Fgpu;
     if (d_info) *d_info = t->d_finfo;
     return SGS_OK;
 }
 
 SGS_API int sgs_tracker_prev_xy_device(const sgs_tracker* t, const float** d_prev_xy) {
-    if (!t || !d_prev_xy) return bad("sgs_tracker_prev_xy_device: NULL");
+    if (!t || !d_prev_xy) return bad("sgs_tracker_prev_xy_device", "NULL");
     *d_prev_xy = t->d_prev;
     return SGS_OK;
 }
@@ -552,48 +601,45 @@ SGS_API int sgs_tracker_track_lk(sgs_tracker* t, int nframes, const int32_t* pre
                                  const uint8_t* last_flags, const int32_t* last_octave, const float* last_angle, const int32_t* last_n,
                                  const float* tcw_cur, const float* tcw_last, float th, int mono, int check_orientation, sgs_keypoint* kps_out,
                                  uint8_t* desc_out, float* u_right_out, int32_t* counts_out, int32_t* cur_mp_out, int32_t* nmatches_out) {
-    if (!t || !prev_index) return bad("sgs_tracker_track_lk: NULL argument");
-    if (nframes < 1 || nframes > t->last_nframes) return bad("sgs_tracker_track_lk: nframes exceeds the last sgs_tracker_extract call");
+    const char* const fn = "sgs_tracker_track_lk";
+    LastFrame last;
+    last.xyz = last_xyz; last.desc = last_desc; last.flags = last_flags; last.octave = last_octave; last.angle = last_angle; last.n = last_n;
+    last.tcw_cur = tcw_cur; last.tcw_last = tcw_last;
+    HostOutputs out;
+    out.kps = kps_out; out.desc = desc_out; out.u_right = u_right_out; out.counts = counts_out; out.cur_mp = cur_mp_out; out.nmatches = nmatches_out;
+    if (!t || !prev_index || !u_right || !nboxes || !have_dyn || !last.complete() || !out.complete()) return bad(fn, "NULL argument");
+    if (!frames_ok(fn, nframes, t->last_nframes, prev_index)) return SGS_ERR_INVALID;
     SGS_CUDA_TRY(cudaSetDevice(t->device));
-    for (int f = 0; f < nframes; ++f) if (prev_index[f] < 0 || prev_index[f] >= nframes) return bad("sgs_tracker_track_lk: prev_index out of range");
-    if (!u_right || !nboxes || !have_dyn || !last_xyz || !last_desc || !last_flags || !last_octave || !last_angle || !last_n || !tcw_cur ||
-        !tcw_last || !kps_out || !desc_out || !counts_out || !cur_mp_out || !nmatches_out) return bad("sgs_tracker_track_lk: NULL argument");
-    const size_t B = nframes;
-    cudaStream_t st = t->st;
-    // what LK and the F estimate need goes first on the compute stream; the bulk of the inputs (last-frame points, u_right) is uploaded on
-    // the copy stream while those kernels run
-    SGS_CUDA_TRY(cudaMemcpyAsync(t->d_pidx, prev_index, sizeof(int32_t) * B, cudaMemcpyHostToDevice, st));
-    if (F) SGS_CUDA_TRY(cudaMemcpyAsync(t->d_F, F, B * 72, cudaMemcpyHostToDevice, st));
-    if (boxes) SGS_CUDA_TRY(cudaMemcpyAsync(t->d_boxes, boxes, B * t->max_boxes * sizeof(sgs_rect), cudaMemcpyHostToDevice, st));
-    SGS_CUDA_TRY(cudaMemcpyAsync(t->d_nboxes, nboxes, B * 4, cudaMemcpyHostToDevice, st)); SGS_CUDA_TRY(cudaMemcpyAsync(t->d_have, have_dyn, B, cudaMemcpyHostToDevice, st));
-    int rc = upload_track_inputs(t, B, u_right, last_xyz, last_desc, last_flags, last_octave, last_angle, last_n, tcw_cur, tcw_last, t->copy_st);
+    TrackInputs in{last};
+    in.u_right = u_right; in.prev_index = prev_index; in.F = F; in.boxes = boxes; in.nboxes = nboxes; in.have_dyn = have_dyn;
+    int rc = stage_host_inputs(t, nframes, in);
     if (rc != SGS_OK) return rc;
-    SGS_CUDA_TRY(cudaEventRecord(t->copy_ev, t->copy_st));
     const uint8_t* d_frames; int pitch; size_t fstride;
     sgs_extractor_level0_device(t->ex.get(), &d_frames, &pitch, &fstride);
-    rc = sgs_tracker_lk_device(t, d_frames, nframes, fstride, pitch, t->d_pidx, st);
+    rc = sgs_tracker_lk_device(t, d_frames, nframes, fstride, pitch, t->d_pidx, t->st);
     if (rc != SGS_OK) return rc;
     if (!F) {       // F == NULL: findFundamentalMat on the device, previous-frame boxes = the boxes of row prev_index[f]
-        rc = sgs_tracker_fundamental_device(t, nframes, t->d_boxes, t->d_nboxes, t->d_have, t->d_pidx, st);
+        rc = sgs_tracker_fundamental_device(t, nframes, t->d_boxes, t->d_nboxes, t->d_have, t->d_pidx, t->st);
         if (rc != SGS_OK) return rc;
     }
-    SGS_CUDA_TRY(cudaStreamWaitEvent(st, t->copy_ev, 0));
-    rc = sgs_tracker_track_device(t, nframes, nullptr, t->d_uright_in, F ? t->d_F : nullptr, t->d_boxes, t->d_nboxes, t->d_have, t->d_lxyz, t->d_ldesc, t->d_lflags,
-                                  t->d_loct, t->d_lang, t->d_ln, t->d_tc, t->d_tl, th, mono, check_orientation, st);
+    SGS_CUDA_TRY(cudaStreamWaitEvent(t->st, t->copy_ev, 0));
+    rc = enqueue_track(t, nframes, t->d_prev, t->d_uright_in, F ? t->d_F : t->d_Fgpu, t->d_boxes, t->d_nboxes, t->d_have, device_last(t), th, mono,
+                       check_orientation, nullptr, nullptr, t->st);
     if (rc != SGS_OK) return rc;
-    rc = download_track_results(t, B, kps_out, desc_out, u_right_out, counts_out, cur_mp_out, nmatches_out, st);
-    if (rc != SGS_OK) return rc;
-    SGS_CUDA_TRY(cudaStreamSynchronize(st));
-    return SGS_OK;
+    return download_results(t, nframes, out);
 }
 
 SGS_API int sgs_tracker_pose_chain_device(sgs_tracker* t, const sgs_posechain_batch* a, int nframes, void* stream) {
-    if (!t || !a) return bad("sgs_tracker_pose_chain_device: NULL");
-    if (!a->last_xyz || !a->last_desc || !a->last_flags || !a->last_octave || !a->last_angle || !a->last_n || !a->tcw_cur || !a->tcw_last || !a->mp_xyz || !a->mp_normal ||
-        !a->mp_min_dist || !a->mp_max_dist || !a->mp_desc || !a->mp_valid || !a->mp_obs || !a->mp_n || !a->tcw_motion || !a->tcw_final || !a->f_mp || !a->outlier || !a->stats)
-        return bad("sgs_tracker_pose_chain_device: NULL array");
-    if (nframes < 1 || nframes > t->last_nframes) return bad("sgs_tracker_pose_chain_device: nframes exceeds the last track call");
-    if (a->mp_cap < 1) return bad("sgs_tracker_pose_chain_device: mp_cap < 1");
+    if (!t || !a) return bad("sgs_tracker_pose_chain_device", "NULL");
+    const char* const fn = "sgs_tracker_pose_chain_device";
+    LastFrame last;
+    last.xyz = a->last_xyz; last.desc = a->last_desc; last.flags = a->last_flags; last.octave = a->last_octave; last.angle = a->last_angle;
+    last.n = a->last_n; last.tcw_cur = a->tcw_cur; last.tcw_last = a->tcw_last;
+    if (!last.complete() || !a->mp_xyz || !a->mp_normal || !a->mp_min_dist || !a->mp_max_dist || !a->mp_desc || !a->mp_valid || !a->mp_obs || !a->mp_n ||
+        !a->tcw_motion || !a->tcw_final || !a->f_mp || !a->outlier || !a->stats)
+        return bad(fn, "NULL array");
+    if (!frames_ok(fn, nframes, t->last_nframes)) return SGS_ERR_INVALID;
+    if (a->mp_cap < 1) return bad(fn, "mp_cap < 1");
     SGS_CUDA_TRY(cudaSetDevice(t->device));
     cudaStream_t st = stream ? (cudaStream_t)stream : t->st;
     const size_t B = t->max_batch, K = t->cap, M = a->mp_cap;
@@ -601,11 +647,10 @@ SGS_API int sgs_tracker_pose_chain_device(sgs_tracker* t, const sgs_posechain_ba
         t->chain_mp_cap = 0;
         t->mt_local.reset();
         sgs_matcher* mt_local = nullptr;
-        int rc = sgs_matcher_create(t->device, t->max_batch, t->cap, a->mp_cap, &mt_local);
+        const int rc = sgs_matcher_create(t->device, t->max_batch, t->cap, a->mp_cap, &mt_local);
         t->mt_local.reset(mt_local);
         if (rc != SGS_OK) return rc;
         HandleResources& R = t->res;
-        const char* const fn = "sgs_tracker_pose_chain_device";
         // 16 bytes of slack past the end of every array, as in sgs_tracker_create
         SGS_CUDA_TRY_AT(fn, R.regrow(&t->d_enable, B + 16)); SGS_CUDA_TRY_AT(fn, R.regrow(&t->d_nm2, B * 4 + 16)); SGS_CUDA_TRY_AT(fn, R.regrow(&t->d_obs, B * K + 16));
         SGS_CUDA_TRY_AT(fn, R.regrow(&t->d_seen, B * M + 16)); SGS_CUDA_TRY_AT(fn, R.regrow(&t->d_ninl, B * 4 + 16)); SGS_CUDA_TRY_AT(fn, R.regrow(&t->d_nml, B * 4 + 16));
@@ -615,15 +660,10 @@ SGS_API int sgs_tracker_pose_chain_device(sgs_tracker* t, const sgs_posechain_ba
         t->chain_mp_cap = a->mp_cap;
     }
     const int F = nframes, cap = t->cap;
-    // 1. the wide-window retry of the frames with fewer than 20 matches
+    // 1. the wide-window retry of the frames with fewer than 20 matches: the search of the track call with 2 th, on those frames, into its own counts
     chain_retry_kernel<<<F, 256, 0, st>>>(t->d_nm, cap, t->d_mp, t->d_enable, a->stats);
-    sgs_lastframe_batch lf;
-    std::memset(&lf, 0, sizeof lf);
-    lf.cam = t->cam;
-    lf.cur_kps = t->keys_un; lf.cur_desc = t->d_desc2; lf.cur_uright = t->d_uright2; lf.cur_n = t->d_cnt2;
-    lf.last_xyz = a->last_xyz; lf.last_desc = a->last_desc; lf.last_flags = a->last_flags; lf.last_octave = a->last_octave; lf.last_angle = a->last_angle; lf.last_n = a->last_n;
-    lf.tcw_cur = a->tcw_cur; lf.tcw_last = a->tcw_last; lf.th = 2.f * a->th; lf.mono = a->mono; lf.check_orientation = a->check_orientation;
-    lf.cur_mp = t->d_mp; lf.nmatches = t->d_nm2; lf.ncand = (uint64_t*)t->d_ncand2; lf.frame_enable = t->d_enable;
+    sgs_lastframe_batch lf = lastframe_search(t, last, 2.f * a->th, a->mono, a->check_orientation);
+    lf.nmatches = t->d_nm2; lf.ncand = (uint64_t*)t->d_ncand2; lf.frame_enable = t->d_enable;
     SGS_CUDA_TRY(cudaMemsetAsync(t->d_ncand2, 0, (size_t)F * 8, st));
     SGS_CUDA_TRY(cudaMemsetAsync(t->d_nm2, 0, (size_t)F * 4, st));
     int rc = sgs_match_project_lastframe_batch_device(t->mt.get(), &lf, F, st);
@@ -674,13 +714,14 @@ SGS_API int sgs_tracker_pose_chain_device(sgs_tracker* t, const sgs_posechain_ba
 // the next sgs_tracker_fundamental_device / _track_device call on the tracker's stream is NOT ordered after -- use sgs_tracker_step for that).
 SGS_API int sgs_tracker_detect_device(sgs_tracker* t, sgs_detector* det, const uint8_t* d_rgb, int64_t frame_stride, int pitch, int width, int height, int nframes,
                                       void* stream) {
-    if (!t || !det || !d_rgb) return bad("sgs_tracker_detect_device: NULL argument");
-    if (nframes < 1 || nframes > t->max_batch) return bad("sgs_tracker_detect_device: nframes outside [1,max_batch]");
+    const char* const fn = "sgs_tracker_detect_device";
+    if (!t || !det || !d_rgb) return bad(fn, "NULL argument");
+    if (!frames_ok(fn, nframes, t->max_batch)) return SGS_ERR_INVALID;
     return sgs_detector_detect_device(det, d_rgb, frame_stride, pitch, width, height, nframes, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, t->d_boxes, t->d_nboxes,
                                       t->d_have, t->max_boxes, t->d_det_status, stream ? stream : (void*)t->det_st);
 }
 SGS_API int sgs_tracker_boxes_device(const sgs_tracker* t, const sgs_rect** d_boxes, const int32_t** d_nboxes, const uint8_t** d_have_dyn) {
-    if (!t) return bad("sgs_tracker_boxes_device: NULL");
+    if (!t) return bad("sgs_tracker_boxes_device", "NULL");
     if (d_boxes) *d_boxes = t->d_boxes;
     if (d_nboxes) *d_nboxes = t->d_nboxes;
     if (d_have_dyn) *d_have_dyn = t->d_have;
@@ -698,20 +739,25 @@ SGS_API int sgs_tracker_step(sgs_tracker* t, sgs_detector* det, const uint8_t* g
                              const uint8_t* last_flags, const int32_t* last_octave, const float* last_angle, const int32_t* last_n, const float* tcw_cur,
                              const float* tcw_last, float th, int mono, int check_orientation, sgs_keypoint* kps_out, uint8_t* desc_out, float* u_right_out,
                              int32_t* counts_out, int32_t* cur_mp_out, int32_t* nmatches_out, sgs_rect* boxes_out, int32_t* nboxes_out, uint8_t* have_out) {
-    if (!t || !det || !gray || !rgb || !prev_index || !u_right || !last_xyz || !last_desc || !last_flags || !last_octave || !last_angle || !last_n || !tcw_cur ||
-        !tcw_last || !kps_out || !desc_out || !counts_out || !cur_mp_out || !nmatches_out) return bad("sgs_tracker_step: NULL argument");
-    if (nframes < 1 || nframes > t->max_batch) return bad("sgs_tracker_step: nframes outside [1,max_batch]");
-    if (rgb_pitch < t->width * 3 || rgb_stride < (size_t)rgb_pitch * t->height) return bad("sgs_tracker_step: rgb pitch / stride too small");
-    for (int f = 0; f < nframes; ++f) if (prev_index[f] < 0 || prev_index[f] >= nframes) return bad("sgs_tracker_step: prev_index out of range");
+    const char* const fn = "sgs_tracker_step";
+    LastFrame last;
+    last.xyz = last_xyz; last.desc = last_desc; last.flags = last_flags; last.octave = last_octave; last.angle = last_angle; last.n = last_n;
+    last.tcw_cur = tcw_cur; last.tcw_last = tcw_last;
+    HostOutputs out;
+    out.kps = kps_out; out.desc = desc_out; out.u_right = u_right_out; out.counts = counts_out; out.cur_mp = cur_mp_out; out.nmatches = nmatches_out;
+    out.boxes = boxes_out; out.nboxes = nboxes_out; out.have = have_out;
+    if (!t || !det || !gray || !rgb || !prev_index || !u_right || !last.complete() || !out.complete()) return bad(fn, "NULL argument");
+    if (!frames_ok(fn, nframes, t->max_batch, prev_index) || !rgb_layout_ok(t, fn, rgb_stride, rgb_pitch)) return SGS_ERR_INVALID;
     SGS_CUDA_TRY(cudaSetDevice(t->device));
-    const size_t B = nframes;
-    int rc = upload_rgb(t, rgb, rgb_stride, rgb_pitch, B);
+    int rc = upload_rgb(t, rgb, rgb_stride, rgb_pitch, nframes);
     if (rc != SGS_OK) return rc;
-    const StepFrames fr{t->d_rgb, (size_t)t->width * 3 * t->height, t->width * 3, t->det_st, gray, gray_stride, gray_pitch, nullptr, 0, 0, nullptr};
-    const StepInputs in{true, prev_index, u_right, last_xyz, last_desc, last_flags, last_octave, last_angle, last_n, tcw_cur, tcw_last};
-    rc = enqueue_step(t, det, fr, nframes, in, th, mono, check_orientation, t->st);
+    StepFrames fr = staged_rgb(t);
+    fr.gray = gray; fr.gray_stride = gray_stride; fr.gray_pitch = gray_pitch;
+    TrackInputs in{last};
+    in.u_right = u_right; in.prev_index = prev_index;
+    rc = enqueue_step(t, det, fr, nframes, in, true, th, mono, check_orientation, t->st);
     if (rc != SGS_OK) return rc;
-    return download_step(t, B, kps_out, desc_out, u_right_out, counts_out, cur_mp_out, nmatches_out, boxes_out, nboxes_out, have_out, nullptr, nullptr);
+    return download_results(t, nframes, out);
 }
 
 // The RGB-D front end (Tracking::GrabImageRGBD + the RGB-D Frame constructor + the first matcher call) on device frames; see sgs_abi.h.
@@ -721,17 +767,21 @@ SGS_API int sgs_tracker_step_rgbd_device(sgs_tracker* t, sgs_detector* det, cons
                                          const float* last_angle, const int32_t* last_n, const float* tcw_cur, const float* tcw_last, float th, int mono,
                                          int check_orientation, void* stream) {
     const char* const fn = "sgs_tracker_step_rgbd_device";
-    if (!t || !det || !d_rgb || !d_depth || !fmt || !d_prev_index || !last_xyz || !last_desc || !last_flags || !last_octave || !last_angle || !last_n ||
-        !tcw_cur || !tcw_last) return bad("sgs_tracker_step_rgbd_device: NULL argument");
-    int rc = check_rgbd_args(t, fn, fmt, nframes, rgb_stride, rgb_pitch, depth_stride, depth_pitch, d_depth);
-    if (rc != SGS_OK) return rc;
+    LastFrame last;
+    last.xyz = last_xyz; last.desc = last_desc; last.flags = last_flags; last.octave = last_octave; last.angle = last_angle; last.n = last_n;
+    last.tcw_cur = tcw_cur; last.tcw_last = tcw_last;
+    if (!t || !det || !d_rgb || !d_depth || !fmt || !d_prev_index || !last.complete()) return bad(fn, "NULL argument");
+    if (!frames_ok(fn, nframes, t->max_batch) || !rgb_layout_ok(t, fn, rgb_stride, rgb_pitch) ||
+        !depth_args_ok(t, fn, fmt, depth_stride, depth_pitch, d_depth)) return SGS_ERR_INVALID;
     SGS_CUDA_TRY(cudaSetDevice(t->device));
-    rc = ensure_rgbd_buffers(t, 0);
+    const int rc = ensure_rgbd_buffers(t, 0);
     if (rc != SGS_OK) return rc;
     cudaStream_t st = stream ? (cudaStream_t)stream : t->st;
-    const StepFrames fr{d_rgb, rgb_stride, rgb_pitch, st, nullptr, 0, 0, d_depth, depth_stride, depth_pitch, fmt};
-    const StepInputs in{false, d_prev_index, nullptr, last_xyz, last_desc, last_flags, last_octave, last_angle, last_n, tcw_cur, tcw_last};
-    return enqueue_step(t, det, fr, nframes, in, th, mono, check_orientation, st);
+    StepFrames fr{d_rgb, rgb_stride, rgb_pitch, st};
+    fr.d_depth = d_depth; fr.depth_stride = depth_stride; fr.depth_pitch = depth_pitch; fr.fmt = fmt;
+    TrackInputs in{last};
+    in.prev_index = d_prev_index;
+    return enqueue_step(t, det, fr, nframes, in, false, th, mono, check_orientation, st);
 }
 
 // The same from host buffers: one upload of the colour frames (detector and gray conversion read it), the raw depth as given, one synchronisation.
@@ -743,34 +793,34 @@ SGS_API int sgs_tracker_step_rgbd(sgs_tracker* t, sgs_detector* det, const uint8
                                   int32_t* cur_mp_out, int32_t* nmatches_out, sgs_rect* boxes_out, int32_t* nboxes_out, uint8_t* have_out,
                                   sgs_keypoint* kps_un_out, float* depth_out) {
     const char* const fn = "sgs_tracker_step_rgbd";
-    if (!t || !det || !rgb || !depth || !fmt || !prev_index || !last_xyz || !last_desc || !last_flags || !last_octave || !last_angle || !last_n || !tcw_cur ||
-        !tcw_last || !kps_out || !desc_out || !counts_out || !cur_mp_out || !nmatches_out) return bad("sgs_tracker_step_rgbd: NULL argument");
-    int rc = check_rgbd_args(t, fn, fmt, nframes, rgb_stride, rgb_pitch, depth_stride, depth_pitch, depth);
-    if (rc != SGS_OK) return rc;
-    for (int f = 0; f < nframes; ++f) if (prev_index[f] < 0 || prev_index[f] >= nframes) return bad("sgs_tracker_step_rgbd: prev_index out of range");
+    LastFrame last;
+    last.xyz = last_xyz; last.desc = last_desc; last.flags = last_flags; last.octave = last_octave; last.angle = last_angle; last.n = last_n;
+    last.tcw_cur = tcw_cur; last.tcw_last = tcw_last;
+    HostOutputs out;
+    out.kps = kps_out; out.desc = desc_out; out.u_right = u_right_out; out.counts = counts_out; out.cur_mp = cur_mp_out; out.nmatches = nmatches_out;
+    out.boxes = boxes_out; out.nboxes = nboxes_out; out.have = have_out; out.kps_un = kps_un_out; out.depth = depth_out;
+    if (!t || !det || !rgb || !depth || !fmt || !prev_index || !last.complete() || !out.complete()) return bad(fn, "NULL argument");
+    if (!frames_ok(fn, nframes, t->max_batch, prev_index) || !rgb_layout_ok(t, fn, rgb_stride, rgb_pitch) ||
+        !depth_args_ok(t, fn, fmt, depth_stride, depth_pitch, depth)) return SGS_ERR_INVALID;
     SGS_CUDA_TRY(cudaSetDevice(t->device));
-    const size_t B = nframes, row = (size_t)t->width * (fmt->depth_type == 0 ? 2 : 4);
-    rc = ensure_rgbd_buffers(t, row * t->height);
+    const size_t row = (size_t)t->width * (fmt->depth_type == 0 ? 2 : 4);
+    int rc = ensure_rgbd_buffers(t, row * t->height);
     if (rc != SGS_OK) return rc;
-    rc = upload_rgb(t, rgb, rgb_stride, rgb_pitch, B);
+    rc = upload_rgb(t, rgb, rgb_stride, rgb_pitch, nframes);
     if (rc != SGS_OK) return rc;
-    if (depth_stride == (size_t)depth_pitch * t->height) {
-        SGS_CUDA_TRY(cudaMemcpy2DAsync(t->d_depth_raw, row, depth, depth_pitch, row, (size_t)t->height * B, cudaMemcpyHostToDevice, t->st));
-    } else {
-        for (size_t f = 0; f < B; ++f)
-            SGS_CUDA_TRY(cudaMemcpy2DAsync(t->d_depth_raw + f * row * t->height, row, (const uint8_t*)depth + f * depth_stride, depth_pitch, row, t->height,
-                                           cudaMemcpyHostToDevice, t->st));
-    }
-    const StepFrames fr{t->d_rgb, (size_t)t->width * 3 * t->height, t->width * 3, t->det_st, nullptr, 0, 0, t->d_depth_raw, row * t->height, (int)row, fmt};
-    const StepInputs in{true, prev_index, nullptr, last_xyz, last_desc, last_flags, last_octave, last_angle, last_n, tcw_cur, tcw_last};
-    rc = enqueue_step(t, det, fr, nframes, in, th, mono, check_orientation, t->st);
+    SGS_CUDA_TRY(upload_frames(t->d_depth_raw, depth, depth_stride, depth_pitch, row, t->height, nframes, t->st));
+    StepFrames fr = staged_rgb(t);
+    fr.d_depth = t->d_depth_raw; fr.depth_stride = row * t->height; fr.depth_pitch = (int)row; fr.fmt = fmt;
+    TrackInputs in{last};
+    in.prev_index = prev_index;      // no u_right: the step computes it from the depth
+    rc = enqueue_step(t, det, fr, nframes, in, true, th, mono, check_orientation, t->st);
     if (rc != SGS_OK) return rc;
-    return download_step(t, B, kps_out, desc_out, u_right_out, counts_out, cur_mp_out, nmatches_out, boxes_out, nboxes_out, have_out, kps_un_out, depth_out);
+    return download_results(t, nframes, out);
 }
 
 SGS_API int sgs_tracker_frame_device(const sgs_tracker* t, const sgs_keypoint** d_kps_un, const float** d_depth) {
-    if (!t) return bad("sgs_tracker_frame_device: NULL handle");
-    if (!t->d_kpsun2) return bad("sgs_tracker_frame_device: no RGB-D step has run on this handle");
+    if (!t) return bad("sgs_tracker_frame_device", "NULL handle");
+    if (!t->d_kpsun2) return bad("sgs_tracker_frame_device", "no RGB-D step has run on this handle");
     if (d_kps_un) *d_kps_un = t->d_kpsun2;
     if (d_depth) *d_depth = t->d_dz2;
     return SGS_OK;
