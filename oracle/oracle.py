@@ -206,15 +206,16 @@ def bf_match(q, t):
 
 
 class FrameArrays:
-    """Keeps the numpy arrays behind an SgoFrame alive."""
+    """Keeps the numpy arrays behind an SgoFrame alive.  bounds = (min_x, min_y, max_x, max_y) (Frame::ComputeImageBounds), default (0, 0, w, h)."""
 
-    def __init__(self, keysUn, uRight, desc, w, h, fx, fy, cx, cy, bf, scaleFactors):
+    def __init__(self, keysUn, uRight, desc, w, h, fx, fy, cx, cy, bf, scaleFactors, bounds=None):
         self.keysUn = np.ascontiguousarray(keysUn, KP_DTYPE)
         self.uRight = np.ascontiguousarray(uRight, np.float32)
         self.desc = np.ascontiguousarray(desc, np.uint8)
         self.scaleFactors = np.ascontiguousarray(scaleFactors, np.float32)
+        b = (0.0, 0.0, float(w), float(h)) if bounds is None else tuple(float(v) for v in bounds)
         self.c = SgoFrame(len(self.keysUn), self.keysUn.ctypes.data, self.uRight.ctypes.data, self.desc.ctypes.data,
-                          0.0, 0.0, float(w), float(h), fx, fy, cx, cy, bf, len(self.scaleFactors),
+                          *b, fx, fy, cx, cy, bf, len(self.scaleFactors),
                           self.scaleFactors.ctypes.data, float(logf(self.scaleFactors[1])) if len(self.scaleFactors) > 1 else 0.0)
 
 

@@ -77,6 +77,15 @@ class LastFrameBatch(C.Structure):
                 ('cur_mp', C.c_void_p), ('cur_mp_obs_in', C.c_void_p), ('nmatches', C.c_void_p), ('ncand', C.c_void_p), ('frame_enable', C.c_void_p)]
 
 
+class KeyFrameBatch(C.Structure):
+    _fields_ = [('cam', Camera),
+                ('cur_kps', C.c_void_p), ('cur_desc', C.c_void_p), ('cur_uright', C.c_void_p), ('cur_n', C.c_void_p),
+                ('kf_xyz', C.c_void_p), ('kf_desc', C.c_void_p), ('kf_valid', C.c_void_p), ('kf_angle', C.c_void_p),
+                ('kf_min_dist', C.c_void_p), ('kf_max_dist', C.c_void_p), ('kf_n', C.c_void_p), ('tcw_cur', C.c_void_p),
+                ('th', C.c_float), ('orb_dist', C.c_int32), ('check_orientation', C.c_int32),
+                ('cur_mp', C.c_void_p), ('nmatches', C.c_void_p), ('ncand', C.c_void_p)]
+
+
 class PoseOptBatch(C.Structure):
     _fields_ = [('cam', Camera), ('tcw_in', C.c_void_p), ('kps', C.c_void_p), ('uright', C.c_void_p), ('n', C.c_void_p), ('cap', C.c_int32),
                 ('has_mp', C.c_void_p), ('mp_index', C.c_void_p), ('points_xyz', C.c_void_p), ('point_cap', C.c_int32), ('inv_level_sigma2', C.c_float * 16),
@@ -333,15 +342,16 @@ def hamming_bf_device(dq, nq, dt, nt, d_idx, d_best, d_second, d_scratch=0, stre
 
 
 class HostFrame:
-    """numpy arrays behind an sgs_frame_view."""
+    """numpy arrays behind an sgs_frame_view.  bounds = (min_x, min_y, max_x, max_y) (sgs_image_bounds), default (0, 0, w, h)."""
 
-    def __init__(self, keysUn, uRight, desc, w, h, fx, fy, cx, cy, bf, scaleFactors):
+    def __init__(self, keysUn, uRight, desc, w, h, fx, fy, cx, cy, bf, scaleFactors, bounds=None):
         self.keysUn = np.ascontiguousarray(keysUn, KP_DTYPE)
         self.uRight = np.ascontiguousarray(uRight, np.float32)
         self.desc = np.ascontiguousarray(desc, np.uint8)
         self.scaleFactors = np.ascontiguousarray(scaleFactors, np.float32)
+        b = (0.0, 0.0, float(w), float(h)) if bounds is None else tuple(float(v) for v in bounds)
         self.c = FrameView(len(self.keysUn), self.keysUn.ctypes.data, self.uRight.ctypes.data, self.desc.ctypes.data,
-                           0.0, 0.0, float(w), float(h), fx, fy, cx, cy, bf, len(self.scaleFactors), self.scaleFactors.ctypes.data)
+                           *b, fx, fy, cx, cy, bf, len(self.scaleFactors), self.scaleFactors.ctypes.data)
 
 
 def match_project_lastframe(cur, Tcw_cur, Tcw_last, last_has_mp, last_xyz, last_desc, last_obs, last_octave, last_angle, th,
@@ -410,9 +420,10 @@ def dynreject_batch_device(d_kps, d_desc, d_counts, cap, nframes, d_prev, d_F, d
                                            d_kps_out, d_desc_out, d_counts_out, d_keep, stream))
 
 
-def make_camera(w, h, cam, scale_factors):
+def make_camera(w, h, cam, scale_factors, bounds=None):
+    """sgs_camera with the image bounds (min_x, min_y, max_x, max_y), default (0, 0, w, h)."""
     c = Camera()
-    c.min_x, c.min_y, c.max_x, c.max_y = 0.0, 0.0, float(w), float(h)
+    c.min_x, c.min_y, c.max_x, c.max_y = (0.0, 0.0, float(w), float(h)) if bounds is None else tuple(float(v) for v in bounds)
     c.fx, c.fy, c.cx, c.cy, c.bf = cam['fx'], cam['fy'], cam['cx'], cam['cy'], cam['bf']
     c.nlevels = len(scale_factors)
     for i, v in enumerate(scale_factors):

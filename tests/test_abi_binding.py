@@ -16,7 +16,7 @@ INCLUDE = os.path.join(ROOT, 'include')
 STRUCTS = {B.OrbParams: 'sgs_orb_params', B.Settings: 'sgs_settings', B.FrameView: 'sgs_frame_view', B.Camera: 'sgs_camera',
            B.LastFrameBatch: 'sgs_lastframe_batch', B.PoseOptBatch: 'sgs_poseopt_batch', B.PoseChainBatch: 'sgs_posechain_batch',
            B.FuseBatch: 'sgs_fuse_batch', B.InitBatch: 'sgs_init_batch', B.BowBatch: 'sgs_bow_batch', B.FrustumBatch: 'sgs_frustum_batch',
-           B.LocalMapBatch: 'sgs_localmap_batch'}
+           B.LocalMapBatch: 'sgs_localmap_batch', B.KeyFrameBatch: 'sgs_keyframe_batch'}
 # numpy dtype -> (C struct, C member of each dtype field where the names differ)
 DTYPES = {'KP_DTYPE': (B.KP_DTYPE, 'sgs_keypoint', {}), 'OBJ_DTYPE': (B.OBJ_DTYPE, 'sgs_object2d', {k: 'rect.' + k for k in 'xywh'})}
 

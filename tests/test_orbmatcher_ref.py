@@ -4,6 +4,8 @@ from the reference tree against stand-ins for cv::Mat / cv::KeyPoint and for the
 parity tests, and the oracle's restatement must return the same number of matches and the same map point for every keypoint.  This is what makes the
 matcher control flow (window search, best / second-best with the ratio test, level gates, stereo gate, rotation histogram, claim rules) a pinned part of
 the oracle rather than the builder's reading of it.  The cv::Mat arithmetic inside the stand-in follows the rules probed with cv2 (tests/golden/frustum.npz).
+The constructed cases of tests/match_cases.py (claim pile-ups, ratio flips, steals, image bounds, gate and histogram edges) run through the same
+reference calls, and each case's proof checks on the result that the order-dependent path it was built for was taken.
 No device needed.  Skipped only when the library was never built (the reference tree is absent AND no prebuilt copy travelled)."""
 import ctypes as C
 import os
@@ -11,6 +13,7 @@ import os
 import numpy as np
 import pytest
 
+import match_cases as MC
 import oracle as O
 import scenarios as S
 
@@ -32,12 +35,13 @@ def _p(a):
 
 def _cam(s):
     c = s['cam']
-    return np.array([c['fx'], c['fy'], c['cx'], c['cy'], c['bf'], 0, 0, s['w'], s['h']], np.float32)
+    b = s.get('bounds', (0, 0, s['w'], s['h']))
+    return np.array([c['fx'], c['fy'], c['cx'], c['cy'], c['bf'], *b], np.float32)
 
 
 def _frame(s):
     c = s['cam']
-    return O.FrameArrays(s['kps'], s['uright'], s['desc'], s['w'], s['h'], c['fx'], c['fy'], c['cx'], c['cy'], c['bf'], s['sf'])
+    return O.FrameArrays(s['kps'], s['uright'], s['desc'], s['w'], s['h'], c['fx'], c['fy'], c['cx'], c['cy'], c['bf'], s['sf'], bounds=s.get('bounds'))
 
 
 def ref_last(L, s, th, mono, check_ori, cur_mp=None, cur_obs=None):
@@ -52,6 +56,91 @@ def ref_last(L, s, th, mono, check_ori, cur_mp=None, cur_obs=None):
     nm = L.ref_search_by_projection_last(n, _p(kps), _p(ur), _p(d), _p(cam), len(sf), _p(sf), _p(Tc), _p(Tl), len(has), _p(has), _p(xyz), _p(ld), _p(lo), _p(loct), _p(la),
                                          C.c_float(th), int(mono), int(check_ori), _p(mp), _p(ob))
     return nm, mp
+
+
+def _cur(s):
+    return (np.ascontiguousarray(s['kps'], O.KP_DTYPE), np.ascontiguousarray(s['uright'], np.float32), np.ascontiguousarray(s['desc'], np.uint8),
+            np.ascontiguousarray(s['sf'], np.float32), _cam(s))
+
+
+def ref_local(L, s, th, ratio, id_base=7):
+    """The reference's SearchByProjection(F, vpMapPoints, th): (nmatches, f_mp, f_obs) from the scenario's f_mp / f_obs."""
+    kps, ur, d, sf, cam = _cur(s)
+    mp = np.ascontiguousarray(s['f_mp'], np.int32).copy(); ob = np.ascontiguousarray(s['f_obs'], np.uint8).copy()
+    arrs = [np.ascontiguousarray(s['inview'], np.uint8), np.ascontiguousarray(s['projx'], np.float32), np.ascontiguousarray(s['projy'], np.float32),
+            np.ascontiguousarray(s['projxr'], np.float32), np.ascontiguousarray(s['level'], np.int32), np.ascontiguousarray(s['viewcos'], np.float32),
+            np.ascontiguousarray(s['mp_desc'], np.uint8), np.ascontiguousarray(s['mp_obs'], np.uint8)]
+    nm = L.ref_search_by_projection_local(len(kps), _p(kps), _p(ur), _p(d), _p(cam), len(sf), _p(sf), len(arrs[0]), *[_p(x) for x in arrs], C.c_float(th), C.c_float(ratio),
+                                          id_base, _p(mp), _p(ob))
+    return nm, mp, ob
+
+
+def ref_kf(L, s, th, orb_dist, ori):
+    """The reference's SearchByProjection(Frame&, KeyFrame*, sAlreadyFound, th, ORBdist): (nmatches, cur_mp) from the scenario's cur_mp."""
+    L.ref_search_by_projection_kf.restype = C.c_int
+    kps, ur, d, sf, cam = _cur(s)
+    Tc = np.ascontiguousarray(s['Tcw_cur'], np.float32).reshape(16)
+    a = [np.ascontiguousarray(s['kf_valid'], np.uint8), np.ascontiguousarray(s['last_xyz'], np.float32), np.ascontiguousarray(s['last_desc'], np.uint8),
+         np.ascontiguousarray(s['last_angle'], np.float32), np.ascontiguousarray(s['min_dist'], np.float32), np.ascontiguousarray(s['max_dist'], np.float32)]
+    mp = np.ascontiguousarray(s['cur_mp'], np.int32).copy()
+    nm = L.ref_search_by_projection_kf(len(kps), _p(kps), _p(ur), _p(d), _p(cam), len(sf), _p(sf), _p(Tc), len(a[0]), *[_p(x) for x in a], C.c_float(th), orb_dist, int(ori), _p(mp))
+    return nm, mp
+
+
+def ref_sim3(L, s, T, nrm, matched, th):
+    """The reference's SearchByProjection(pKF, Scw, vpPoints, vpMatched, th) with Scw = T (scale 1): (nmatches, updated vpMatched)."""
+    L.ref_search_by_projection_sim3.restype = C.c_int
+    f32 = np.float32
+    kps, ur, d, sf, cam = _cur(s)
+    T = np.ascontiguousarray(T, f32)
+    a = [np.ascontiguousarray(s['kf_valid'], np.uint8), np.ascontiguousarray(s['last_xyz'], f32), np.ascontiguousarray(nrm, f32), np.ascontiguousarray(s['min_dist'], f32),
+         np.ascontiguousarray(s['max_dist'], f32), np.ascontiguousarray(s['last_desc'], np.uint8)]
+    m = np.ascontiguousarray(matched, np.int32).copy()
+    nm = L.ref_search_by_projection_sim3(len(kps), _p(kps), _p(ur), _p(d), _p(cam), len(sf), _p(sf), _p(T.reshape(16).copy()), len(a[0]), *[_p(x) for x in a], int(th), _p(m))
+    return nm, m
+
+
+def ref_init(L, s, window, ratio, ori):
+    """The reference's SearchForInitialization: (nmatches, vnMatches12, updated vbPrevMatched)."""
+    L.ref_search_for_initialization.restype = C.c_int
+    c = s['cam']; cam = np.array([c['fx'], c['fy'], c['cx'], c['cy'], c['bf'], *s.get('bounds', (0, 0, 640, 480))], np.float32); sf = np.ascontiguousarray(s['sf'], np.float32)
+    k1 = np.ascontiguousarray(s['k1'], O.KP_DTYPE); k2 = np.ascontiguousarray(s['k2'], O.KP_DTYPE)
+    d1 = np.ascontiguousarray(s['d1'], np.uint8); d2 = np.ascontiguousarray(s['d2'], np.uint8)
+    prev = np.ascontiguousarray(s['prev'], np.float32).copy(); m = np.zeros(len(k1), np.int32)
+    nm = L.ref_search_for_initialization(len(k1), _p(k1), _p(d1), len(k2), _p(k2), _p(d2), _p(cam), len(sf), _p(sf), _p(prev), window, C.c_float(ratio), int(ori), _p(m))
+    return nm, m, prev
+
+
+def ref_case(L, c):
+    """A constructed case of tests/match_cases.py through the reference: the result dict of match_cases.run_oracle (without ncand)."""
+    p = c['params']
+    if c['kind'] == 'last':
+        nm, mp = ref_last(L, c, p['th'], p['mono'], p['check_ori'], cur_mp=c['cur_mp'], cur_obs=c['cur_obs'])
+        return dict(nm=nm, mp=mp)
+    if c['kind'] == 'kf':
+        nm, mp = ref_kf(L, c, p['th'], p['orb_dist'], p['check_ori'])
+        return dict(nm=nm, mp=mp)
+    if c['kind'] == 'local':
+        nm, mp, ob = ref_local(L, c, p['th'], p['nnratio'], id_base=MC.ID_BASE)
+        return dict(nm=nm, mp=mp, obs=ob)
+    if c['kind'] == 'sim3':
+        nm, m = ref_sim3(L, c, c['Tcw_cur'], c['normal'], c['matched'], p['th'])
+        return dict(nm=nm, matched=m)
+    nm, m, prev = ref_init(L, c, p['window'], p['nnratio'], p['check_ori'])
+    return dict(nm=nm, m12=m, prev=prev)
+
+
+@pytest.mark.parametrize('name', MC.names())
+def test_constructed_case_equals_the_reference(name):
+    """The constructed cases of tests/match_cases.py: the oracle equals the reference's own ORBmatcher.cc, and the case's proof holds on
+    that result -- the order-dependent path the case was built for (rescan, tentative claims, ratio flips, steals, bounds, gate and
+    histogram edges) was really taken."""
+    c = MC.CASES[name]
+    o = MC.run_oracle(c)
+    r = ref_case(_lib(), c)
+    for k, v in r.items():
+        assert np.array_equal(v, o[k]), (name, k, v, o[k])
+    c['proof'](o)
 
 
 @pytest.mark.parametrize('seed', range(6))
@@ -87,18 +176,10 @@ def test_search_by_projection_local_equals_the_reference(seed):
     L = _lib()
     s = S.random_localmap_scenario(seed, n_cur=1000, n_mp=2500 + 100 * seed, conflict=[0.2, 0.5][seed % 2])
     fo = _frame(s)
-    n = len(s['kps'])
-    kps = np.ascontiguousarray(s['kps'], O.KP_DTYPE); ur = np.ascontiguousarray(s['uright'], np.float32); d = np.ascontiguousarray(s['desc'], np.uint8)
-    sf = np.ascontiguousarray(s['sf'], np.float32); cam = _cam(s)
     for th, ratio in ((3.0, 0.8), (1.0, 0.8), (5.0, 0.6)):
         a = (s['inview'], s['projx'], s['projy'], s['projxr'], s['level'], s['viewcos'], s['mp_desc'], s['mp_obs'], th, ratio, s['f_mp'], s['f_obs'])
         nm_o, mp_o, ob_o, _ = O.search_by_projection_local(fo, *a, id_base=7)
-        mp = np.ascontiguousarray(s['f_mp'], np.int32).copy(); ob = np.ascontiguousarray(s['f_obs'], np.uint8).copy()
-        arrs = [np.ascontiguousarray(s['inview'], np.uint8), np.ascontiguousarray(s['projx'], np.float32), np.ascontiguousarray(s['projy'], np.float32),
-                np.ascontiguousarray(s['projxr'], np.float32), np.ascontiguousarray(s['level'], np.int32), np.ascontiguousarray(s['viewcos'], np.float32),
-                np.ascontiguousarray(s['mp_desc'], np.uint8), np.ascontiguousarray(s['mp_obs'], np.uint8)]
-        nm_r = L.ref_search_by_projection_local(n, _p(kps), _p(ur), _p(d), _p(cam), len(sf), _p(sf), len(arrs[0]), *[_p(x) for x in arrs], C.c_float(th), C.c_float(ratio), 7,
-                                                _p(mp), _p(ob))
+        nm_r, mp, ob = ref_local(L, s, th, ratio)
         assert nm_r == nm_o, (seed, th, nm_r, nm_o)
         assert np.array_equal(mp, mp_o) and np.array_equal(ob, ob_o)
         assert nm_o > 100
@@ -115,18 +196,13 @@ def test_descriptor_distance_equals_the_reference():
 @pytest.mark.parametrize('seed', range(4))
 def test_relocalisation_search_equals_the_reference(seed):
     """SearchByProjection(Frame&, KeyFrame*, sAlreadyFound, th, ORBdist) (src/ORBmatcher.cc:1474-1601) incl. MapPoint::PredictScale through libm's logf."""
-    L = _lib(); L.ref_search_by_projection_kf.restype = C.c_int
+    L = _lib()
     s = S.keyframe_scenario(seed, n_cur=900 + 50 * seed, n_kf=800 + 70 * seed, conflict=[0.2, 0.5][seed % 2])
     fo = _frame(s)
-    n = len(s['kps'])
-    kps = np.ascontiguousarray(s['kps'], O.KP_DTYPE); ur = np.ascontiguousarray(s['uright'], np.float32); d = np.ascontiguousarray(s['desc'], np.uint8)
-    sf = np.ascontiguousarray(s['sf'], np.float32); cam = _cam(s); Tc = np.ascontiguousarray(s['Tcw_cur'], np.float32).reshape(16)
-    a = [np.ascontiguousarray(s['kf_valid'], np.uint8), np.ascontiguousarray(s['last_xyz'], np.float32), np.ascontiguousarray(s['last_desc'], np.uint8),
-         np.ascontiguousarray(s['last_angle'], np.float32), np.ascontiguousarray(s['min_dist'], np.float32), np.ascontiguousarray(s['max_dist'], np.float32)]
+    a = [s['kf_valid'], s['last_xyz'], s['last_desc'], s['last_angle'], s['min_dist'], s['max_dist']]
     for th, orb_dist, ori in ((10.0, 100, True), (3.0, 64, True), (10.0, 100, False)):
         nm_o, mp_o, _ = O.search_by_projection_kf(fo, s['Tcw_cur'], *a, th, orb_dist, ori, cur_mp=s['cur_mp'])
-        mp = np.ascontiguousarray(s['cur_mp'], np.int32).copy()
-        nm_r = L.ref_search_by_projection_kf(n, _p(kps), _p(ur), _p(d), _p(cam), len(sf), _p(sf), _p(Tc), len(a[0]), *[_p(x) for x in a], C.c_float(th), orb_dist, int(ori), _p(mp))
+        nm_r, mp = ref_kf(L, s, th, orb_dist, ori)
         assert nm_r == nm_o, (seed, th, nm_r, nm_o)
         assert np.array_equal(mp, mp_o)
         assert nm_o > 30
@@ -135,14 +211,10 @@ def test_relocalisation_search_equals_the_reference(seed):
 @pytest.mark.parametrize('seed,window,ori', [(1, 100, True), (2, 100, False), (3, 40, True)])
 def test_search_for_initialization_equals_the_reference(seed, window, ori):
     import test_match_init as TI
-    L = _lib(); L.ref_search_for_initialization.restype = C.c_int
+    L = _lib()
     s = TI.init_scenario(seed)
     nm_o, m_o, prev_o = O.search_for_initialization(s['f1'], s['f2'], s['prev'], window, 0.9, ori)
-    c = s['cam']; cam = np.array([c['fx'], c['fy'], c['cx'], c['cy'], c['bf'], 0, 0, 640, 480], np.float32); sf = np.ascontiguousarray(s['sf'], np.float32)
-    k1 = np.ascontiguousarray(s['k1'], O.KP_DTYPE); k2 = np.ascontiguousarray(s['k2'], O.KP_DTYPE)
-    d1 = np.ascontiguousarray(s['d1'], np.uint8); d2 = np.ascontiguousarray(s['d2'], np.uint8)
-    prev = np.ascontiguousarray(s['prev'], np.float32).copy(); m = np.zeros(len(k1), np.int32)
-    nm_r = L.ref_search_for_initialization(len(k1), _p(k1), _p(d1), len(k2), _p(k2), _p(d2), _p(cam), len(sf), _p(sf), _p(prev), window, C.c_float(0.9), int(ori), _p(m))
+    nm_r, m, prev = ref_init(L, s, window, 0.9, ori)
     assert nm_r == nm_o and np.array_equal(m, m_o) and np.array_equal(prev, prev_o)
     assert nm_o > 40
 
@@ -212,7 +284,7 @@ def test_search_by_projection_sim3_equals_the_reference(seed, ncur, nmp, th):
     (RGB-D); the reference's own decomposition (row norm, division, -Rcw.t()*tcw) runs inside the call -- the test requires that the row norm rounds to 1.0f so
     that the Mat / scalar division (not pinned by the stand-in) is the identity."""
     import test_match_sim3 as TS
-    L = _lib(); L.ref_search_by_projection_sim3.restype = C.c_int
+    L = _lib()
     f32 = np.float32
     s, _, nrm, matched = TS.sim3_inputs(seed, ncur, nmp)
     T = np.ascontiguousarray(s['Tcw_cur'], f32)
@@ -221,12 +293,7 @@ def test_search_by_projection_sim3_equals_the_reference(seed, ncur, nmp, th):
     Ow = np.array([f32(-(float(R[0, r]) * float(t[0]) + float(R[1, r]) * float(t[1]) + float(R[2, r]) * float(t[2]))) for r in range(3)], f32)      # -Rcw.t()*tcw, double accumulator
     fo = _frame(s)
     nm_o, m_o = O.search_by_projection_sim3(fo, T, Ow, s['kf_valid'], s['last_xyz'], nrm, s['min_dist'], s['max_dist'], s['last_desc'], float(th), matched)
-    kps = np.ascontiguousarray(s['kps'], O.KP_DTYPE); ur = np.ascontiguousarray(s['uright'], f32); d = np.ascontiguousarray(s['desc'], np.uint8)
-    sf = np.ascontiguousarray(s['sf'], f32); cam = _cam(s)
-    a = [np.ascontiguousarray(s['kf_valid'], np.uint8), np.ascontiguousarray(s['last_xyz'], f32), np.ascontiguousarray(nrm, f32), np.ascontiguousarray(s['min_dist'], f32),
-         np.ascontiguousarray(s['max_dist'], f32), np.ascontiguousarray(s['last_desc'], np.uint8)]
-    m = np.ascontiguousarray(matched, np.int32).copy()
-    nm_r = L.ref_search_by_projection_sim3(len(kps), _p(kps), _p(ur), _p(d), _p(cam), len(sf), _p(sf), _p(T.reshape(16).copy()), len(a[0]), *[_p(x) for x in a], int(th), _p(m))
+    nm_r, m = ref_sim3(L, s, T, nrm, matched, th)
     assert nm_r == nm_o, (nm_r, nm_o)
     assert np.array_equal(m, m_o) and nm_o > 20
 
