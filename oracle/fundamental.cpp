@@ -7,7 +7,8 @@
 // (solveCubic) and is PINNED against cv2 4.13 run in the build container (tests/golden/make_golden_fm.py ->
 // tests/golden/fm_ransac.npz): F agrees to ~1e-12 and the inlier masks are identical.  Behaviour that defines the result:
 //   * RNG rng((uint64)-1), MWC generator x = (uint32)x * 4164903690 + (x >> 32); uniform(0, n) = next() % n
-//   * 7 distinct indices per iteration, redrawn (<= 10000 attempts) while the LAST point is collinear with two earlier ones
+//   * 7 distinct indices per iteration, redrawn while the LAST point is collinear with two earlier ones: at most 10000 attempts in
+//     RANSAC, which passes that cap to getSubset, and getSubset's default of 1000 in LMedS; a failed first draw returns no matrix
 //   * the 7-point solver normalises the 7 points (centroid, mean distance sqrt 2) [4.13 behaviour, found by probe], takes the two
 //     missing right singular vectors from JacobiSVD's completion step (fixed RNG(0x12345678) sign vectors projected off the row
 //     space), solves det(l f1 + (1 - l) f2) = 0 with cv::solveCubic, and scales each F to F33 = 1
@@ -257,9 +258,10 @@ SGO_API int sgo_find_fundamental_ransac(const float* m1, const float* m2, int n,
     if (confidence < DBL_EPSILON || confidence > 1 - DBL_EPSILON) confidence = 0.99;
     if (n < 15) {
         // fundam.cpp cv::findFundamentalMat: fewer than 15 pairs never reach RANSAC.  < 7: empty; == 7: the 7-point solver directly (up to three
-        // stacked solutions; the first is returned); 8..14: LMeDSPointSetRegistrator(cb, 7, confidence).run (ptsetreg.cpp), maxIters = 1000:
-        // a fixed number of samples (outlier ratio 0.45), the model with the smallest median error (element count/2 of the sorted errors), inliers
-        // within sigma = 2.5 * 1.4826 * (1 + 5 / (count - 7)) * sqrt(median); the result is dropped when fewer than 7 pairs are inliers.
+        // stacked solutions; the first is returned); 8..14: LMeDSPointSetRegistrator(cb, 7, confidence, max_iters).run (ptsetreg.cpp): a fixed
+        // number of samples, max(RANSACUpdateNumIters(confidence, 0.45, 7, max_iters), 3), each drawn in at most 1000 attempts (getSubset's
+        // default; RANSAC passes 10000), the model with the smallest median error (element count/2 of the sorted errors), inliers within
+        // sigma = 2.5 * 1.4826 * (1 + 5 / (count - 7)) * sqrt(median); the result is dropped when fewer than 7 pairs are inliers.
         if (n < 7) return 0;
         if (n == 7) {             // runKernel directly: the stacked solutions; callers read rows 0..2 = the first one (src/Frame.cc:617-619)
             double models7[27];
@@ -271,14 +273,14 @@ SGO_API int sgo_find_fundamental_ransac(const float* m1, const float* m2, int n,
             return 1;
         }
         CvRng rng((uint64_t)-1);
-        const int niters = std::max(update_num_iters(confidence, 0.45, 7, 1000), 3);
+        const int niters = std::max(update_num_iters(confidence, 0.45, 7, max_iters), 3);
         double min_median = DBL_MAX, best[9], models[27];
         float ms1[14], ms2[14];
         std::vector<float> err(n);
         int iter = 0;
         for (iter = 0; iter < niters; iter++) {
             bool found = false;
-            for (int attempt = 0; attempt < 10000 && !found; attempt++) {
+            for (int attempt = 0; attempt < 1000 && !found; attempt++) {
                 int idx[7];
                 for (int i = 0; i < 7; i++) {
                     int v;

@@ -12,6 +12,8 @@
 //     Jacobi sweeps (same subspace, ~1e-15 relative difference in F).
 // All arithmetic is FP64 with individually rounded products and sums (-fmad=false), errors are rounded to float before the
 // threshold test like OpenCV's.  Fewer than 15 pairs take OpenCV's other branches in the same kernel: LMedS (8..14), plain 7-point (7), empty (< 7).
+// A sample is redrawn at most 10000 times in RANSAC and 1000 times in LMedS (OpenCV passes 10000 to getSubset only from RANSAC), and LMedS
+// runs max(RANSACUpdateNumIters(confidence, 0.45, 7, max_iters), 3) samples: both branches honour the caller's max_iters.
 #include <cuda_runtime.h>
 
 #include <cfloat>
@@ -25,6 +27,8 @@ namespace sgs {
 constexpr int kFmThreads = 256;
 constexpr int kFmRound = 32;          // iterations per round (the first round draws kFmFirstRound)
 constexpr int kFmFirstRound = 8;
+constexpr int kFmRansacAttempts = 10000;  // getSubset's cap on redraws per sample: RANSAC passes 10000,
+constexpr int kFmLmedsAttempts = 1000;    // LMedS keeps the default of 1000
 
 struct FmRng {
     unsigned long long state;
@@ -200,13 +204,13 @@ __device__ __forceinline__ float fm_error(const float4 p, const double* F) {    
 }
 
 // RANSACPointSetRegistrator / LMeDSPointSetRegistrator::getSubset for `want` consecutive iterations (sequential RNG state: one thread).
-// Returns the number of samples drawn; *ok = 0 when a draw failed (10000 attempts without a non-collinear sample): the estimator's loop ends there.
-__device__ int fm_draw_samples(FmRng& rng, const float4* pts, int n, int want, int (*idx_out)[7], int* ok) {
+// Returns the number of samples drawn; *ok = 0 when a draw failed (max_attempts attempts without a non-collinear sample): the estimator's loop ends there.
+__device__ int fm_draw_samples(FmRng& rng, const float4* pts, int n, int want, int max_attempts, int (*idx_out)[7], int* ok) {
     int got = 0;
     *ok = 1;
     for (; got < want; ++got) {
         bool found = false;
-        for (int attempt = 0; attempt < 10000 && !found; ++attempt) {
+        for (int attempt = 0; attempt < max_attempts && !found; ++attempt) {
             float2 a[7], b[7];
             int* idx = idx_out[got];
             for (int i = 0; i < 7; ++i) {
@@ -327,20 +331,21 @@ __global__ void __launch_bounds__(kFmThreads) fm_ransac_kernel(const sgs_keypoin
         return;
     }
     if (n < 15) {
-        // 8..14 pairs: cv::findFundamentalMat switches to LMeDSPointSetRegistrator(cb, 7, confidence) (fundam.cpp; ptsetreg.cpp): a FIXED number of
-        // samples (outlier ratio 0.45, at most 1000), the model with the smallest median error (element n/2 of the sorted errors, strict '<'),
-        // inliers within sigma = 2.5 * 1.4826 * (1 + 5 / (n - 7)) * sqrt(median) (at least 0.001); fewer than 7 inliers -> empty matrix.
+        // 8..14 pairs: cv::findFundamentalMat switches to LMeDSPointSetRegistrator(cb, 7, confidence, max_iters) (fundam.cpp; ptsetreg.cpp): a FIXED
+        // number of samples (outlier ratio 0.45, at most max_iters, at least 3), each drawn in at most 1000 attempts, the model with the smallest
+        // median error (element n/2 of the sorted errors, strict '<'), inliers within sigma = 2.5 * 1.4826 * (1 + 5 / (n - 7)) * sqrt(median)
+        // (at least 0.001); fewer than 7 inliers -> empty matrix.
         __shared__ float s_med[kFmRound * 3];
         __shared__ double s_minmed;
         __shared__ int s_lm_good;
-        const int niters = max(fm_update_iters(confidence, 0.45, 1000), 3);
+        const int niters = max(fm_update_iters(confidence, 0.45, max_iters), 3);
         if (tid == 0) { s_done = 0; s_rng = 0xffffffffffffffffULL; s_minmed = DBL_MAX; s_drawn_ok = 1; s_lm_good = 0; }
         __syncthreads();
         while (true) {
             if (tid == 0) {
                 FmRng rng; rng.state = s_rng;
                 int okd = 1;
-                s_round = fm_draw_samples(rng, s_pts, n, min(kFmRound, niters - s_done), s_idx, &okd);
+                s_round = fm_draw_samples(rng, s_pts, n, min(kFmRound, niters - s_done), kFmLmedsAttempts, s_idx, &okd);
                 if (!okd) s_drawn_ok = 0;
                 s_rng = rng.state;
             }
@@ -394,8 +399,6 @@ __global__ void __launch_bounds__(kFmThreads) fm_ransac_kernel(const sgs_keypoin
         if (mask_out) for (int i = tid; i < n_all; i += kFmThreads) mask_out[(int64_t)f * cap + i] = (ok && i < n && fm_inlier(s_pts[i], s_best, tl)) ? 1 : 0;
         return;
     }
-    if (thresh <= 0) thresh = 3;
-    if (confidence < DBL_EPSILON || confidence > 1 - DBL_EPSILON) confidence = 0.99;
     const float t = (float)(thresh * thresh);
     if (tid == 0) { s_n = n; s_niters = max(max_iters, 1); s_done = 0; s_maxgood = 0; s_rng = 0xffffffffffffffffULL; s_drawn_ok = 1; }
     __syncthreads();
@@ -406,7 +409,7 @@ __global__ void __launch_bounds__(kFmThreads) fm_ransac_kernel(const sgs_keypoin
             FmRng rng; rng.state = s_rng;
             const int want = min(first ? kFmFirstRound : kFmRound, s_niters - s_done);
             int okd = 1;
-            const int got = fm_draw_samples(rng, s_pts, n, want, s_idx, &okd);      // a failed draw ends the loop (or fails it when it is the first iteration)
+            const int got = fm_draw_samples(rng, s_pts, n, want, kFmRansacAttempts, s_idx, &okd);      // a failed draw ends the loop (or fails it when it is the first iteration)
             if (!okd) s_drawn_ok = 0;
             s_round = got;
             s_rng = rng.state;
