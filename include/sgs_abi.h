@@ -341,6 +341,13 @@ SGS_API int sgs_settings_load(const char* path, sgs_settings* out);
  *                                 (0 = root when that level is <= 0).  A feature enters the FeatureVector iff its weight is > 0.
  *   sgs_match_bow_batch_device  : ORBmatcher::SearchByBoW(KeyFrame*, Frame&, vpMapPointMatches) (src/ORBmatcher.cc:159-290) for `nframes`
  *                                 (key frame, frame) pairs: match_f[j] = key-frame feature whose map point goes to frame feature j, or -1.
+ * Limits (pinned by tests/test_gpu_bow_cases.py):
+ *   - at most 4096 children per vocabulary node (sgs_vocabulary_create returns SGS_ERR_UNSUPPORTED beyond);
+ *   - at most 8192 features per side and frame: kf_cap and f_cap in 1 .. 8192 (SGS_ERR_UNSUPPORTED, nothing launched, beyond);
+ *   - descriptor rows (vocabulary nodes, d_desc, kf_desc, f_desc) are read as uint4: every descriptor array must be 16-byte aligned;
+ *   - levelsup >= L files every feature under node 0 (the root), so the matchers see one bucket;
+ *   - counts above the cap are clamped to the cap; rows past a frame's count are not written by the transform, and the matcher sets
+ *     every match_f row past the count (up to the cap) to -1.
  * ------------------------------------------------------------------------------------ */
 typedef struct sgs_vocabulary sgs_vocabulary;
 SGS_API int sgs_vocabulary_create(int device, int k, int L, int nnodes, const int32_t* parent, const uint8_t* node_desc,
