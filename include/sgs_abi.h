@@ -749,6 +749,37 @@ SGS_API int sgs_tracker_step_rgbd(sgs_tracker* t, sgs_detector* det, const uint8
                                   int check_orientation, sgs_keypoint* kps_out, uint8_t* desc_out, float* u_right_out, int32_t* counts_out,
                                   int32_t* cur_mp_out, int32_t* nmatches_out, sgs_rect* boxes_out, int32_t* nboxes_out, uint8_t* have_out,
                                   sgs_keypoint* kps_un_out, float* depth_out);
+/* The RGB-D step for LIVE streams, one new frame per stream per call, the previous frames kept on the device.  The tracker has max_batch stream
+ * slots, 0 .. max_batch-1.  Frame f of a call is the next frame of slot d_slot[f]; slots are distinct within a call, and any subset of them, in any order,
+ * may appear.  For frame f in slot s:
+ *   previous frame   the last frame any earlier stream call on this handle gave to s (a stream may skip calls);
+ *   first frame      s has never held a frame, or d_new_stream[f] != 0 (d_new_stream may be NULL: all 0).  A first frame behaves as a row with
+ *                    prev_index[f] == f of sgs_tracker_step_rgbd_device: LK tracks into its own image, F is NaN with info status 3, every keypoint is kept;
+ *   dynamic state    the flag and person boxes the previous frame ended with filter the point pairs (src/Frame.cc:454-472); the flag counts as false when
+ *                    the previous frame was itself a first frame (quirk Q13);
+ *   after the call   s holds this frame's LK pyramid levels, its boxes and flag, and whether it was a first frame.
+ * Every result -- sgs_tracker_results_device, the boxes, sgs_tracker_frame_device, sgs_tracker_fundamental_device_ptr, sgs_tracker_prev_xy_device -- equals
+ * bit for bit what sgs_tracker_step_rgbd_device returns for a batch that holds each stream's previous frame and chains them with prev_index.  The batch
+ * entry points on the same handle neither read nor change the slots; sgs_tracker_pose_chain_device after a stream call reads its mvKeysUn.  The
+ * slots survive everything but the handle: the reference keeps this state at file scope through Tracking::Reset, so a caller mirroring it keeps
+ * new_stream = 0 across a reset, and sets it when a different sequence starts feeding the slot.
+ * d_slot [F], d_new_stream [F]: device arrays, not checked (out-of-range or duplicate slots are undefined).  The other arguments are those of
+ * sgs_tracker_step_rgbd_device.  Calls on different streams must be ordered by the caller: each reads the slots the previous one wrote.
+ * A call refused with SGS_ERR_INVALID changes no slot.  After SGS_ERR_CUDA the state of that call's slots is unspecified: restart them with new_stream. */
+SGS_API int sgs_tracker_step_rgbd_stream_device(sgs_tracker* t, sgs_detector* det, const uint8_t* d_rgb, size_t rgb_stride, int rgb_pitch, const void* d_depth,
+                                                size_t depth_stride, int depth_pitch, const sgs_rgbd_format* fmt, int nframes, const int32_t* d_slot,
+                                                const uint8_t* d_new_stream, const float* last_xyz, const uint8_t* last_desc, const uint8_t* last_flags,
+                                                const int32_t* last_octave, const float* last_angle, const int32_t* last_n, const float* tcw_cur,
+                                                const float* tcw_last, float th, int mono, int check_orientation, void* stream);
+/* The same from HOST buffers (slot [F], new_stream [F] or NULL, outputs as sgs_tracker_step_rgbd).  Refuses nframes outside [1, max_batch], a NULL slot,
+ * a slot outside [0, max_batch) and a slot given twice with SGS_ERR_INVALID before anything runs.  Synchronises. */
+SGS_API int sgs_tracker_step_rgbd_stream(sgs_tracker* t, sgs_detector* det, const uint8_t* rgb, size_t rgb_stride, int rgb_pitch, const void* depth,
+                                         size_t depth_stride, int depth_pitch, const sgs_rgbd_format* fmt, int nframes, const int32_t* slot,
+                                         const uint8_t* new_stream, const float* last_xyz, const uint8_t* last_desc, const uint8_t* last_flags,
+                                         const int32_t* last_octave, const float* last_angle, const int32_t* last_n, const float* tcw_cur,
+                                         const float* tcw_last, float th, int mono, int check_orientation, sgs_keypoint* kps_out, uint8_t* desc_out,
+                                         float* u_right_out, int32_t* counts_out, int32_t* cur_mp_out, int32_t* nmatches_out, sgs_rect* boxes_out,
+                                         int32_t* nboxes_out, uint8_t* have_out, sgs_keypoint* kps_un_out, float* depth_out);
 /* Device pointers to the compacted mvKeysUn [F][cap] and mvDepth [F][cap] (-1 without depth) of the last RGB-D step; SGS_ERR_INVALID before the first. */
 SGS_API int sgs_tracker_frame_device(const sgs_tracker* t, const sgs_keypoint** d_kps_un, const float** d_depth);
 /* Text listing of the kernel list: one line per kernel with its fused element-wise tail and activation-pool buffers.  SGS_ERR_CAPACITY

@@ -20,6 +20,7 @@
 #include <vector>
 
 #include "host_stage.cuh"
+#include "internal_launch.cuh"
 #include "sgs_common.h"
 
 namespace sgs {
@@ -247,7 +248,7 @@ __global__ void __launch_bounds__(kFmThreads) fm_ransac_kernel(const sgs_keypoin
                                                                const float2* __restrict__ prev_xy, const int32_t* __restrict__ counts, int cap,
                                                                const sgs_rect* __restrict__ prev_boxes, const int32_t* __restrict__ prev_nboxes,
                                                                const uint8_t* __restrict__ prev_have_dyn, int max_boxes,
-                                                               const int32_t* __restrict__ prev_index, double thresh,
+                                                               const int32_t* __restrict__ prev_index, const uint8_t* __restrict__ no_prev_f, double thresh,
                                                                double confidence, int max_iters, double* __restrict__ F_out,
                                                                int32_t* __restrict__ info, uint8_t* __restrict__ mask_out) {
     extern __shared__ float4 s_pts[];                  // [cap] (x1, y1, x2, y2), the pairs handed to the estimator, in order
@@ -265,9 +266,10 @@ __global__ void __launch_bounds__(kFmThreads) fm_ransac_kernel(const sgs_keypoin
         return cur_xy[(int64_t)f * cap + i];
     };
     // ---- selection (src/Frame.cc:454-472): ordered compaction of the pairs whose previous point is outside the previous boxes
-    // prev_index (may be NULL): the batch row holding the previous frame's boxes; prev_index[f] == f marks a frame without a previous one
+    // prev_index (may be NULL): the batch row holding the previous frame's boxes; prev_index[f] == f marks a frame without a previous one.
+    // no_prev_f (stream steps, prev_index NULL): the same mark per frame, the previous frame's boxes and flag gathered into row f
     const int fb = prev_index ? prev_index[f] : f;
-    const bool no_prev = prev_index && fb == f;
+    const bool no_prev = no_prev_f ? no_prev_f[f] != 0 : prev_index && fb == f;
     // The reference keeps "the previous frame had potential dynamic objects" at file scope and writes it only inside the rejection (src/Frame.cc:482-491), which
     // the first frame of a stream never runs (:154-162): the detections of a stream's first frame do not filter the pairs of its second frame (quirk Q13,
     // pinned by tests/test_frame_ref.py against the reference's own Frame.cc).  With prev_index the rows say which frames are first ones.
@@ -471,14 +473,14 @@ __global__ void __launch_bounds__(kFmThreads) fm_ransac_kernel(const sgs_keypoin
 }
 
 int fm_launch(const sgs_keypoint* d_kps, const float2* d_cur, const float2* d_prev, const int32_t* d_counts, int cap, int nframes,
-              const sgs_rect* d_boxes, const int32_t* d_nboxes, const uint8_t* d_have_dyn, int max_boxes, const int32_t* d_prev_index, double thresh,
-              double confidence, int max_iters, double* d_F, int32_t* d_info, uint8_t* d_mask, cudaStream_t st) {
+              const sgs_rect* d_boxes, const int32_t* d_nboxes, const uint8_t* d_have_dyn, int max_boxes, const int32_t* d_prev_index,
+              const uint8_t* d_no_prev, double thresh, double confidence, int max_iters, double* d_F, int32_t* d_info, uint8_t* d_mask, cudaStream_t st) {
     const size_t smem = (size_t)cap * sizeof(float4);
     if (smem > 200 * 1024) { set_error("fundamental: %d pairs per frame do not fit shared memory", cap); return SGS_ERR_UNSUPPORTED; }
     if (smem > 40 * 1024)      // per device and cheap: set whenever the default 48 KB would not do
         SGS_CUDA_TRY(cudaFuncSetAttribute(fm_ransac_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     fm_ransac_kernel<<<nframes, kFmThreads, smem, st>>>(d_kps, d_cur, d_prev, d_counts, cap, d_boxes, d_nboxes, d_have_dyn, max_boxes, d_prev_index,
-                                                        thresh, confidence, max_iters, d_F, d_info, d_mask);
+                                                        d_no_prev, thresh, confidence, max_iters, d_F, d_info, d_mask);
     SGS_CUDA_TRY(cudaGetLastError());
     return SGS_OK;
 }
@@ -495,7 +497,7 @@ SGS_API int sgs_fundamental_batch_device(const sgs_keypoint* d_kps, const float*
     if (!d_kps || !d_prev_xy || !d_counts || !d_F || cap < 1 || nframes < 1) { set_error("sgs_fundamental_batch_device: bad argument"); return SGS_ERR_INVALID; }
     if (d_prev_have_dyn && (!d_prev_boxes || !d_prev_nboxes || max_boxes < 1)) { set_error("sgs_fundamental_batch_device: boxes missing"); return SGS_ERR_INVALID; }
     return fm_launch(d_kps, nullptr, reinterpret_cast<const float2*>(d_prev_xy), d_counts, cap, nframes, d_prev_boxes, d_prev_nboxes, d_prev_have_dyn,
-                     max_boxes, d_prev_index, ransac_thresh, confidence, max_iters, d_F, d_info, nullptr, (cudaStream_t)stream);
+                     max_boxes, d_prev_index, nullptr, ransac_thresh, confidence, max_iters, d_F, d_info, nullptr, (cudaStream_t)stream);
 }
 
 SGS_API int sgs_fundamental_ransac(const float* pts1_xy, const float* pts2_xy, int n, double ransac_thresh, double confidence, int max_iters,
@@ -510,7 +512,7 @@ SGS_API int sgs_fundamental_ransac(const float* pts1_xy, const float* pts2_xy, i
     S.in(&d_a, pts1_xy, 2 * (size_t)n); S.in(&d_b, pts2_xy, 2 * (size_t)n); S.out(&d_F, 9); S.out(&d_info, 4); S.out(&d_mask, n);
     if (S.commit() != SGS_OK) return SGS_ERR_CUDA;
     const int rc = fm_launch(nullptr, reinterpret_cast<const float2*>(d_a), reinterpret_cast<const float2*>(d_b), nullptr, n, 1, nullptr, nullptr, nullptr, 0,
-                             nullptr, ransac_thresh, confidence, max_iters, d_F, d_info, d_mask, nullptr);
+                             nullptr, nullptr, ransac_thresh, confidence, max_iters, d_F, d_info, d_mask, nullptr);
     if (rc != SGS_OK) return rc;
     S.to_host(F, d_F, 9);
     if (mask) S.to_host(mask, d_mask, n);

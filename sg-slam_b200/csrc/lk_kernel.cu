@@ -18,11 +18,13 @@
 #include <vector>
 
 #include "host_stage.cuh"
+#include "internal_launch.cuh"
 #include "sgs_common.h"
 
 namespace sgs {
 
 constexpr int kWin = 21, kLkMaxLevel = 3, kLkMaxCount = 30;
+static_assert(kLkMaxLevel + 1 == sizeof(LkPyramid::off) / sizeof(int64_t), "LkPyramid describes every level");
 constexpr int kLkWarps = 4;
 
 constexpr int kLkPad = 24;            // the window reaches 22 px past the image on every side
@@ -255,7 +257,8 @@ __global__ void __launch_bounds__(kLkWarps * 32) lk_track_kernel(const __grid_co
     const int p = blockIdx.x * kLkWarps + warp;
     const int n = counts ? min(counts[f], cap) : cap;
     if (p >= n) return;
-    const int fj = prev_index ? prev_index[f] : f;       // frame of the batch that plays the role of the previous image
+    // row of L.J that plays the role of the previous image; < 0 (stream steps, a stream's first frame): the frame's own image
+    const int fj = prev_index ? prev_index[f] : f;
     const int64_t pi = (int64_t)f * cap + p;
     float ptx, pty;
     if (kps) { ptx = kps[pi].x; pty = kps[pi].y; } else { const float2 q = pts[pi]; ptx = q.x; pty = q.y; }
@@ -269,7 +272,7 @@ __global__ void __launch_bounds__(kLkWarps * 32) lk_track_kernel(const __grid_co
         const int pitch = L.pitch[level];
         const uint8_t* Iimg = L.I[level] + (int64_t)f * L.fstride[level];
         const uint32_t* Dimg = L.D[level] + (int64_t)f * L.fstride[level];
-        const uint8_t* Jimg = L.J[level] + (int64_t)fj * L.fstride[level];
+        const uint8_t* Jimg = fj < 0 ? Iimg : L.J[level] + (int64_t)fj * L.fstride[level];
         const float sc = 1.f / (float)(1 << level);
         float px = __fmul_rn(ptx, sc), py = __fmul_rn(pty, sc);
         float qx, qy;
@@ -382,12 +385,13 @@ void build_pyramid(sgs_lk* k, const uint8_t* d_l0, int pitch0, int64_t fstride0,
     }
 }
 
+// j_store (may be NULL): padded levels in the geometry of d_pyrJ holding the previous images, row d_prev_index[f] for frame f (< 0: its own image)
 int run_lk(sgs_lk* k, const uint8_t* d_cur, const uint8_t* d_prev, const int32_t* d_prev_index, int nframes, size_t frame_stride, int pitch,
-           const sgs_keypoint* d_kps, const float* d_pts, const int32_t* d_counts, int cap, float* d_out, cudaStream_t st) {
+           const sgs_keypoint* d_kps, const float* d_pts, const int32_t* d_counts, int cap, float* d_out, cudaStream_t st, const uint8_t* j_store = nullptr) {
     k->timer.begin();
     k->timer.mark(0, st);
     build_pyramid(k, d_cur, pitch, (int64_t)frame_stride, k->d_pyrI, k->d_der, nframes, st);
-    const bool same_batch = d_prev_index != nullptr;     // previous images are other frames of the same batch: one pyramid serves both roles
+    const bool same_batch = d_prev_index != nullptr;     // previous images are other frames of the same batch (or the store): no J pyramid to build
     if (!same_batch) build_pyramid(k, d_prev, pitch, (int64_t)frame_stride, k->d_pyrJ, nullptr, nframes, st);
     LkLevels L;
     L.max_level = k->max_level;
@@ -395,7 +399,7 @@ int run_lk(sgs_lk* k, const uint8_t* d_cur, const uint8_t* d_prev, const int32_t
         if (l <= k->max_level) {
             const int64_t o = k->loff[l] + k->lorg[l];
             L.w[l] = k->lw[l]; L.h[l] = k->lh[l]; L.pitch[l] = k->lp[l]; L.fstride[l] = k->lfs[l];
-            L.I[l] = k->d_pyrI + o; L.J[l] = (same_batch ? k->d_pyrI : k->d_pyrJ) + o; L.D[l] = k->d_der + o;
+            L.I[l] = k->d_pyrI + o; L.J[l] = (j_store ? j_store : same_batch ? k->d_pyrI : k->d_pyrJ) + o; L.D[l] = k->d_der + o;
         } else { L.I[l] = L.J[l] = nullptr; L.D[l] = nullptr; L.w[l] = L.h[l] = L.pitch[l] = 0; L.fstride[l] = 0; }
     }
     k->timer.mark(1, st);
@@ -406,6 +410,20 @@ int run_lk(sgs_lk* k, const uint8_t* d_cur, const uint8_t* d_prev, const int32_t
     return SGS_OK;
 }
 }  // namespace
+
+namespace sgs {
+LkPyramid lk_pyramid(const sgs_lk* k) {
+    LkPyramid p;
+    p.I = k->d_pyrI; p.bytes = k->pyr_elems + 256; p.max_level = k->max_level;
+    for (int l = 0; l <= kLkMaxLevel; ++l) { p.off[l] = l <= k->max_level ? k->loff[l] : 0; p.frame_bytes[l] = l <= k->max_level ? k->lfs[l] : 0; }
+    return p;
+}
+
+int lk_track_from_store(sgs_lk* k, const uint8_t* d_cur, int nframes, size_t frame_stride, int pitch, const sgs_keypoint* d_kps, const int32_t* d_counts,
+                        int cap, const uint8_t* d_store, const int32_t* d_row, float* d_prev_xy, cudaStream_t st) {
+    return run_lk(k, d_cur, nullptr, d_row, nframes, frame_stride, pitch, d_kps, nullptr, d_counts, cap, d_prev_xy, st, d_store);
+}
+}  // namespace sgs
 
 extern "C" {
 

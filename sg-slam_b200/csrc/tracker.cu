@@ -6,6 +6,7 @@
 //                         Tracking::TrackWithMotionModel, src/Tracking.cc:924), on the device-resident extraction results.
 //   sgs_tracker_step / sgs_tracker_step_rgbd(_device): the whole front end with the detector on its own stream; the RGB-D step starts from the
 //                         colour and raw depth frames (grab.cu) and adds UndistortKeyPoints + ComputeStereoFromRGBD (one shared body, enqueue_step).
+//   sgs_tracker_step_rgbd_stream(_device): the RGB-D step for live streams, one new frame per stream slot, the previous frames kept in StreamState.
 // One H2D of the frames, one H2D of the per-frame track inputs, one D2H of the compacted results + matches.
 #include <cuda_runtime.h>
 
@@ -15,9 +16,24 @@
 #include <vector>
 
 #include "host_stage.cuh"
+#include "internal_launch.cuh"
 #include "sgs_common.h"
 
 template <class T> using Child = std::unique_ptr<T, void (*)(T*)>;      // a handle the tracker owns, released by its sgs_*_destroy
+
+// What the RGB-D stream steps keep per stream slot (0 .. max_batch-1) between calls -- the reference's file-scope imGrayPre,
+// bPreFrameHavePotentialDynamicObj and vPreFramePotentialDynamicBorder (src/Frame.cc:27-33) -- and the per-frame arrays of one call.  Allocated on the
+// first stream call, apart from every buffer the batch calls write, so that those calls can neither read nor change it.
+struct StreamState {
+    // per slot: the last frame's padded LK levels (the geometry of sgs_lk's pyramid, LkPyramid), its boxes [max_boxes], nboxes, flag, and
+    // bit 0 = the slot holds a frame, bit 1 = that frame was a first frame
+    uint8_t* levels = nullptr; sgs_rect* boxes = nullptr; int32_t* nboxes = nullptr; uint8_t* have = nullptr; uint8_t* state = nullptr;
+    // per frame of a call: slot, new_stream (host entry point's copies), the LK row (slot, or -1 for a first frame), the first-frame mark, and the previous
+    // frame's flag (quirk Q13 applied), nboxes and boxes, gathered for findFundamentalMat
+    int32_t* slot = nullptr; uint8_t* new_stream = nullptr; int32_t* row = nullptr; uint8_t* first = nullptr; uint8_t* pre_have = nullptr;
+    int32_t* pre_nboxes = nullptr; sgs_rect* pre_boxes = nullptr;
+    bool ready = false;
+};
 
 struct sgs_tracker {
     explicit sgs_tracker(int dev) : device(dev), res(dev) {}
@@ -58,6 +74,7 @@ struct sgs_tracker {
     double* d_po_err = nullptr; uint8_t* d_po_level = nullptr;
     uint8_t* d_inview = nullptr; float* d_projx = nullptr; float* d_projy = nullptr; float* d_projxr = nullptr; int32_t* d_level = nullptr; float* d_viewcos = nullptr;
     unsigned long long* d_ncand2 = nullptr;
+    StreamState ss;                             // the RGB-D stream steps
 };
 
 namespace sgs {
@@ -179,6 +196,44 @@ __global__ void __launch_bounds__(256) chain_final_kernel(const int32_t* __restr
     __syncthreads();
     if (threadIdx.x == 0) { stats[8 * f + 6] = nml[f]; stats[8 * f + 7] = s_cnt; }
 }
+// ---- the RGB-D stream steps (StreamState) ----------------------------------------------------------------------------------------------------
+// Per frame of a call, before LK: a first frame (its slot never held a frame, or new_stream[f]) tracks into its own image and has no previous frame;
+// any other frame reads its slot's stored levels, and the flag and boxes its previous frame ended with.  The flag counts as false when that frame was
+// itself a first frame: the reference writes it only inside the rejection, which a first frame never runs (src/Frame.cc:154-162, quirk Q13).
+__global__ void stream_resolve_kernel(int nframes, const int32_t* __restrict__ slot, const uint8_t* __restrict__ new_stream, const uint8_t* __restrict__ s_state,
+                                      const uint8_t* __restrict__ s_have, const int32_t* __restrict__ s_nboxes, const sgs_rect* __restrict__ s_boxes, int max_boxes,
+                                      int32_t* __restrict__ row, uint8_t* __restrict__ first, uint8_t* __restrict__ pre_have, int32_t* __restrict__ pre_nboxes,
+                                      sgs_rect* __restrict__ pre_boxes) {
+    const int f = blockIdx.x * blockDim.x + threadIdx.x;
+    if (f >= nframes) return;
+    const int s = slot[f];
+    const uint8_t st = s_state[s];
+    const bool fi = !(st & 1) || (new_stream && new_stream[f]);
+    row[f] = fi ? -1 : s;
+    first[f] = fi ? 1 : 0;
+    pre_have[f] = (!fi && s_have[s] && !(st & 2)) ? 1 : 0;
+    pre_nboxes[f] = fi ? 0 : s_nboxes[s];
+    if (!fi) for (int b = 0; b < max_boxes; ++b) pre_boxes[(int64_t)f * max_boxes + b] = s_boxes[(int64_t)s * max_boxes + b];
+}
+// After LK and findFundamentalMat: frame f's padded levels (current-image pyramid, row f), boxes, flag and first-frame mark become the state of slot[f].
+// Grid (x, nframes); the levels are copied in 16-byte words.
+__global__ void __launch_bounds__(256) stream_commit_kernel(const LkPyramid P, uint8_t* __restrict__ s_levels, const int32_t* __restrict__ slot,
+                                                            const uint8_t* __restrict__ first, const sgs_rect* __restrict__ boxes, const int32_t* __restrict__ nboxes,
+                                                            const uint8_t* __restrict__ have, int max_boxes, sgs_rect* __restrict__ s_boxes,
+                                                            int32_t* __restrict__ s_nboxes, uint8_t* __restrict__ s_have, uint8_t* __restrict__ s_state) {
+    const int f = blockIdx.y, s = slot[f];
+#pragma unroll
+    for (int l = 0; l < 4; ++l) {
+        const int64_t n16 = l <= P.max_level ? P.frame_bytes[l] / 16 : 0;
+        const uint4* src = reinterpret_cast<const uint4*>(P.I + P.off[l] + (int64_t)f * P.frame_bytes[l]);
+        uint4* dst = reinterpret_cast<uint4*>(s_levels + P.off[l] + (int64_t)s * P.frame_bytes[l]);
+        for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n16; i += (int64_t)gridDim.x * blockDim.x) dst[i] = src[i];
+    }
+    if (blockIdx.x == 0) {
+        for (int b = threadIdx.x; b < max_boxes; b += blockDim.x) s_boxes[(int64_t)s * max_boxes + b] = boxes[(int64_t)f * max_boxes + b];
+        if (threadIdx.x == 0) { s_nboxes[s] = nboxes[f]; s_have[s] = have[f]; s_state[s] = 1 | (first[f] ? 2 : 0); }
+    }
+}
 }  // namespace sgs
 
 using namespace sgs;
@@ -194,6 +249,17 @@ bool frames_ok(const char* fn, int nframes, int limit, const int32_t* prev_index
     if (nframes < 1 || nframes > limit) { set_error("%s: nframes = %d outside [1,%d]", fn, nframes, limit); return false; }
     for (int f = 0; prev_index && f < nframes; ++f)
         if (prev_index[f] < 0 || prev_index[f] >= nframes) { set_error("%s: prev_index out of range", fn); return false; }
+    return true;
+}
+
+// nframes in [1, limit]; slot [nframes] (host): distinct stream slots in [0, limit)
+bool slots_ok(const char* fn, int nframes, int limit, const int32_t* slot) {
+    if (!frames_ok(fn, nframes, limit)) return false;
+    std::vector<uint8_t> seen(limit, 0);
+    for (int f = 0; f < nframes; ++f) {
+        if (slot[f] < 0 || slot[f] >= limit) { set_error("%s: slot[%d] = %d outside [0,%d)", fn, f, slot[f], limit); return false; }
+        if (seen[slot[f]]++) { set_error("%s: slot %d appears twice", fn, slot[f]); return false; }
+    }
     return true;
 }
 
@@ -252,12 +318,14 @@ sgs_lastframe_batch lastframe_search(const sgs_tracker* t, const LastFrame& l, f
 }
 
 // The per-frame inputs of a track call.  NULL: not given -- computed on the device (u_right of an RGB-D step, F), or the tracker's own
-// array as it is (boxes).  prev_xy replaces prev_index in sgs_tracker_track, which runs no LK.
+// array as it is (boxes).  prev_xy replaces prev_index in sgs_tracker_track, which runs no LK.  slot (stream steps) replaces prev_index: the previous
+// frames come from the slots' StreamState; new_stream may be NULL.
 struct TrackInputs {
     LastFrame last;
     const float* u_right = nullptr;
     const int32_t* prev_index = nullptr; const float* prev_xy = nullptr; const double* F = nullptr;
     const sgs_rect* boxes = nullptr; const int32_t* nboxes = nullptr; const uint8_t* have_dyn = nullptr;
+    const int32_t* slot = nullptr; const uint8_t* new_stream = nullptr;
 };
 
 // Host inputs -> the tracker's device arrays.  What LK and the F estimate read goes first, on the tracker's stream; the bulk (u_right, the
@@ -272,6 +340,8 @@ int stage_host_inputs(sgs_tracker* t, size_t B, const TrackInputs& in) {
     if (in.boxes) SGS_CUDA_TRY(h2d(t->d_boxes, in.boxes, B * t->max_boxes * sizeof(sgs_rect), st));
     if (in.nboxes) SGS_CUDA_TRY(h2d(t->d_nboxes, in.nboxes, B * 4, st));
     if (in.have_dyn) SGS_CUDA_TRY(h2d(t->d_have, in.have_dyn, B, st));
+    if (in.slot) SGS_CUDA_TRY(h2d(t->ss.slot, in.slot, B * 4, st));
+    if (in.new_stream) SGS_CUDA_TRY(h2d(t->ss.new_stream, in.new_stream, B, st));
     const LastFrame& l = in.last;
     if (in.u_right) SGS_CUDA_TRY(h2d(t->d_uright_in, in.u_right, B * K * 4, cs));
     SGS_CUDA_TRY(h2d(t->d_lxyz, l.xyz, B * M * 12, cs)); SGS_CUDA_TRY(h2d(t->d_ldesc, l.desc, B * M * 32, cs));
@@ -331,6 +401,22 @@ int ensure_rgbd_buffers(sgs_tracker* t, size_t raw_bytes) {
         SGS_CUDA_TRY(R.regrow(&t->d_dz, B * K * 4 + 16)); SGS_CUDA_TRY(R.regrow(&t->d_dz2, B * K * 4 + 16)); SGS_CUDA_TRY(R.regrow(&t->d_kpsun2, B * K * sizeof(sgs_keypoint) + 16));
     }
     SGS_CUDA_TRY(R.grow(&t->d_depth_raw, &t->d_depth_raw_cap, raw_bytes * B));
+    return SGS_OK;
+}
+
+// the StreamState, allocated on the first stream call; every slot starts empty (cleared on `st`, ahead of the call's first read)
+int ensure_stream_state(sgs_tracker* t, cudaStream_t st) {
+    StreamState& S = t->ss;
+    if (S.ready) return SGS_OK;     // set last: a failed first attempt is repeated whole by the next call
+    HandleResources& R = t->res;
+    const size_t B = t->max_batch, MB = t->max_boxes;
+    SGS_CUDA_TRY(R.regrow(&S.levels, lk_pyramid(t->lk.get()).bytes)); SGS_CUDA_TRY(R.regrow(&S.boxes, B * MB * sizeof(sgs_rect) + 16));
+    SGS_CUDA_TRY(R.regrow(&S.nboxes, B * 4 + 16)); SGS_CUDA_TRY(R.regrow(&S.have, B + 16)); SGS_CUDA_TRY(R.regrow(&S.state, B + 16));
+    SGS_CUDA_TRY(R.regrow(&S.slot, B * 4 + 16)); SGS_CUDA_TRY(R.regrow(&S.new_stream, B + 16)); SGS_CUDA_TRY(R.regrow(&S.row, B * 4 + 16));
+    SGS_CUDA_TRY(R.regrow(&S.first, B + 16)); SGS_CUDA_TRY(R.regrow(&S.pre_have, B + 16)); SGS_CUDA_TRY(R.regrow(&S.pre_nboxes, B * 4 + 16));
+    SGS_CUDA_TRY(R.regrow(&S.pre_boxes, B * MB * sizeof(sgs_rect) + 16));
+    SGS_CUDA_TRY(cudaMemsetAsync(S.state, 0, B, st));
+    S.ready = true;
     return SGS_OK;
 }
 
@@ -398,20 +484,43 @@ int enqueue_step(sgs_tracker* t, sgs_detector* det, const StepFrames& fr, int nf
         if (rc != SGS_OK) return rc;
     }
     t->last_nframes = nframes;
-    const int32_t* d_pidx = in.prev_index;
+    const int32_t* d_pidx = in.prev_index; const int32_t* d_slot = in.slot; const uint8_t* d_new = in.new_stream;
     LastFrame last = in.last;
     if (host_inputs) {
         rc = stage_host_inputs(t, B, in);
         if (rc != SGS_OK) return rc;
         d_pidx = t->d_pidx; last = device_last(t);
+        d_slot = t->ss.slot; d_new = in.new_stream ? t->ss.new_stream : nullptr;
     }
-    rc = sgs_tracker_lk_device(t, d_frames, nframes, fstride, pitch, d_pidx, st);
+    // stream step: each frame's previous frame is the last one its slot received (StreamState), not a row of this batch
+    const bool streams = in.slot != nullptr;
+    const StreamState& S = t->ss;
+    const Extracted ex = extracted(t);
+    if (streams) {
+        stream_resolve_kernel<<<(nframes + 127) / 128, 128, 0, st>>>(nframes, d_slot, d_new, S.state, S.have, S.nboxes, S.boxes, t->max_boxes, S.row, S.first,
+                                                                      S.pre_have, S.pre_nboxes, S.pre_boxes);
+        rc = lk_track_from_store(t->lk.get(), d_frames, nframes, fstride, pitch, ex.kps, ex.n, ex.cap, S.levels, S.row, t->d_prev, st);
+    } else {
+        rc = sgs_tracker_lk_device(t, d_frames, nframes, fstride, pitch, d_pidx, st);
+    }
     if (rc != SGS_OK) return rc;
     SGS_CUDA_TRY(cudaStreamWaitEvent(st, t->det_ev, 0));                  // the join of src/Frame.cc:478-481: boxes of every frame of the batch are there
-    rc = sgs_tracker_fundamental_device(t, nframes, nullptr, nullptr, nullptr, d_pidx, st);
+    if (streams) {
+        // the parameters of sgs_tracker_fundamental_device; the previous boxes and flag are the gathered ones.  Then LK has read the slots' levels, and
+        // the frames become their slots' state.
+        rc = fm_launch(ex.kps, nullptr, reinterpret_cast<const float2*>(t->d_prev), ex.n, ex.cap, nframes, S.pre_boxes, S.pre_nboxes, S.pre_have, t->max_boxes,
+                       nullptr, S.first, 1.0, 0.99, 1000, t->d_Fgpu, t->d_finfo, nullptr, st);
+        if (rc != SGS_OK) return rc;
+        const LkPyramid P = lk_pyramid(t->lk.get());
+        const int gx = (int)std::max<int64_t>(1, (P.frame_bytes[0] / 16 + 2047) / 2048);
+        stream_commit_kernel<<<dim3(gx, nframes), 256, 0, st>>>(P, S.levels, d_slot, S.first, t->d_boxes, t->d_nboxes, t->d_have, t->max_boxes, S.boxes,
+                                                                S.nboxes, S.have, S.state);
+        SGS_CUDA_TRY(cudaGetLastError());
+    } else {
+        rc = sgs_tracker_fundamental_device(t, nframes, nullptr, nullptr, nullptr, d_pidx, st);
+    }
     if (rc != SGS_OK) return rc;
     if (rgbd) {     // Frame.cc:146-174 undistorts and looks the depth up after the rejection; both are per point, so doing them first gives the same values
-        const Extracted ex = extracted(t);
         rc = sgs_undistort_batch_device(ex.kps, ex.n, ex.cap, nframes, t->cam.fx, t->cam.fy, t->cam.cx, t->cam.cy, fr.fmt->dist_coef, t->d_kpsun, st);
         if (rc != SGS_OK) return rc;
         rc = sgs_stereo_from_depth_batch_device(ex.kps, t->d_kpsun, ex.n, ex.cap, nframes, depth, depth_fstride, depth_pitch, t->cam.bf, t->d_uright_in, t->d_dz, st);
@@ -813,6 +922,68 @@ SGS_API int sgs_tracker_step_rgbd(sgs_tracker* t, sgs_detector* det, const uint8
     fr.d_depth = t->d_depth_raw; fr.depth_stride = row * t->height; fr.depth_pitch = (int)row; fr.fmt = fmt;
     TrackInputs in{last};
     in.prev_index = prev_index;      // no u_right: the step computes it from the depth
+    rc = enqueue_step(t, det, fr, nframes, in, true, th, mono, check_orientation, t->st);
+    if (rc != SGS_OK) return rc;
+    return download_results(t, nframes, out);
+}
+
+// The RGB-D step for live streams, one new frame per stream slot: the previous frames are the slots' (StreamState); see sgs_abi.h.
+SGS_API int sgs_tracker_step_rgbd_stream_device(sgs_tracker* t, sgs_detector* det, const uint8_t* d_rgb, size_t rgb_stride, int rgb_pitch, const void* d_depth,
+                                                size_t depth_stride, int depth_pitch, const sgs_rgbd_format* fmt, int nframes, const int32_t* d_slot,
+                                                const uint8_t* d_new_stream, const float* last_xyz, const uint8_t* last_desc, const uint8_t* last_flags,
+                                                const int32_t* last_octave, const float* last_angle, const int32_t* last_n, const float* tcw_cur,
+                                                const float* tcw_last, float th, int mono, int check_orientation, void* stream) {
+    const char* const fn = "sgs_tracker_step_rgbd_stream_device";
+    LastFrame last;
+    last.xyz = last_xyz; last.desc = last_desc; last.flags = last_flags; last.octave = last_octave; last.angle = last_angle; last.n = last_n;
+    last.tcw_cur = tcw_cur; last.tcw_last = tcw_last;
+    if (!t || !det || !d_rgb || !d_depth || !fmt || !d_slot || !last.complete()) return bad(fn, "NULL argument");
+    if (!frames_ok(fn, nframes, t->max_batch) || !rgb_layout_ok(t, fn, rgb_stride, rgb_pitch) ||
+        !depth_args_ok(t, fn, fmt, depth_stride, depth_pitch, d_depth)) return SGS_ERR_INVALID;
+    SGS_CUDA_TRY(cudaSetDevice(t->device));
+    cudaStream_t st = stream ? (cudaStream_t)stream : t->st;
+    int rc = ensure_rgbd_buffers(t, 0);
+    if (rc != SGS_OK) return rc;
+    rc = ensure_stream_state(t, st);
+    if (rc != SGS_OK) return rc;
+    StepFrames fr{d_rgb, rgb_stride, rgb_pitch, st};
+    fr.d_depth = d_depth; fr.depth_stride = depth_stride; fr.depth_pitch = depth_pitch; fr.fmt = fmt;
+    TrackInputs in{last};
+    in.slot = d_slot; in.new_stream = d_new_stream;
+    return enqueue_step(t, det, fr, nframes, in, false, th, mono, check_orientation, st);
+}
+
+// The same from host buffers; the slots are checked (range, duplicates) before anything runs.
+SGS_API int sgs_tracker_step_rgbd_stream(sgs_tracker* t, sgs_detector* det, const uint8_t* rgb, size_t rgb_stride, int rgb_pitch, const void* depth,
+                                         size_t depth_stride, int depth_pitch, const sgs_rgbd_format* fmt, int nframes, const int32_t* slot,
+                                         const uint8_t* new_stream, const float* last_xyz, const uint8_t* last_desc, const uint8_t* last_flags,
+                                         const int32_t* last_octave, const float* last_angle, const int32_t* last_n, const float* tcw_cur,
+                                         const float* tcw_last, float th, int mono, int check_orientation, sgs_keypoint* kps_out, uint8_t* desc_out,
+                                         float* u_right_out, int32_t* counts_out, int32_t* cur_mp_out, int32_t* nmatches_out, sgs_rect* boxes_out,
+                                         int32_t* nboxes_out, uint8_t* have_out, sgs_keypoint* kps_un_out, float* depth_out) {
+    const char* const fn = "sgs_tracker_step_rgbd_stream";
+    LastFrame last;
+    last.xyz = last_xyz; last.desc = last_desc; last.flags = last_flags; last.octave = last_octave; last.angle = last_angle; last.n = last_n;
+    last.tcw_cur = tcw_cur; last.tcw_last = tcw_last;
+    HostOutputs out;
+    out.kps = kps_out; out.desc = desc_out; out.u_right = u_right_out; out.counts = counts_out; out.cur_mp = cur_mp_out; out.nmatches = nmatches_out;
+    out.boxes = boxes_out; out.nboxes = nboxes_out; out.have = have_out; out.kps_un = kps_un_out; out.depth = depth_out;
+    if (!t || !det || !rgb || !depth || !fmt || !slot || !last.complete() || !out.complete()) return bad(fn, "NULL argument");
+    if (!slots_ok(fn, nframes, t->max_batch, slot) || !rgb_layout_ok(t, fn, rgb_stride, rgb_pitch) ||
+        !depth_args_ok(t, fn, fmt, depth_stride, depth_pitch, depth)) return SGS_ERR_INVALID;
+    SGS_CUDA_TRY(cudaSetDevice(t->device));
+    const size_t row = (size_t)t->width * (fmt->depth_type == 0 ? 2 : 4);
+    int rc = ensure_rgbd_buffers(t, row * t->height);
+    if (rc != SGS_OK) return rc;
+    rc = ensure_stream_state(t, t->st);
+    if (rc != SGS_OK) return rc;
+    rc = upload_rgb(t, rgb, rgb_stride, rgb_pitch, nframes);
+    if (rc != SGS_OK) return rc;
+    SGS_CUDA_TRY(upload_frames(t->d_depth_raw, depth, depth_stride, depth_pitch, row, t->height, nframes, t->st));
+    StepFrames fr = staged_rgb(t);
+    fr.d_depth = t->d_depth_raw; fr.depth_stride = row * t->height; fr.depth_pitch = (int)row; fr.fmt = fmt;
+    TrackInputs in{last};
+    in.slot = slot; in.new_stream = new_stream;
     rc = enqueue_step(t, det, fr, nframes, in, true, th, mono, check_orientation, t->st);
     if (rc != SGS_OK) return rc;
     return download_results(t, nframes, out);

@@ -451,6 +451,13 @@ class Tracker(_Handle):
         out_ptrs: kps, desc, u_right (or 0), counts, cur_mp, nmatches   (all raw host addresses)"""
         check(lib().sgs_tracker_track(self.h, nframes, *ptrs, th, int(mono), int(check_ori), *out_ptrs))
 
+    def step_rgbd_stream_device(self, det, d_rgb, rgb_stride, rgb_pitch, d_depth, depth_stride, depth_pitch, fmt, nframes, d_slot, d_new_stream, last_ptrs,
+                                th, mono, check_ori, stream=0):
+        """sgs_tracker_step_rgbd_stream_device: frame f is the next frame of stream slot d_slot[f]; d_new_stream: a device uint8 array or 0 (none);
+        last_ptrs: the eight last-frame device arrays (xyz, desc, flags, octave, angle, n, tcw_cur, tcw_last).  Enqueued on `stream`, not synchronised."""
+        check(lib().sgs_tracker_step_rgbd_stream_device(self.h, det.h, d_rgb, rgb_stride, rgb_pitch, d_depth, depth_stride, depth_pitch, C.byref(fmt), nframes,
+                                                        d_slot, d_new_stream or None, *last_ptrs, th, int(mono), int(check_ori), stream or None))
+
 
 class LK(_Handle):
     """cv::calcOpticalFlowPyrLK with the reference's parameters (sgs_lk_* of include/sgs_abi.h)."""
