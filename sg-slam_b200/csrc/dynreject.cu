@@ -7,6 +7,7 @@
 
 #include <vector>
 
+#include "block_compact.cuh"
 #include "host_stage.cuh"
 #include "sgs_common.h"
 
@@ -57,20 +58,17 @@ __global__ void __launch_bounds__(kDynThreads) dynreject_batch_kernel(const sgs_
                                                                       sgs_keypoint* __restrict__ kps_out, uint8_t* __restrict__ desc_out,
                                                                       int32_t* __restrict__ counts_out, uint8_t* __restrict__ keep_out) {
     extern __shared__ int32_t s_pos[];   // [cap] exclusive positions (or -1)
-    __shared__ int s_warp[kDynThreads / 32];
-    __shared__ int s_total, s_carry;
     __shared__ double sF[9];
     const int f = blockIdx.x;
     const int n = min(counts[f], cap);
     const int64_t base = (int64_t)f * cap;
     if (threadIdx.x < 9) sF[threadIdx.x] = Fm[9 * f + threadIdx.x];
-    if (threadIdx.x == 0) { s_carry = 0; }
     __syncthreads();
     const bool have_F = !(sF[0] != sF[0]);   // NaN marks the empty matrix (quirk Q11: keep everything)
     const bool dyn = have_dyn[f] != 0;
     const int nb = dyn ? min(nboxes[f], max_boxes) : 0;
     const sgs_rect* bx = boxes + (int64_t)f * max_boxes;
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    int total = 0;
     for (int i0 = 0; i0 < n; i0 += kDynThreads) {
         const int i = i0 + threadIdx.x;
         bool ok = false;
@@ -81,19 +79,10 @@ __global__ void __launch_bounds__(kDynThreads) dynreject_batch_kernel(const sgs_
             ok = have_F ? epi_keep(k.x, k.y, p.x, p.y, sF, inb, nullptr) : true;
             if (keep_out) keep_out[base + i] = ok ? 1 : 0;
         }
-        const unsigned m = __ballot_sync(0xffffffffu, ok);
-        if (lane == 0) s_warp[warp] = __popc(m);
-        __syncthreads();
-        int off = s_carry;
-        for (int w = 0; w < warp; ++w) off += s_warp[w];
-        if (i < n) s_pos[i] = ok ? off + __popc(m & ((1u << lane) - 1)) : -1;
-        __syncthreads();
-        if (threadIdx.x == 0) { int t = 0; for (int w = 0; w < kDynThreads / 32; ++w) t += s_warp[w]; s_carry += t; }
-        __syncthreads();
+        const int slot = block_ordered_slot<kDynThreads>(ok, total);
+        if (i < n) s_pos[i] = slot;
     }
-    if (threadIdx.x == 0) s_total = s_carry;
     __syncthreads();
-    const int total = s_total;
     const bool restore = dyn && ((double)total < (double)nfeatures * 0.1);     // Frame.cc:599
     const int n_out = restore ? n : total;
     if (threadIdx.x == 0) counts_out[f] = n_out;

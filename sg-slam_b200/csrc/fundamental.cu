@@ -4,9 +4,10 @@
 // listed in DESIGN.md and pinned to cv2 by the parity tests).  Here the loop is re-cut for the GPU without changing its outcome:
 //   * one block per frame; the frame's correspondences sit in shared memory;
 //   * the sample indices of a ROUND of iterations are drawn ahead by one thread (the MWC generator and the redraw rules do not
-//     depend on the models), one thread per iteration solves its 7-point problem, then the whole block counts the inliers of every
-//     candidate model; a single thread finally replays the accept / update-niters decisions in iteration order, so the winner, the
-//     adaptive stop and the tie-breaks are those of the sequential loop.  Iterations drawn past the stop are discarded.
+//     depend on the models), one thread per iteration solves its 7-point problem, then every candidate model is scored (RANSAC: the
+//     whole block counts its inliers; LMedS: the solving thread takes its median error); a single thread finally replays the accept /
+//     update-niters decisions in iteration order, so the winner, the adaptive stop and the tie-breaks are those of the sequential loop.
+//     Iterations drawn past the stop are discarded.  RANSAC and LMedS run this one loop (fm_sample_rounds) with their own scoring.
 //   * the 2-dimensional null space of the 7x9 system is the span OpenCV's JacobiSVD completion step produces: fixed pseudo-random
 //     sign vectors projected off the row space.  The row space comes from a twice-applied modified Gram-Schmidt instead of the
 //     Jacobi sweeps (same subspace, ~1e-15 relative difference in F).
@@ -19,6 +20,7 @@
 #include <cfloat>
 #include <vector>
 
+#include "block_compact.cuh"
 #include "host_stage.cuh"
 #include "internal_launch.cuh"
 #include "sgs_common.h"
@@ -26,7 +28,7 @@
 namespace sgs {
 
 constexpr int kFmThreads = 256;
-constexpr int kFmRound = 32;          // iterations per round (the first round draws kFmFirstRound)
+constexpr int kFmRound = 32;          // iterations per round (RANSAC's first round draws kFmFirstRound)
 constexpr int kFmFirstRound = 8;
 constexpr int kFmRansacAttempts = 10000;  // getSubset's cap on redraws per sample: RANSAC passes 10000,
 constexpr int kFmLmedsAttempts = 1000;    // LMedS keeps the default of 1000
@@ -186,15 +188,6 @@ __device__ int fm_run7point(const float2* m1, const float2* m2, double* Fout) {
     return n;
 }
 
-__device__ __forceinline__ bool fm_inlier(const float4 p, const double* F, float t) {      // FMEstimatorCallback::computeError + findInliers
-    const double x1 = p.x, y1 = p.y, x2 = p.z, y2 = p.w;
-    double a = F[0] * x1 + F[1] * y1 + F[2], b = F[3] * x1 + F[4] * y1 + F[5], c = F[6] * x1 + F[7] * y1 + F[8];
-    const double s2 = 1. / (a * a + b * b), d2 = x2 * a + y2 * b + c;
-    a = F[0] * x2 + F[3] * y2 + F[6]; b = F[1] * x2 + F[4] * y2 + F[7]; c = F[2] * x2 + F[5] * y2 + F[8];
-    const double s1 = 1. / (a * a + b * b), d1 = x1 * a + y1 * b + c;
-    const float err = (float)fmax(d1 * d1 * s1, d2 * d2 * s2);
-    return err <= t;
-}
 __device__ __forceinline__ float fm_error(const float4 p, const double* F) {                  // FMEstimatorCallback::computeError, one pair
     const double x1 = p.x, y1 = p.y, x2 = p.z, y2 = p.w;
     double a = F[0] * x1 + F[1] * y1 + F[2], b = F[3] * x1 + F[4] * y1 + F[5], c = F[6] * x1 + F[7] * y1 + F[8];
@@ -241,46 +234,131 @@ __device__ int fm_update_iters(double p, double ep, int max_iters) {     // RANS
     return denom >= 0 || -num >= max_iters * (-denom) ? max_iters : (int)rint(num / denom);
 }
 
-// cur points come from keypoints (kps != nullptr) or a float2 array; prev from a float2 array.
-// info[f] = {pairs used, inliers of the returned model, iterations run, status (0 ok, 1 fewer than 7 pairs, 2 no model, 3 no previous frame)}
-// 7 pairs: the 7-point solver directly; 8..14 pairs: LMedS; 15 and more: RANSAC -- the three branches of cv::findFundamentalMat(FM_RANSAC).
-__global__ void __launch_bounds__(kFmThreads) fm_ransac_kernel(const sgs_keypoint* __restrict__ kps, const float2* __restrict__ cur_xy,
-                                                               const float2* __restrict__ prev_xy, const int32_t* __restrict__ counts, int cap,
-                                                               const sgs_rect* __restrict__ prev_boxes, const int32_t* __restrict__ prev_nboxes,
-                                                               const uint8_t* __restrict__ prev_have_dyn, int max_boxes,
-                                                               const int32_t* __restrict__ prev_index, const uint8_t* __restrict__ no_prev_f, double thresh,
-                                                               double confidence, int max_iters, double* __restrict__ F_out,
-                                                               int32_t* __restrict__ info, uint8_t* __restrict__ mask_out) {
-    extern __shared__ float4 s_pts[];                  // [cap] (x1, y1, x2, y2), the pairs handed to the estimator, in order
-    __shared__ double s_models[kFmRound * 3][9];
-    __shared__ int s_nmodels[kFmRound], s_good[kFmRound * 3], s_idx[kFmRound][7];
-    __shared__ double s_best[9];
-    __shared__ int s_warp[kFmThreads / 32];
-    __shared__ int s_n, s_niters, s_done, s_round, s_maxgood, s_carry, s_drawn_ok;
-    __shared__ unsigned long long s_rng;
-    const int f = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int n_all = counts ? min(counts[f], cap) : cap;
-    const float2* prev = prev_xy + (int64_t)f * cap;
-    auto cur_pt = [&](int i) -> float2 {
-        if (kps) { const sgs_keypoint k = kps[(int64_t)f * cap + i]; return make_float2(k.x, k.y); }
-        return cur_xy[(int64_t)f * cap + i];
-    };
-    // ---- selection (src/Frame.cc:454-472): ordered compaction of the pairs whose previous point is outside the previous boxes
-    // prev_index (may be NULL): the batch row holding the previous frame's boxes; prev_index[f] == f marks a frame without a previous one.
-    // no_prev_f (stream steps, prev_index NULL): the same mark per frame, the previous frame's boxes and flag gathered into row f
-    const int fb = prev_index ? prev_index[f] : f;
-    const bool no_prev = no_prev_f ? no_prev_f[f] != 0 : prev_index && fb == f;
+// Block state of the sampling loop and the model it keeps
+struct FmShared {
+    double models[kFmRound * 3 * 9];        // the 7-point models of the round's iterations: model m (of iteration m / 3) at models + 9 * m
+    double best[9];
+    union { int good[kFmRound * 3]; float med[kFmRound * 3]; };      // each model's score: RANSAC inlier count, LMedS median error
+    int nmodels[kFmRound], idx[kFmRound][7];
+    int round, done, niters, drawn_ok, maxgood;
+    double minmed;
+    unsigned long long rng;
+};
+
+// run7Point on sample s.idx[it]: models 3 * it ... into s.models, their number into s.nmodels[it]
+__device__ void fm_solve_sample(FmShared& s, const float4* pts, int it) {
+    float2 a[7], b[7];
+    for (int i = 0; i < 7; ++i) { const float4 p = pts[s.idx[it][i]]; a[i] = make_float2(p.x, p.y); b[i] = make_float2(p.z, p.w); }
+    s.nmodels[it] = fm_run7point(a, b, s.models + 27 * it);
+}
+
+// RANSAC (15 pairs and more): a model's score is its number of inliers (error <= t), counted by the whole block; the first model with more than
+// max(best, 6) inliers is kept and shortens the loop (RANSACUpdateNumIters).
+struct FmRansac {
+    static constexpr int kFirstRound = kFmFirstRound, kAttempts = kFmRansacAttempts;
+    int n; float t; double confidence;
+    __device__ void score(FmShared& s, const float4* pts, int round) const {
+        if (threadIdx.x < kFmRound * 3) s.good[threadIdx.x] = 0;
+        __syncthreads();
+        for (int it = 0; it < round; ++it) {
+            const int nm = s.nmodels[it];
+            for (int k = 0; k < nm; ++k) {
+                const double* Fm = s.models + 9 * (it * 3 + k);
+                int cnt = 0;
+                for (int i = threadIdx.x; i < n; i += kFmThreads) cnt += fm_error(pts[i], Fm) <= t ? 1 : 0;
+#pragma unroll
+                for (int o = 16; o > 0; o >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
+                if ((threadIdx.x & 31) == 0 && cnt) atomicAdd(&s.good[it * 3 + k], cnt);
+            }
+        }
+    }
+    __device__ void take(FmShared& s, int m) const {
+        const int good = s.good[m];
+        if (good > max(s.maxgood, 6)) {
+            for (int i = 0; i < 9; ++i) s.best[i] = s.models[9 * m + i];
+            s.maxgood = good;
+            s.niters = fm_update_iters(confidence, (double)(n - good) / n, s.niters);
+        }
+    }
+};
+
+// LMedS (8..14 pairs): a model's score is the median of its n errors (element n / 2 of the sorted errors), taken by the thread that solved it; a
+// strictly smaller median replaces the kept model.
+struct FmLmeds {
+    static constexpr int kFirstRound = kFmRound, kAttempts = kFmLmedsAttempts;
+    int n;
+    __device__ void score(FmShared& s, const float4* pts, int round) const {
+        const int it = threadIdx.x;
+        if (it >= round) return;
+        for (int k = 0; k < s.nmodels[it]; ++k) {
+            float e[14];
+            for (int i = 0; i < n; ++i) {                              // insertion sort of the n <= 14 errors
+                const float v = fm_error(pts[i], s.models + 9 * (it * 3 + k));
+                int j = i;
+                for (; j > 0 && e[j - 1] > v; --j) e[j] = e[j - 1];
+                e[j] = v;
+            }
+            s.med[it * 3 + k] = e[n / 2];
+        }
+    }
+    __device__ void take(FmShared& s, int m) const {
+        const double med = (double)s.med[m];
+        if (med < s.minmed) { s.minmed = med; for (int i = 0; i < 9; ++i) s.best[i] = s.models[9 * m + i]; }
+    }
+};
+
+// The sampling loop of RANSACPointSetRegistrator::run and LMeDSPointSetRegistrator::run over the n pairs, for at most niters iterations, in rounds:
+// thread 0 draws the round's samples (the generator state carries over in s.rng), one thread per iteration solves its 7-point problem, the policy
+// scores every model, then thread 0 replays the policy's decisions in iteration and model order, so the kept model, the stop and the tie-breaks are
+// those of the sequential loop.  Iterations drawn past the stop are discarded; a failed draw ends the loop after its round.
+template <class Policy>
+__device__ void fm_sample_rounds(FmShared& s, const float4* pts, int n, int niters, const Policy& pol) {
+    const int tid = threadIdx.x;
+    if (tid == 0) { s.rng = 0xffffffffffffffffULL; s.drawn_ok = 1; s.done = 0; s.niters = niters; s.maxgood = 0; s.minmed = DBL_MAX; }
+    __syncthreads();
+    for (bool first = true;; first = false) {
+        if (tid == 0) {
+            FmRng rng; rng.state = s.rng;
+            int ok = 1;
+            s.round = fm_draw_samples(rng, pts, n, min(first ? Policy::kFirstRound : kFmRound, s.niters - s.done), Policy::kAttempts, s.idx, &ok);
+            if (!ok) s.drawn_ok = 0;
+            s.rng = rng.state;
+        }
+        __syncthreads();
+        const int round = s.round;
+        if (tid < round) fm_solve_sample(s, pts, tid);
+        pol.score(s, pts, round);
+        __syncthreads();
+        if (tid == 0)
+            for (int it = 0; it < round && s.done < s.niters; ++it, ++s.done)
+                for (int k = 0; k < s.nmodels[it]; ++k) pol.take(s, it * 3 + k);
+        __syncthreads();
+        if (s.done >= s.niters || !s.drawn_ok) break;
+        __syncthreads();
+    }
+}
+
+// Selection (src/Frame.cc:454-468): the pairs of frame f handed to the estimator, into pts in order, and their number.  When the previous frame
+// had potential dynamic objects, the pairs whose previous point lies outside its boxes, if more than 20 are left; otherwise all n_all pairs.
+// no_prev: frame f has no previous frame.
+__device__ int fm_select_pairs(const FmArgs& A, int f, int n_all, float4* pts, bool& no_prev) {
+    const int fb = A.prev_index ? A.prev_index[f] : f;
+    no_prev = A.no_prev ? A.no_prev[f] != 0 : A.prev_index && fb == f;
     // The reference keeps "the previous frame had potential dynamic objects" at file scope and writes it only inside the rejection (src/Frame.cc:482-491), which
     // the first frame of a stream never runs (:154-162): the detections of a stream's first frame do not filter the pairs of its second frame (quirk Q13,
     // pinned by tests/test_frame_ref.py against the reference's own Frame.cc).  With prev_index the rows say which frames are first ones.
-    const bool pre_dyn = prev_have_dyn && prev_have_dyn[fb] != 0 && !(prev_index && prev_index[fb] == fb);
-    if (tid == 0) s_carry = 0;
-    __syncthreads();
+    const bool pre_dyn = A.prev_have_dyn && A.prev_have_dyn[fb] != 0 && !(A.prev_index && A.prev_index[fb] == fb);
+    const float2* prev = A.prev + (int64_t)f * A.cap;
+    auto cur_pt = [&](int i) -> float2 {
+        if (A.kps) { const sgs_keypoint k = A.kps[(int64_t)f * A.cap + i]; return make_float2(k.x, k.y); }
+        return A.cur[(int64_t)f * A.cap + i];
+    };
+    int n = 0;
     if (pre_dyn && !no_prev) {
-        const sgs_rect* boxes = prev_boxes + (int64_t)fb * max_boxes;
-        const int nb = min(prev_nboxes[fb], max_boxes);
+        const sgs_rect* boxes = A.prev_boxes + (int64_t)fb * A.max_boxes;
+        const int nb = min(A.prev_nboxes[fb], A.max_boxes);
         for (int base = 0; base < n_all; base += kFmThreads) {
-            const int i = base + tid;
+            const int i = base + threadIdx.x;
             bool keep = false;
             float2 c = make_float2(0.f, 0.f), p = c;
             if (i < n_all) {
@@ -291,196 +369,77 @@ __global__ void __launch_bounds__(kFmThreads) fm_ransac_kernel(const sgs_keypoin
                     if (p.x > r.x && p.x < __fadd_rn(r.x, r.w) && p.y > r.y && p.y < __fadd_rn(r.y, r.h)) { keep = false; break; }
                 }
             }
-            const unsigned bal = __ballot_sync(0xffffffffu, keep);
-            if (lane == 0) s_warp[warp] = __popc(bal);
-            __syncthreads();
-            int off = s_carry;
-            for (int w = 0; w < warp; ++w) off += s_warp[w];
-            if (keep) s_pts[off + __popc(bal & ((1u << lane) - 1u))] = make_float4(c.x, c.y, p.x, p.y);
-            __syncthreads();
-            if (tid == 0) { int tot = 0; for (int w = 0; w < kFmThreads / 32; ++w) tot += s_warp[w]; s_carry += tot; }
-            __syncthreads();
+            const int slot = block_ordered_slot<kFmThreads>(keep, n);
+            if (slot >= 0) pts[slot] = make_float4(c.x, c.y, p.x, p.y);
         }
     }
-    int n = s_carry;
     if (!(pre_dyn && n > 20)) {
         __syncthreads();
-        for (int i = tid; i < n_all; i += kFmThreads) { const float2 c = cur_pt(i), p = prev[i]; s_pts[i] = make_float4(c.x, c.y, p.x, p.y); }
+        for (int i = threadIdx.x; i < n_all; i += kFmThreads) { const float2 c = cur_pt(i), p = prev[i]; pts[i] = make_float4(c.x, c.y, p.x, p.y); }
         n = n_all;
     }
     __syncthreads();
-    double* Fo = F_out + (int64_t)f * 9;
-    int32_t* inf = info ? info + (int64_t)f * 4 : nullptr;
-    if (thresh <= 0) thresh = 3;
-    if (confidence < DBL_EPSILON || confidence > 1 - DBL_EPSILON) confidence = 0.99;
-    const double kNaN = __longlong_as_double(0x7ff8000000000000LL);
-    if (n < 7 || no_prev) {           // cv::findFundamentalMat returns an empty matrix below 7 pairs (fundam.cpp): "empty F" = NaN here
-        if (tid < 9) Fo[tid] = kNaN;
-        if (tid == 0 && inf) { inf[0] = n; inf[1] = 0; inf[2] = 0; inf[3] = no_prev ? 3 : 1; }
-        if (mask_out) for (int i = tid; i < n_all; i += kFmThreads) mask_out[(int64_t)f * cap + i] = 0;
-        return;
-    }
-    if (n == 7) {                     // exactly 7 pairs: the 7-point solver itself, up to three stacked solutions; the reference reads rows 0..2 = the first
-        if (tid == 0) {
-            float2 a[7], b[7];
-            for (int i = 0; i < 7; ++i) { const float4 p = s_pts[i]; a[i] = make_float2(p.x, p.y); b[i] = make_float2(p.z, p.w); }
-            double Fm[27];
-            const int nm = fm_run7point(a, b, Fm);
-            for (int i = 0; i < 9; ++i) Fo[i] = nm > 0 ? Fm[i] : kNaN;
-            if (inf) { inf[0] = n; inf[1] = nm > 0 ? 7 : 0; inf[2] = 1; inf[3] = nm > 0 ? 0 : 2; }
-        }
-        if (mask_out) for (int i = tid; i < n_all; i += kFmThreads) mask_out[(int64_t)f * cap + i] = i < n ? 1 : 0;      // OpenCV sets the whole mask
-        return;
-    }
-    if (n < 15) {
-        // 8..14 pairs: cv::findFundamentalMat switches to LMeDSPointSetRegistrator(cb, 7, confidence, max_iters) (fundam.cpp; ptsetreg.cpp): a FIXED
-        // number of samples (outlier ratio 0.45, at most max_iters, at least 3), each drawn in at most 1000 attempts, the model with the smallest
-        // median error (element n/2 of the sorted errors, strict '<'), inliers within sigma = 2.5 * 1.4826 * (1 + 5 / (n - 7)) * sqrt(median)
-        // (at least 0.001); fewer than 7 inliers -> empty matrix.
-        __shared__ float s_med[kFmRound * 3];
-        __shared__ double s_minmed;
-        __shared__ int s_lm_good;
-        const int niters = max(fm_update_iters(confidence, 0.45, max_iters), 3);
-        if (tid == 0) { s_done = 0; s_rng = 0xffffffffffffffffULL; s_minmed = DBL_MAX; s_drawn_ok = 1; s_lm_good = 0; }
-        __syncthreads();
-        while (true) {
-            if (tid == 0) {
-                FmRng rng; rng.state = s_rng;
-                int okd = 1;
-                s_round = fm_draw_samples(rng, s_pts, n, min(kFmRound, niters - s_done), kFmLmedsAttempts, s_idx, &okd);
-                if (!okd) s_drawn_ok = 0;
-                s_rng = rng.state;
-            }
-            __syncthreads();
-            const int round = s_round;
-            if (tid < round) {
-                float2 a[7], b[7];
-                for (int i = 0; i < 7; ++i) { const float4 p = s_pts[s_idx[tid][i]]; a[i] = make_float2(p.x, p.y); b[i] = make_float2(p.z, p.w); }
-                double Fm[27];
-                const int nm = fm_run7point(a, b, Fm);
-                s_nmodels[tid] = nm;
-                for (int k = 0; k < nm; ++k) {
-                    float e[14];
-                    for (int i = 0; i < n; ++i) {                              // insertion sort of the n <= 14 errors
-                        const float v = fm_error(s_pts[i], Fm + 9 * k);
-                        int j = i;
-                        for (; j > 0 && e[j - 1] > v; --j) e[j] = e[j - 1];
-                        e[j] = v;
-                    }
-                    s_med[tid * 3 + k] = e[n / 2];
-                    for (int i = 0; i < 9; ++i) s_models[tid * 3 + k][i] = Fm[9 * k + i];
-                }
-            }
-            __syncthreads();
-            if (tid == 0) {                                                    // sequential replay: strict improvement, iteration order, model order
-                double mm = s_minmed;
-                for (int it = 0; it < round; ++it)
-                    for (int k = 0; k < s_nmodels[it]; ++k) {
-                        const double med = (double)s_med[it * 3 + k];
-                        if (med < mm) { mm = med; for (int i = 0; i < 9; ++i) s_best[i] = s_models[it * 3 + k][i]; }
-                    }
-                s_minmed = mm; s_done += round;
-            }
-            __syncthreads();
-            if (s_done >= niters || !s_drawn_ok) break;
-            __syncthreads();
-        }
-        bool ok = s_minmed < DBL_MAX;
-        float tl = 0.f;
-        if (ok) {
-            double sigma = 2.5 * 1.4826 * (1 + 5. / (n - 7)) * sqrt(s_minmed);
-            sigma = fmax(sigma, 0.001);
-            tl = (float)(sigma * sigma);
-            if (tid < n && fm_inlier(s_pts[tid], s_best, tl)) atomicAdd(&s_lm_good, 1);
-        }
-        __syncthreads();
-        const int good = s_lm_good;
-        ok = ok && good >= 7;
-        if (tid < 9) Fo[tid] = ok ? s_best[tid] : kNaN;
-        if (tid == 0 && inf) { inf[0] = n; inf[1] = good; inf[2] = s_done; inf[3] = ok ? 0 : 2; }
-        if (mask_out) for (int i = tid; i < n_all; i += kFmThreads) mask_out[(int64_t)f * cap + i] = (ok && i < n && fm_inlier(s_pts[i], s_best, tl)) ? 1 : 0;
-        return;
-    }
-    const float t = (float)(thresh * thresh);
-    if (tid == 0) { s_n = n; s_niters = max(max_iters, 1); s_done = 0; s_maxgood = 0; s_rng = 0xffffffffffffffffULL; s_drawn_ok = 1; }
-    __syncthreads();
-    bool first = true;
-    while (true) {
-        // ---- draw the samples of this round (sequential state: one thread)
-        if (tid == 0) {
-            FmRng rng; rng.state = s_rng;
-            const int want = min(first ? kFmFirstRound : kFmRound, s_niters - s_done);
-            int okd = 1;
-            const int got = fm_draw_samples(rng, s_pts, n, want, kFmRansacAttempts, s_idx, &okd);      // a failed draw ends the loop (or fails it when it is the first iteration)
-            if (!okd) s_drawn_ok = 0;
-            s_round = got;
-            s_rng = rng.state;
-        }
-        __syncthreads();
-        const int round = s_round;
-        // ---- one thread per iteration: the 7-point models
-        if (tid < round) {
-            float2 a[7], b[7];
-            for (int i = 0; i < 7; ++i) { const float4 p = s_pts[s_idx[tid][i]]; a[i] = make_float2(p.x, p.y); b[i] = make_float2(p.z, p.w); }
-            double Fm[27];
-            const int nm = fm_run7point(a, b, Fm);
-            s_nmodels[tid] = nm;
-            for (int k = 0; k < nm; ++k)
-                for (int i = 0; i < 9; ++i) s_models[tid * 3 + k][i] = Fm[9 * k + i];
-        }
-        if (tid < kFmRound * 3) s_good[tid] = 0;
-        __syncthreads();
-        // ---- inlier counts of every candidate model: the block sweeps the points once per model
-        for (int it = 0; it < round; ++it) {
-            const int nm = s_nmodels[it];
-            for (int k = 0; k < nm; ++k) {
-                const double* Fm = s_models[it * 3 + k];
-                int cnt = 0;
-                for (int i = tid; i < n; i += kFmThreads) cnt += fm_inlier(s_pts[i], Fm, t) ? 1 : 0;
-#pragma unroll
-                for (int o = 16; o > 0; o >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
-                if (lane == 0 && cnt) atomicAdd(&s_good[it * 3 + k], cnt);
-            }
-        }
-        __syncthreads();
-        // ---- replay the sequential accept / update decisions in iteration order
-        if (tid == 0) {
-            int done = s_done, niters = s_niters, maxgood = s_maxgood;
-            for (int it = 0; it < round && done < niters; ++it, ++done) {
-                for (int k = 0; k < s_nmodels[it]; ++k) {
-                    const int good = s_good[it * 3 + k];
-                    if (good > max(maxgood, 6)) {
-                        for (int i = 0; i < 9; ++i) s_best[i] = s_models[it * 3 + k][i];
-                        maxgood = good;
-                        niters = fm_update_iters(confidence, (double)(n - good) / n, niters);
-                    }
-                }
-            }
-            s_done = done; s_niters = niters; s_maxgood = maxgood;
-        }
-        __syncthreads();
-        first = false;
-        if (s_done >= s_niters || !s_drawn_ok) break;
-        __syncthreads();
-    }
-    const bool ok = s_maxgood > 0;
-    if (tid < 9) Fo[tid] = ok ? s_best[tid] : __longlong_as_double(0x7ff8000000000000LL);
-    if (tid == 0 && inf) { inf[0] = n; inf[1] = s_maxgood; inf[2] = s_done; inf[3] = ok ? 0 : 2; }
-    if (mask_out) {         // mask of the returned model over the pairs used (positions >= n are cleared)
-        for (int i = tid; i < n_all; i += kFmThreads)
-            mask_out[(int64_t)f * cap + i] = (ok && i < n && fm_inlier(s_pts[i], s_best, t)) ? 1 : 0;
-    }
+    return n;
 }
 
-int fm_launch(const sgs_keypoint* d_kps, const float2* d_cur, const float2* d_prev, const int32_t* d_counts, int cap, int nframes,
-              const sgs_rect* d_boxes, const int32_t* d_nboxes, const uint8_t* d_have_dyn, int max_boxes, const int32_t* d_prev_index,
-              const uint8_t* d_no_prev, double thresh, double confidence, int max_iters, double* d_F, int32_t* d_info, uint8_t* d_mask, cudaStream_t st) {
-    const size_t smem = (size_t)cap * sizeof(float4);
-    if (smem > 200 * 1024) { set_error("fundamental: %d pairs per frame do not fit shared memory", cap); return SGS_ERR_UNSUPPORTED; }
+// One block per frame.  info[f] = {pairs used, inliers of the returned model, iterations run, status (0 ok, 1 fewer than 7 pairs, 2 no model, 3 no
+// previous frame)}.  7 pairs: the 7-point solver directly; 8..14 pairs: LMedS; 15 and more: RANSAC -- the three branches of
+// cv::findFundamentalMat(FM_RANSAC).
+__global__ void __launch_bounds__(kFmThreads) fm_ransac_kernel(const __grid_constant__ FmArgs A) {
+    extern __shared__ float4 s_pts[];                  // [cap] (x1, y1, x2, y2), the pairs handed to the estimator, in order
+    __shared__ FmShared s;
+    const int f = blockIdx.x, tid = threadIdx.x;
+    const int n_all = A.counts ? min(A.counts[f], A.cap) : A.cap;
+    bool no_prev;
+    const int n = fm_select_pairs(A, f, n_all, s_pts, no_prev);
+    const double thresh = A.thresh <= 0 ? 3 : A.thresh;
+    const double confidence = A.confidence < DBL_EPSILON || A.confidence > 1 - DBL_EPSILON ? 0.99 : A.confidence;
+    // the outcome: F = s.best when ok; the mask marks the pairs i < n with error <= t under F, or all of them (mask_all)
+    bool ok = false, mask_all = false;
+    int good = 0, iters = 0;
+    float t = 0.f;
+    if (n < 7 || no_prev) {
+        // cv::findFundamentalMat returns an empty matrix below 7 pairs (fundam.cpp): "empty F" = NaN here
+    } else if (n == 7) {
+        // exactly 7 pairs: the 7-point solver itself, up to three stacked solutions; the reference reads rows 0..2 = the first.  OpenCV sets the whole mask.
+        if (tid == 0) {
+            for (int i = 0; i < 7; ++i) s.idx[0][i] = i;
+            fm_solve_sample(s, s_pts, 0);
+            for (int i = 0; i < 9; ++i) s.best[i] = s.models[i];
+        }
+        __syncthreads();
+        ok = s.nmodels[0] > 0; good = ok ? 7 : 0; iters = 1; mask_all = true;
+    } else if (n < 15) {
+        // 8..14 pairs: cv::findFundamentalMat switches to LMeDSPointSetRegistrator(cb, 7, confidence, max_iters) (fundam.cpp; ptsetreg.cpp): a FIXED
+        // number of samples (outlier ratio 0.45, at most max_iters, at least 3), each drawn in at most 1000 attempts, the model with the smallest
+        // median error, inliers within sigma = 2.5 * 1.4826 * (1 + 5 / (n - 7)) * sqrt(median) (at least 0.001); fewer than 7 inliers -> empty matrix.
+        fm_sample_rounds(s, s_pts, n, max(fm_update_iters(confidence, 0.45, A.max_iters), 3), FmLmeds{n});
+        const bool found = s.minmed < DBL_MAX;
+        if (found) {
+            const double sigma = fmax(2.5 * 1.4826 * (1 + 5. / (n - 7)) * sqrt(s.minmed), 0.001);
+            t = (float)(sigma * sigma);
+        }
+        good = __syncthreads_count(found && tid < n && fm_error(s_pts[tid], s.best) <= t);
+        ok = found && good >= 7; iters = s.done;
+    } else {
+        t = (float)(thresh * thresh);
+        fm_sample_rounds(s, s_pts, n, max(A.max_iters, 1), FmRansac{n, t, confidence});
+        ok = s.maxgood > 0; good = s.maxgood; iters = s.done;
+    }
+    const int status = no_prev ? 3 : n < 7 ? 1 : ok ? 0 : 2;
+    if (tid < 9) A.F[(int64_t)f * 9 + tid] = ok ? s.best[tid] : __longlong_as_double(0x7ff8000000000000LL);
+    if (tid == 0 && A.info) { int32_t* inf = A.info + (int64_t)f * 4; inf[0] = n; inf[1] = good; inf[2] = iters; inf[3] = status; }
+    if (A.mask)             // the mask over every pair of the frame (positions >= n are cleared)
+        for (int i = tid; i < n_all; i += kFmThreads)
+            A.mask[(int64_t)f * A.cap + i] = i < n && (mask_all || (ok && fm_error(s_pts[i], s.best) <= t)) ? 1 : 0;
+}
+
+int fm_launch(const FmArgs& a, cudaStream_t st) {
+    const size_t smem = (size_t)a.cap * sizeof(float4);
+    if (smem > 200 * 1024) { set_error("fundamental: %d pairs per frame do not fit shared memory", a.cap); return SGS_ERR_UNSUPPORTED; }
     if (smem > 40 * 1024)      // per device and cheap: set whenever the default 48 KB would not do
         SGS_CUDA_TRY(cudaFuncSetAttribute(fm_ransac_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    fm_ransac_kernel<<<nframes, kFmThreads, smem, st>>>(d_kps, d_cur, d_prev, d_counts, cap, d_boxes, d_nboxes, d_have_dyn, max_boxes, d_prev_index,
-                                                        d_no_prev, thresh, confidence, max_iters, d_F, d_info, d_mask);
+    fm_ransac_kernel<<<a.nframes, kFmThreads, smem, st>>>(a);
     SGS_CUDA_TRY(cudaGetLastError());
     return SGS_OK;
 }
@@ -496,8 +455,11 @@ SGS_API int sgs_fundamental_batch_device(const sgs_keypoint* d_kps, const float*
                                          const int32_t* d_prev_index, double ransac_thresh, double confidence, int max_iters, double* d_F, int32_t* d_info, void* stream) {
     if (!d_kps || !d_prev_xy || !d_counts || !d_F || cap < 1 || nframes < 1) { set_error("sgs_fundamental_batch_device: bad argument"); return SGS_ERR_INVALID; }
     if (d_prev_have_dyn && (!d_prev_boxes || !d_prev_nboxes || max_boxes < 1)) { set_error("sgs_fundamental_batch_device: boxes missing"); return SGS_ERR_INVALID; }
-    return fm_launch(d_kps, nullptr, reinterpret_cast<const float2*>(d_prev_xy), d_counts, cap, nframes, d_prev_boxes, d_prev_nboxes, d_prev_have_dyn,
-                     max_boxes, d_prev_index, nullptr, ransac_thresh, confidence, max_iters, d_F, d_info, nullptr, (cudaStream_t)stream);
+    FmArgs a{};
+    a.kps = d_kps; a.prev = reinterpret_cast<const float2*>(d_prev_xy); a.counts = d_counts; a.cap = cap; a.nframes = nframes;
+    a.prev_boxes = d_prev_boxes; a.prev_nboxes = d_prev_nboxes; a.prev_have_dyn = d_prev_have_dyn; a.max_boxes = max_boxes; a.prev_index = d_prev_index;
+    a.thresh = ransac_thresh; a.confidence = confidence; a.max_iters = max_iters; a.F = d_F; a.info = d_info;
+    return fm_launch(a, (cudaStream_t)stream);
 }
 
 SGS_API int sgs_fundamental_ransac(const float* pts1_xy, const float* pts2_xy, int n, double ransac_thresh, double confidence, int max_iters,
@@ -511,8 +473,10 @@ SGS_API int sgs_fundamental_ransac(const float* pts1_xy, const float* pts2_xy, i
     HostStage S("sgs_fundamental_ransac");
     S.in(&d_a, pts1_xy, 2 * (size_t)n); S.in(&d_b, pts2_xy, 2 * (size_t)n); S.out(&d_F, 9); S.out(&d_info, 4); S.out(&d_mask, n);
     if (S.commit() != SGS_OK) return SGS_ERR_CUDA;
-    const int rc = fm_launch(nullptr, reinterpret_cast<const float2*>(d_a), reinterpret_cast<const float2*>(d_b), nullptr, n, 1, nullptr, nullptr, nullptr, 0,
-                             nullptr, nullptr, ransac_thresh, confidence, max_iters, d_F, d_info, d_mask, nullptr);
+    FmArgs a{};
+    a.cur = reinterpret_cast<const float2*>(d_a); a.prev = reinterpret_cast<const float2*>(d_b); a.cap = n; a.nframes = 1;
+    a.thresh = ransac_thresh; a.confidence = confidence; a.max_iters = max_iters; a.F = d_F; a.info = d_info; a.mask = d_mask;
+    const int rc = fm_launch(a, nullptr);
     if (rc != SGS_OK) return rc;
     S.to_host(F, d_F, 9);
     if (mask) S.to_host(mask, d_mask, n);

@@ -22,10 +22,20 @@ int lk_track_from_store(sgs_lk* k, const uint8_t* d_cur, int nframes, size_t fra
                         int cap, const uint8_t* d_store, const int32_t* d_row, float* d_prev_xy, cudaStream_t st);
 
 // ---- fundamental.cu
-// sgs_fundamental_batch_device's launch.  d_no_prev (may be NULL): d_no_prev[f] != 0 marks a frame without a previous frame (status 3), in place of
-// d_prev_index[f] == f; the previous boxes and flag are then read from row f.
-int fm_launch(const sgs_keypoint* d_kps, const float2* d_cur, const float2* d_prev, const int32_t* d_counts, int cap, int nframes,
-              const sgs_rect* d_boxes, const int32_t* d_nboxes, const uint8_t* d_have_dyn, int max_boxes, const int32_t* d_prev_index,
-              const uint8_t* d_no_prev, double thresh, double confidence, int max_iters, double* d_F, int32_t* d_info, uint8_t* d_mask, cudaStream_t st);
+// The arguments of fm_launch (device pointers; fill from FmArgs{} so that what is left out is NULL).  Frame f's pairs: current points
+// kps[f * cap + i] (or cur[f * cap + i] when kps is NULL), previous points prev[f * cap + i], i < counts[f] (every frame has cap pairs when
+// counts is NULL).
+struct FmArgs {
+    const sgs_keypoint* kps; const float2* cur; const float2* prev; const int32_t* counts; int cap, nframes;
+    // the previous frames' person boxes [.][max_boxes], their number and the potential-dynamic flag (prev_have_dyn NULL: no pair is filtered)
+    const sgs_rect* prev_boxes; const int32_t* prev_nboxes; const uint8_t* prev_have_dyn; int max_boxes;
+    // At most one of the two.  prev_index[f]: the row holding frame f's previous boxes and flag, == f for a frame without a previous frame.
+    // no_prev[f] != 0: frame f has no previous frame; its previous boxes and flag are in row f.  With neither, every frame has a previous frame, read from row f.
+    const int32_t* prev_index; const uint8_t* no_prev;
+    double thresh, confidence; int max_iters;
+    double* F; int32_t* info; uint8_t* mask;     // [nframes][9], [nframes][4] (may be NULL), [nframes][cap] (may be NULL)
+};
+// sgs_fundamental_batch_device's launch
+int fm_launch(const FmArgs& a, cudaStream_t st);
 
 }  // namespace sgs

@@ -15,6 +15,7 @@
 #include <memory>
 #include <vector>
 
+#include "block_compact.cuh"
 #include "host_stage.cuh"
 #include "internal_launch.cuh"
 #include "sgs_common.h"
@@ -78,39 +79,29 @@ struct sgs_tracker {
 };
 
 namespace sgs {
+constexpr int kCompactThreads = 256;
 // ordered compaction of the per-keypoint side arrays (u_right; after an RGB-D step also mvKeysUn and mvDepth, kun_in / dz_in may be NULL) with the
 // verdicts of the dyn-reject kernel
 __global__ void compact_uright_kernel(const float* __restrict__ ur_in, const uint8_t* __restrict__ keep, const int32_t* __restrict__ n_in,
                                       const int32_t* __restrict__ n_out, int cap, float* __restrict__ ur_out, int32_t* __restrict__ mp,
                                       const sgs_keypoint* __restrict__ kun_in, sgs_keypoint* __restrict__ kun_out, const float* __restrict__ dz_in,
                                       float* __restrict__ dz_out) {
-    __shared__ int s_warp[8];
-    __shared__ int s_carry;
     const int f = blockIdx.x;
     const int n = min(n_in[f], cap);
     const bool restored = n_out[f] == n;   // restore-all (or nothing rejected): identity
     const int64_t base = (int64_t)f * cap;
-    if (threadIdx.x == 0) s_carry = 0;
-    __syncthreads();
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    for (int i0 = 0; i0 < n; i0 += 256) {
+    int kept = 0;
+    for (int i0 = 0; i0 < n; i0 += kCompactThreads) {
         const int i = i0 + threadIdx.x;
         const bool ok = i < n && (restored || keep[base + i]);
-        const unsigned m = __ballot_sync(0xffffffffu, ok);
-        if (lane == 0) s_warp[warp] = __popc(m);
-        __syncthreads();
-        int off = s_carry;
-        for (int w = 0; w < warp; ++w) off += s_warp[w];
-        if (ok) {
-            const int64_t o = base + off + __popc(m & ((1u << lane) - 1));
+        const int slot = block_ordered_slot<kCompactThreads>(ok, kept);
+        if (slot >= 0) {
+            const int64_t o = base + slot;
             ur_out[o] = ur_in[base + i];
             if (kun_in) { kun_out[o] = kun_in[base + i]; dz_out[o] = dz_in[base + i]; }
         }
-        __syncthreads();
-        if (threadIdx.x == 0) { int t = 0; for (int w = 0; w < 8; ++w) t += s_warp[w]; s_carry += t; }
-        __syncthreads();
     }
-    for (int i = threadIdx.x; i < cap; i += 256) mp[base + i] = -1;   // Tracking.cc:916 clears mvpMapPoints before the search
+    for (int i = threadIdx.x; i < cap; i += kCompactThreads) mp[base + i] = -1;   // Tracking.cc:916 clears mvpMapPoints before the search
 }
 // ---- glue of sgs_tracker_pose_chain_device (Tracking::TrackWithMotionModel / TrackLocalMap between the matcher and optimiser calls) ----------
 // src/Tracking.cc:927-931: fewer than 20 matches -> clear the frame's matches and search again with 2 th
@@ -385,7 +376,7 @@ int enqueue_track(sgs_tracker* t, int nframes, const float* prev_xy, const float
     int rc = sgs_dynreject_batch_device(ex.kps, ex.desc, ex.n, ex.cap, nframes, prev_xy, F, boxes, nboxes, t->max_boxes, have_dyn,
                                         t->nfeatures, t->d_kps2, t->d_desc2, t->d_cnt2, t->d_keep, st);
     if (rc != SGS_OK) return rc;
-    compact_uright_kernel<<<nframes, 256, 0, st>>>(u_right, t->d_keep, ex.n, t->d_cnt2, ex.cap, t->d_uright2, t->d_mp, kun, t->d_kpsun2, dz, t->d_dz2);
+    compact_uright_kernel<<<nframes, kCompactThreads, 0, st>>>(u_right, t->d_keep, ex.n, t->d_cnt2, ex.cap, t->d_uright2, t->d_mp, kun, t->d_kpsun2, dz, t->d_dz2);
     t->keys_un = kun ? t->d_kpsun2 : t->d_kps2;
     SGS_CUDA_TRY(cudaMemsetAsync(t->d_ncand, 0, (size_t)nframes * 8, st));
     const sgs_lastframe_batch a = lastframe_search(t, last, th, mono, check_orientation);
@@ -508,8 +499,11 @@ int enqueue_step(sgs_tracker* t, sgs_detector* det, const StepFrames& fr, int nf
     if (streams) {
         // the parameters of sgs_tracker_fundamental_device; the previous boxes and flag are the gathered ones.  Then LK has read the slots' levels, and
         // the frames become their slots' state.
-        rc = fm_launch(ex.kps, nullptr, reinterpret_cast<const float2*>(t->d_prev), ex.n, ex.cap, nframes, S.pre_boxes, S.pre_nboxes, S.pre_have, t->max_boxes,
-                       nullptr, S.first, 1.0, 0.99, 1000, t->d_Fgpu, t->d_finfo, nullptr, st);
+        FmArgs a{};
+        a.kps = ex.kps; a.prev = reinterpret_cast<const float2*>(t->d_prev); a.counts = ex.n; a.cap = ex.cap; a.nframes = nframes;
+        a.prev_boxes = S.pre_boxes; a.prev_nboxes = S.pre_nboxes; a.prev_have_dyn = S.pre_have; a.max_boxes = t->max_boxes; a.no_prev = S.first;
+        a.thresh = 1.0; a.confidence = 0.99; a.max_iters = 1000; a.F = t->d_Fgpu; a.info = t->d_finfo;
+        rc = fm_launch(a, st);
         if (rc != SGS_OK) return rc;
         const LkPyramid P = lk_pyramid(t->lk.get());
         const int gx = (int)std::max<int64_t>(1, (P.frame_bytes[0] / 16 + 2047) / 2048);
