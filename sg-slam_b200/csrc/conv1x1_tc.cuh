@@ -3,8 +3,9 @@
 //     out[p][co] = tail(bias[co] + sum_ci X[p][ci] * W[co][ci])          X: NHWC activations [pixels of all frames][Cin], W: [Cout][Cin]
 //   * operands reach shared memory by TMA (cp.async.bulk.tensor.2d, 128-byte swizzle, out-of-range rows / channels zero-filled) through a ring of
 //     stages guarded by mbarriers; the weight tile of the CTA stays resident in shared memory when it fits,
-//   * the contraction is wgmma.mma_async (tf32, m64n32k8): each of the two consumer warpgroups owns 64 pixels of the 128-pixel tile and the whole
-//     output-channel tile, the activations enter as register fragments read from the swizzled stage, the weights as shared-memory descriptors,
+//   * the contraction is wgmma.mma_async (tf32, m64nNk8 with N = the tile's output channels): each of the two consumer warpgroups owns 64 pixels of
+//     the 128-pixel tile and the whole output-channel tile, the activations enter as register fragments read from the swizzled stage, the weights
+//     as shared-memory descriptors,
 //   * FP32-grade accuracy: every operand is x = hi + lo with hi, lo exactly representable in TF32 (round-to-nearest split); each k-step issues
 //     lo*hi + hi*lo + hi*hi (the dropped lo*lo term is < 2^-22 relative).  Weights are split once at load time, activations in registers,
 //   * epilogue straight from the accumulator registers: bias -> fused element-wise tail -> NHWC store (each warp store covers whole 32-byte sectors).
@@ -16,6 +17,7 @@
 
 #include <cstdint>
 #include <cstring>
+#include <type_traits>
 #include <vector>
 
 #include "host_stage.cuh"
@@ -26,7 +28,7 @@ namespace tc {
 constexpr int kBM = 128;        // pixels per tile = two wgmma M = 64 warpgroups
 constexpr int kBK = 32;         // floats per k-block = one 128-byte swizzle row (16 = one 64-byte row for layers with at most 16 input channels)
 constexpr int kMaxStages = 8;
-constexpr int kWN = 32;         // output channels per wgmma (m64n32k8)
+constexpr int kWN = 32;         // output-channel granule of a tile (the narrowest wgmma, m64n32k8)
 constexpr int kMaxNT = 256;     // output channels per tile (128 accumulator registers per consumer thread)
 constexpr int kMaxChunks = kMaxNT / kWN;
 constexpr int kThreads = 3 * 128;       // two consumer warpgroups + the producer warpgroup (one thread of it issues the loads)
@@ -58,22 +60,77 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
-// d[64 x 32] += a[64 x 8] (register fragment) * b[32 x 8]^T (K-major tile in shared memory)
-__device__ __forceinline__ void wgmma_tf32_n32(float (&d)[16], const uint32_t (&a)[4], uint64_t bdesc) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, 1, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 "
+// d[64 x N] += a[64 x 8] (register fragment) * b[N x 8]^T (K-major tile in shared memory), N = 32 ... 256 in steps of 32.  d holds N / 2 floats per
+// thread in the wgmma register order: d[4j + 2h + q] is row g + 8h, column 8j + 2t + q of the warp's 16 rows (g = lane / 4, t = lane % 4), so the first
+// 16 floats are the m64n32 accumulator of columns 0-31, the next 16 that of columns 32-63, and so on.
+#define SGS_WGMMA_HEAD(n) "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\twgmma.mma_async.sync.aligned.m64n" #n "k8.f32.tf32.tf32 "
+#define SGS_WGMMA_IN "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc)
+#define SGS_ACC8(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3]), "+f"(d[i + 4]), "+f"(d[i + 5]), "+f"(d[i + 6]), "+f"(d[i + 7])
+template <int N>
+__device__ __forceinline__ void wgmma_tf32(float (&d)[N / 2], const uint32_t (&a)[4], uint64_t bdesc) {
+    static_assert(N % 32 == 0 && N >= 32 && N <= 256, "m64nNk8 with N a multiple of 32 up to 256");
+    if constexpr (N == 32)
+        asm volatile(SGS_WGMMA_HEAD(32)
         "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, {%16, %17, %18, %19}, %20, p, 1, 1;\n\t}"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]),
-          "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
-        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc)
-        : "memory");
+                     : SGS_ACC8(0), SGS_ACC8(8)
+                     : SGS_WGMMA_IN : "memory");
+    else if constexpr (N == 64)
+        asm volatile(SGS_WGMMA_HEAD(64)
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1;\n\t}"
+                     : SGS_ACC8(0), SGS_ACC8(8), SGS_ACC8(16), SGS_ACC8(24)
+                     : SGS_WGMMA_IN : "memory");
+    else if constexpr (N == 96)
+        asm volatile(SGS_WGMMA_HEAD(96)
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31,"
+        " %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47}, {%48, %49, %50, %51}, %52, p, 1, 1;\n\t}"
+                     : SGS_ACC8(0), SGS_ACC8(8), SGS_ACC8(16), SGS_ACC8(24), SGS_ACC8(32), SGS_ACC8(40)
+                     : SGS_WGMMA_IN : "memory");
+    else if constexpr (N == 128)
+        asm volatile(SGS_WGMMA_HEAD(128)
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31,"
+        " %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, {%64, %65, %66, %67}, %68, p, 1, 1;\n\t}"
+                     : SGS_ACC8(0), SGS_ACC8(8), SGS_ACC8(16), SGS_ACC8(24), SGS_ACC8(32), SGS_ACC8(40), SGS_ACC8(48), SGS_ACC8(56)
+                     : SGS_WGMMA_IN : "memory");
+    else if constexpr (N == 160)
+        asm volatile(SGS_WGMMA_HEAD(160)
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31,"
+        " %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63,"
+        " %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79}, {%80, %81, %82, %83}, %84, p, 1, 1;\n\t}"
+                     : SGS_ACC8(0), SGS_ACC8(8), SGS_ACC8(16), SGS_ACC8(24), SGS_ACC8(32), SGS_ACC8(40), SGS_ACC8(48), SGS_ACC8(56), SGS_ACC8(64), SGS_ACC8(72)
+                     : SGS_WGMMA_IN : "memory");
+    else if constexpr (N == 192)
+        asm volatile(SGS_WGMMA_HEAD(192)
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31,"
+        " %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63,"
+        " %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95}, {%96, %97, %98, %99}, %100, p, 1, 1;\n\t}"
+                     : SGS_ACC8(0), SGS_ACC8(8), SGS_ACC8(16), SGS_ACC8(24), SGS_ACC8(32), SGS_ACC8(40), SGS_ACC8(48), SGS_ACC8(56), SGS_ACC8(64), SGS_ACC8(72), SGS_ACC8(80), SGS_ACC8(88)
+                     : SGS_WGMMA_IN : "memory");
+    else if constexpr (N == 224)
+        asm volatile(SGS_WGMMA_HEAD(224)
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31,"
+        " %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63,"
+        " %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95,"
+        " %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111}, {%112, %113, %114, %115}, %116, p, 1, 1;\n\t}"
+                     : SGS_ACC8(0), SGS_ACC8(8), SGS_ACC8(16), SGS_ACC8(24), SGS_ACC8(32), SGS_ACC8(40), SGS_ACC8(48), SGS_ACC8(56), SGS_ACC8(64), SGS_ACC8(72), SGS_ACC8(80), SGS_ACC8(88), SGS_ACC8(96), SGS_ACC8(104)
+                     : SGS_WGMMA_IN : "memory");
+    else if constexpr (N == 256)
+        asm volatile(SGS_WGMMA_HEAD(256)
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31,"
+        " %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63,"
+        " %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95,"
+        " %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, {%128, %129, %130, %131}, %132, p, 1, 1;\n\t}"
+                     : SGS_ACC8(0), SGS_ACC8(8), SGS_ACC8(16), SGS_ACC8(24), SGS_ACC8(32), SGS_ACC8(40), SGS_ACC8(48), SGS_ACC8(56), SGS_ACC8(64), SGS_ACC8(72), SGS_ACC8(80), SGS_ACC8(88), SGS_ACC8(96), SGS_ACC8(104), SGS_ACC8(112), SGS_ACC8(120)
+                     : SGS_WGMMA_IN : "memory");
 }
+#undef SGS_ACC8
+#undef SGS_WGMMA_IN
+#undef SGS_WGMMA_HEAD
 
 // wgmma shared-memory descriptor of a K-major tile whose rows are one swizzle row (ROWB = 128 or 64 bytes) and whose 8-row groups are 8 * ROWB
 // bytes apart: start >> 4 | LBO (unused by swizzled K-major tiles) << 16 | SBO << 32 | layout << 62 (SWIZZLE_128B = 1, SWIZZLE_64B = 2).
-// A k-step inside the swizzle row advances the start address by its byte offset (the tiles are aligned to the swizzle pattern).
+// A k-step inside the swizzle row advances the start address by its byte offset (the tiles are aligned to the swizzle pattern).  The same
+// descriptor serves any N: the wgmma's k extent (8 floats = 32 bytes) stays inside one swizzle row, so LBO is never used, and its N / 8 row groups
+// are read SBO apart -- the NT rows of a weight tile are one such run.
 template <int ROWB>
 __device__ __forceinline__ uint64_t kmajor_desc(uint32_t saddr) {
     static_assert(ROWB == 128 || ROWB == 64, "one swizzle row per tile row");
@@ -111,17 +168,19 @@ struct TcGeom {
 // mbarriers: full[s] (TMA -> consumers), empty[s] (every consumer warp's MMAs on slot s have completed -> producer), bfull (resident weights).
 // EpiFn: struct with  template <int N> __device__ void run(float (&v)[N], int64_t idx0) const   applied to N consecutive channels of one pixel;
 // idx0 = pixel * Cout + channel (the NHWC index of same-shape operand tensors).
-// MAXC: the most 32-channel chunks a tile of this instantiation has (NT <= 32 * MAXC).  Narrow tiles (MAXC = kNarrowChunks) run two CTAs per SM
-// (ctas_per_sm): each CTA's epilogue -- the stores and the fused tail's operand loads -- overlaps the other CTA's MMAs; every thread keeps the
-// at most 80 registers that two 384-thread CTAs leave (no setmaxnreg split).  Wide tiles run one CTA per SM with the 232 / 40 split.
-template <int MAXC>
-constexpr int ctas_per_sm() { return MAXC < kMaxChunks ? 2 : 1; }
-template <class EpiFn, int BKT, int MAXC>
-__global__ void __launch_bounds__(kThreads, ctas_per_sm<MAXC>()) conv1x1_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapBh,
+// NC: the 32-channel chunks of the tile (NT == 32 * NC); each split term of a k-step is one m64n(NT)k8 wgmma over the whole tile.  Narrow tiles
+// (NC = kNarrowChunks) run two CTAs per SM (ctas_per_sm): each CTA's epilogue -- the stores and the fused tail's operand loads -- overlaps the other
+// CTA's MMAs; every thread keeps the at most 80 registers that two 384-thread CTAs leave (no setmaxnreg split).  Wide tiles run one CTA per SM with
+// the 232 / 40 split.
+template <int NC>
+constexpr int ctas_per_sm() { return NC <= kNarrowChunks ? 2 : 1; }
+template <class EpiFn, int BKT, int NC>
+__global__ void __launch_bounds__(kThreads, ctas_per_sm<NC>()) conv1x1_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapBh,
                                                               const __grid_constant__ CUtensorMap mapBl, const float* __restrict__ bias,
                                                               float* __restrict__ out, const TcGeom G, const EpiFn epi) {
-    static_assert(MAXC >= 1 && MAXC <= kMaxChunks, "chunks per tile");
-    constexpr bool kSplitRegs = ctas_per_sm<MAXC>() == 1;
+    static_assert(NC >= 1 && NC <= kMaxChunks, "chunks per tile");
+    constexpr int NT = NC * kWN;
+    constexpr bool kSplitRegs = ctas_per_sm<NC>() == 1;
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     __shared__ __align__(8) uint64_t s_full[kMaxStages], s_empty[kMaxStages], s_bfull;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -179,20 +238,19 @@ __global__ void __launch_bounds__(kThreads, ctas_per_sm<MAXC>()) conv1x1_tc_kern
 
     // ---------------------------------------------------------------------------------------------------- consumers
     // Fragment ownership (wgmma m64nNk8, tf32): warp w of the warpgroup owns rows 16w + g and 16w + g + 8 (g = lane / 4); the A fragment holds
-    // columns t and t + 4 of the k-step (t = lane % 4), the accumulator of a 32-channel chunk the channel pairs 8j + 2t, j = 0..3.
+    // columns t and t + 4 of the k-step (t = lane % 4), the accumulator the channel pairs 8j + 2t, j = 0..NT/8-1 (wgmma_tf32: acc[4j + 2h + q]).
     if constexpr (kSplitRegs) asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory");
     const int wg = warp >> 2, g = lane >> 2, t = lane & 3;
     const int r0 = 64 * wg + 16 * (warp & 3) + g;                            // tile row of fragment rows 0 (and r0 + 8)
-    const int nch = G.NT / kWN;                                              // 32-channel chunks of the tile (uniform, <= MAXC)
-    const int ncol = min(G.NT, G.Cout - n0);                                 // real output channels of this tile (uniform)
+    const int ncol = min(NT, G.Cout - n0);                                   // real output channels of this tile (uniform)
+    // bias of channel n0 + 2t + d at bias_t[d]: the epilogue's loads then differ by constant offsets (one base address, not one per channel pair)
+    const float* bias_t = bias ? bias + n0 + 2 * t : nullptr;
     if (G.b_resident) mbar_wait(smem_addr(&s_bfull), 0);
-    float acc[MAXC][16];
+    float acc[NT / 2];
     uint32_t g_ring = 0;
     for (int it = 0; it < my_tiles; ++it) {
 #pragma unroll
-        for (int c = 0; c < MAXC; ++c)
-#pragma unroll
-            for (int i = 0; i < 16; ++i) acc[c][i] = 0.f;
+        for (int i = 0; i < NT / 2; ++i) acc[i] = 0.f;
         for (int kb = 0; kb < G.KB; ++kb, ++g_ring) {
             const uint32_t s = g_ring % (uint32_t)G.stages, ph = (g_ring / (uint32_t)G.stages) & 1u;
             mbar_wait(smem_addr(&s_full[s]), ph);
@@ -214,16 +272,11 @@ __global__ void __launch_bounds__(kThreads, ctas_per_sm<MAXC>()) conv1x1_tc_kern
             wgmma_fence();
 #pragma unroll
             for (int j = 0; j < KS; ++j) {
-                if (j < ksteps) {
-#pragma unroll
-                    for (int c = 0; c < MAXC; ++c) {
-                        if (c < nch) {
-                            const uint32_t b = bh0 + (uint32_t)(c * kWN * ROWB + j * 32);
-                            wgmma_tf32_n32(acc[c], al[j], kmajor_desc<ROWB>(b));
-                            wgmma_tf32_n32(acc[c], ah[j], kmajor_desc<ROWB>(b + b_bytes));
-                            wgmma_tf32_n32(acc[c], ah[j], kmajor_desc<ROWB>(b));
-                        }
-                    }
+                if (j < ksteps) {                                            // every output element sees lo*hi, hi*lo, hi*hi of each k-step, in that order
+                    const uint32_t b = bh0 + (uint32_t)(j * 32);
+                    wgmma_tf32<NT>(acc, al[j], kmajor_desc<ROWB>(b));
+                    wgmma_tf32<NT>(acc, ah[j], kmajor_desc<ROWB>(b + b_bytes));
+                    wgmma_tf32<NT>(acc, ah[j], kmajor_desc<ROWB>(b));
                 }
             }
             wgmma_commit();
@@ -243,21 +296,21 @@ __global__ void __launch_bounds__(kThreads, ctas_per_sm<MAXC>()) conv1x1_tc_kern
             float* o = out + G.base_off + off + n0;
             const int64_t idx = (int64_t)p * G.Cout + n0;
 #pragma unroll
-            for (int c = 0; c < MAXC; ++c) {
+            for (int c = 0; c < NC; ++c) {
                 if (c * kWN >= ncol) break;
 #pragma unroll
-                for (int j = 0; j < 4; ++j) {
-                    const int col = c * kWN + 8 * j + 2 * t;
+                for (int j = 4 * c; j < 4 * c + 4; ++j) {                      // 8-channel groups of the 32-channel chunk c
+                    const int col = 8 * j + 2 * t;
                     if (col + 1 < ncol && G.vec_ok) {
-                        float v[2] = {__fadd_rn(acc[c][4 * j + 2 * h], bias ? __ldg(bias + n0 + col) : 0.f),
-                                      __fadd_rn(acc[c][4 * j + 2 * h + 1], bias ? __ldg(bias + n0 + col + 1) : 0.f)};
+                        float v[2] = {__fadd_rn(acc[4 * j + 2 * h], bias_t ? __ldg(bias_t + 8 * j) : 0.f),
+                                      __fadd_rn(acc[4 * j + 2 * h + 1], bias_t ? __ldg(bias_t + 8 * j + 1) : 0.f)};
                         epi.template run<2>(v, idx + col);
                         *reinterpret_cast<float2*>(o + col) = make_float2(v[0], v[1]);
                     } else {
 #pragma unroll
                         for (int q = 0; q < 2; ++q) {
                             if (col + q < ncol) {
-                                float one[1] = {__fadd_rn(acc[c][4 * j + 2 * h + q], bias ? __ldg(bias + n0 + col + q) : 0.f)};
+                                float one[1] = {__fadd_rn(acc[4 * j + 2 * h + q], bias_t ? __ldg(bias_t + 8 * j + q) : 0.f)};
                                 epi.template run<1>(one, idx + col + q);
                                 o[col + q] = one[0];
                             }
@@ -407,9 +460,23 @@ inline bool launch_conv1x1_tc_map(const GemmPlan& P, const CUtensorMap& mapA, in
         kern<<<dim3(gx, P.n_tiles), kThreads, P.smem_bytes, st>>>(mapA, P.map_hi, P.map_lo, bias, out, G, epi);
         return true;
     };
-    bool ok;
-    if (narrow) ok = P.BK == 16 ? go(conv1x1_tc_kernel<EpiFn, 16, kNarrowChunks>) : go(conv1x1_tc_kernel<EpiFn, 32, kNarrowChunks>);
-    else ok = P.BK == 16 ? go(conv1x1_tc_kernel<EpiFn, 16, kMaxChunks>) : go(conv1x1_tc_kernel<EpiFn, 32, kMaxChunks>);
+    // one instance per k-block width and tile width: the wgmma's N is a compile-time constant
+    auto by_width = [&](auto bk) -> bool {
+        constexpr int BKT = decltype(bk)::value;
+        switch (P.NT / kWN) {
+        case 1: return go(conv1x1_tc_kernel<EpiFn, BKT, 1>);
+        case 2: return go(conv1x1_tc_kernel<EpiFn, BKT, 2>);
+        case 3: return go(conv1x1_tc_kernel<EpiFn, BKT, 3>);
+        case 4: return go(conv1x1_tc_kernel<EpiFn, BKT, 4>);
+        case 5: return go(conv1x1_tc_kernel<EpiFn, BKT, 5>);
+        case 6: return go(conv1x1_tc_kernel<EpiFn, BKT, 6>);
+        case 7: return go(conv1x1_tc_kernel<EpiFn, BKT, 7>);
+        case 8: return go(conv1x1_tc_kernel<EpiFn, BKT, 8>);
+        }
+        return false;
+    };
+    static_assert(kMaxChunks == 8, "one case per tile width");
+    const bool ok = P.BK == 16 ? by_width(std::integral_constant<int, 16>{}) : by_width(std::integral_constant<int, 32>{});
     if (!ok) return false;
     return cudaGetLastError() == cudaSuccess;
 }
