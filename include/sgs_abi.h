@@ -74,7 +74,14 @@ SGS_API int sgs_device_count(int* n);
 typedef struct sgs_extractor sgs_extractor;
 
 /* ORBextractor::ORBextractor (src/ORBextractor.cc:411-471) + buffer allocation for frames of width x height,
- * up to max_batch frames per call, on CUDA device `device`. */
+ * up to max_batch frames per call, on CUDA device `device`.
+ * Limits (pinned by tests/test_gpu_orb_cases.py):
+ *   - width and height in [1, 4096]; 4097 returns SGS_ERR_INVALID;
+ *   - scale_factor exactly 2.0 returns SGS_ERR_UNSUPPORTED (cv::resize would switch to INTER_AREA);
+ *   - every level must hold at least one 30-px FAST cell in each direction, and must not be portrait (quirk Q2): SGS_ERR_UNSUPPORTED;
+ *   - the quadtree keeps its node arrays in shared memory: nfeatures may be at most about 1393 (the exact limit is
+ *     2 * max(N, 4 * roots) + 4 * roots + 16 <= 2806 nodes for the largest level budget N; 640x480 with one level accepts 1393 and
+ *     refuses 1394 with SGS_ERR_UNSUPPORTED). */
 SGS_API int sgs_extractor_create(const sgs_orb_params* params, int width, int height, int max_batch, int device,
                                  sgs_extractor** out);
 SGS_API void sgs_extractor_destroy(sgs_extractor* ex);
