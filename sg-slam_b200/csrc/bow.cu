@@ -21,6 +21,7 @@
 #include <vector>
 
 #include "host_stage.cuh"
+#include "match_rules.cuh"
 #include "sgs_common.h"
 
 struct sgs_vocabulary {
@@ -34,14 +35,8 @@ struct sgs_vocabulary {
 namespace sgs {
 
 constexpr int kBowThreads = 256;
-constexpr int kBowThLow = 50, kBowHisto = 30;      // TH_LOW, HISTO_LENGTH (src/ORBmatcher.cc:37-39)
 
 struct VocDev { const int32_t* first; const int32_t* count; const int32_t* children; const int32_t* word; const uint8_t* desc; const double* weight; int L; };
-
-__device__ __forceinline__ int popc256v(const uint4& a0, const uint4& a1, const uint4& b0, const uint4& b1) {
-    return __popc(a0.x ^ b0.x) + __popc(a0.y ^ b0.y) + __popc(a0.z ^ b0.z) + __popc(a0.w ^ b0.w) + __popc(a1.x ^ b1.x) + __popc(a1.y ^ b1.y) +
-           __popc(a1.z ^ b1.z) + __popc(a1.w ^ b1.w);
-}
 
 __global__ void __launch_bounds__(256) bow_transform_kernel(const VocDev V, const uint8_t* __restrict__ desc, const int32_t* __restrict__ counts, int cap,
                                                             int levelsup, int32_t* __restrict__ word, double* __restrict__ weight, int32_t* __restrict__ node) {
@@ -63,7 +58,7 @@ __global__ void __launch_bounds__(256) bow_transform_kernel(const VocDev V, cons
             const int c = c0 + lane;
             if (c < nch) {
                 const uint4* cd = reinterpret_cast<const uint4*>(V.desc + 32 * (int64_t)__ldg(V.children + first + c));
-                best = min(best, ((unsigned)popc256v(d0, d1, __ldg(cd), __ldg(cd + 1)) << 12) | (unsigned)c);
+                best = min(best, ((unsigned)descriptor_distance(d0, d1, __ldg(cd), __ldg(cd + 1)) << 12) | (unsigned)c);
             }
         }
         best = __reduce_min_sync(0xffffffffu, best);
@@ -109,13 +104,13 @@ __global__ void __launch_bounds__(kBowThreads) bow_search_kernel(const BowArgs A
     int32_t* run_start = reinterpret_cast<int32_t*>(fkey + A.f_pow2);   // [kf_pow2 + 1]
     int32_t* events = run_start + A.kf_pow2 + 1;                    // [max(kf_cap, f_cap)] (bin << 16 | index in the result array)
     uint8_t* taken = reinterpret_cast<uint8_t*>(events + max(A.kf_cap, A.f_cap));  // [f_cap]
-    __shared__ int hist[kBowHisto];
+    __shared__ int hist[kHistoLen];
     __shared__ int s_nk, s_nf, s_nruns, s_nevent, s_nmatch;
     const int f = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int nk_all = min(A.kf_n[f], A.kf_cap), nf_all = min(A.f_n[f], A.f_cap);
     const int64_t ko = (int64_t)f * A.kf_cap, fo = (int64_t)f * A.f_cap;
     if (tid == 0) { s_nk = 0; s_nf = 0; s_nruns = 0; s_nevent = 0; s_nmatch = 0; }
-    if (tid < kBowHisto) hist[tid] = 0;
+    if (tid < kHistoLen) hist[tid] = 0;
     for (int i = tid; i < A.kf_pow2; i += blockDim.x) {
         uint64_t key = ~0ull;
         if (i < nk_all && A.kf_weight[ko + i] > 0 && A.kf_valid[ko + i] && !(A.pair_mode == 2 && A.only_stereo && !A.kf_stereo[ko + i])) key = ((uint64_t)(uint32_t)A.kf_node[ko + i] << 32) | (uint32_t)i;      // invalid map points never act
@@ -177,8 +172,8 @@ __global__ void __launch_bounds__(kBowThreads) bow_search_kernel(const BowArgs A
                 for (int p = b0 + lane; p < b1; p += 32) {
                     const int realF = (int)(uint32_t)fkey[p];
                     if (taken[realF]) continue;
-                    const int dist = popc256v(k0, k1, __ldg(fdesc + 2 * realF), __ldg(fdesc + 2 * realF + 1));
-                    if (dist > kBowThLow) continue;
+                    const int dist = descriptor_distance(k0, k1, __ldg(fdesc + 2 * realF), __ldg(fdesc + 2 * realF + 1));
+                    if (dist > kThLow) continue;
                     const float x2 = A.f_xy[2 * (fo + realF)], y2 = A.f_xy[2 * (fo + realF) + 1];
                     const int oc = A.f_octave[fo + realF];
                     if (!st1 && !A.f_stereo[fo + realF]) {
@@ -198,7 +193,7 @@ __global__ void __launch_bounds__(kBowThreads) bow_search_kernel(const BowArgs A
             for (int p = b0 + lane; p < b1; p += 32) {
                 const int realF = (int)(uint32_t)fkey[p];
                 if (taken[realF]) continue;                          // :214
-                const int dist = popc256v(k0, k1, __ldg(fdesc + 2 * realF), __ldg(fdesc + 2 * realF + 1));
+                const int dist = descriptor_distance(k0, k1, __ldg(fdesc + 2 * realF), __ldg(fdesc + 2 * realF + 1));
                 const unsigned key = ((unsigned)dist << 16) | (unsigned)(p - b0);
                 if (key < key1) { d2 = min(d2, (int)(key1 >> 16)); key1 = key; }
                 else d2 = min(d2, dist);
@@ -207,7 +202,7 @@ __global__ void __launch_bounds__(kBowThreads) bow_search_kernel(const BowArgs A
             const int c2 = key1 == K1 ? d2 : min((int)(key1 >> 16), 256);
             const int best2 = __reduce_min_sync(0xffffffffu, c2 > 256 ? 256 : c2);
             const int best1 = K1 == 0xffffffffu ? 256 : (int)(K1 >> 16);
-            accept = (A.pair_mode ? best1 < kBowThLow : best1 <= kBowThLow) && (float)best1 < __fmul_rn(A.nnratio, (float)best2);        // :237-240 / :599-601
+            accept = (A.pair_mode ? best1 < kThLow : best1 <= kThLow) && (float)best1 < __fmul_rn(A.nnratio, (float)best2);        // :237-240 / :599-601
             }
             if (accept) {
                 const int realF = (int)(uint32_t)fkey[b0 + (int)(K1 & 0xffffu)];
@@ -216,10 +211,7 @@ __global__ void __launch_bounds__(kBowThreads) bow_search_kernel(const BowArgs A
                     const int slot = A.pair_mode ? realK : realF;
                     A.match_f[oo + slot] = A.pair_mode ? realF : realK;
                     if (A.check_ori) {
-                        float rot = __fsub_rn(A.kf_angle[ko + realK], A.f_angle[fo + realF]);
-                        if (rot < 0.f) rot = __fadd_rn(rot, 360.f);
-                        int bin = (int)roundf(__fmul_rn(rot, (float)kBowHisto / 360.0f));
-                        if (bin == kBowHisto) bin = 0;
+                        const int bin = rotation_bin(A.kf_angle[ko + realK], A.f_angle[fo + realF]);
                         atomicAdd(&hist[bin], 1);
                         events[atomicAdd(&s_nevent, 1)] = (bin << 16) | slot;
                     }
@@ -231,27 +223,8 @@ __global__ void __launch_bounds__(kBowThreads) bow_search_kernel(const BowArgs A
     }
     if (lane == 0 && nmatch) atomicAdd(&s_nmatch, nmatch);
     __syncthreads();
-    if (A.check_ori) {
-        // ComputeThreeMaxima (src/ORBmatcher.cc:1603-1645) on the bin counts, then drop the matches outside the three main bins
-        __shared__ int s_i1, s_i2, s_i3;
-        if (tid == 0) {
-            int max1 = 0, max2 = 0, max3 = 0, i1 = -1, i2 = -1, i3 = -1;
-            for (int i = 0; i < kBowHisto; ++i) {
-                const int s = hist[i];
-                if (s > max1) { max3 = max2; max2 = max1; max1 = s; i3 = i2; i2 = i1; i1 = i; }
-                else if (s > max2) { max3 = max2; max2 = s; i3 = i2; i2 = i; }
-                else if (s > max3) { max3 = s; i3 = i; }
-            }
-            if ((float)max2 < __fmul_rn(0.1f, (float)max1)) { i2 = -1; i3 = -1; }
-            else if ((float)max3 < __fmul_rn(0.1f, (float)max1)) i3 = -1;
-            s_i1 = i1; s_i2 = i2; s_i3 = i3;
-        }
-        __syncthreads();
-        int removed = 0;
-        for (int e = tid; e < s_nevent; e += blockDim.x) {
-            const int bin = events[e] >> 16, j = events[e] & 0xffff;
-            if (bin != s_i1 && bin != s_i2 && bin != s_i3) { A.match_f[oo + j] = -1; ++removed; }
-        }
+    if (A.check_ori) {                                              // :270-288 / :636-654
+        const int removed = drop_outside_main_bins(hist, events, s_nevent, A.match_f + oo);
         if (removed) atomicSub(&s_nmatch, removed);
         __syncthreads();
     }

@@ -9,8 +9,8 @@
 #include <cuda_runtime.h>
 
 #include "host_stage.cuh"
+#include "match_rules.cuh"
 #include "sgs_common.h"
-#include "sgs_logf.h"
 
 namespace sgs {
 
@@ -82,11 +82,10 @@ __global__ void __launch_bounds__(256) frustum_kernel(const sgs_frustum_batch A,
         const float Ox = (float)(((double)(-R0) * t0 + (double)(-R3) * t1) + (double)(-R6) * t2);
         const float Oy = (float)(((double)(-R1) * t0 + (double)(-R4) * t1) + (double)(-R7) * t2);
         const float Oz = (float)(((double)(-R2) * t0 + (double)(-R5) * t1) + (double)(-R8) * t2);
-        const float X = A.mp_xyz[3 * o], Y = A.mp_xyz[3 * o + 1], Z = A.mp_xyz[3 * o + 2];
-        // mRcw * P + mtcw: OpenCV's small-matrix gemm path (float products summed in float, then (float)((double)sum + (double)c))
-        const float PcX = (float)((double)__fadd_rn(__fadd_rn(__fmul_rn(R0, X), __fmul_rn(R1, Y)), __fmul_rn(R2, Z)) + (double)t0);
-        const float PcY = (float)((double)__fadd_rn(__fadd_rn(__fmul_rn(R3, X), __fmul_rn(R4, Y)), __fmul_rn(R5, Z)) + (double)t1);
-        const float PcZ = (float)((double)__fadd_rn(__fadd_rn(__fmul_rn(R6, X), __fmul_rn(R7, Y)), __fmul_rn(R8, Z)) + (double)t2);
+        const float* P = A.mp_xyz + 3 * o;
+        const float X = P[0], Y = P[1], Z = P[2];
+        // mRcw * P + mtcw: OpenCV's small-matrix gemm path
+        const float PcX = gemm3_row(R0, R1, R2, P, t0), PcY = gemm3_row(R3, R4, R5, P, t1), PcZ = gemm3_row(R6, R7, R8, P, t2);
         bool ok = !(PcZ < 0.0f);
         const float invz = __fdiv_rn(1.0f, PcZ);
         const float u = __fadd_rn(__fmul_rn(__fmul_rn(A.cam.fx, PcX), invz), A.cam.cx), v = __fadd_rn(__fmul_rn(__fmul_rn(A.cam.fy, PcY), invz), A.cam.cy);
@@ -99,10 +98,7 @@ __global__ void __launch_bounds__(256) frustum_kernel(const sgs_frustum_batch A,
         const float vc = (float)((((double)Px * nx + (double)Py * ny) + (double)Pz * nz) / (double)dist);
         ok = ok && !(vc < A.viewing_cos_limit);
         if (ok) {
-            const float ratio = __fdiv_rn(A.mp_max_dist[o], dist);
-            int ns = (int)ceilf(__fdiv_rn(glibc_logf(ratio), log_sf));          // MapPoint.cc:402-418, libm logf restated (sgs_logf.h)
-            ns = ns < 0 ? 0 : (ns >= nlevels ? nlevels - 1 : ns);
-            in = 1; pu = u; pv = v; pxr = __fsub_rn(u, __fmul_rn(A.cam.bf, invz)); lvl = ns; vcos = vc;
+            in = 1; pu = u; pv = v; pxr = __fsub_rn(u, __fmul_rn(A.cam.bf, invz)); lvl = predict_scale(A.mp_max_dist[o], dist, log_sf, nlevels); vcos = vc;
         }
     }
     A.mp_inview[o] = in; A.proj_x[o] = pu; A.proj_y[o] = pv; A.proj_xr[o] = pxr; A.level[o] = lvl; A.view_cos[o] = vcos;

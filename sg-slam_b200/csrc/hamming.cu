@@ -10,17 +10,13 @@
 #include <vector>
 
 #include "host_stage.cuh"
+#include "match_rules.cuh"
 #include "sgs_common.h"
 
 namespace sgs {
 
 constexpr int kBfThreads = 128;
 constexpr int kBfTile = 256;  // train descriptors per shared-memory tile (8 KB)
-
-__device__ __forceinline__ int hamming256(const uint4& a0, const uint4& a1, const uint4& b0, const uint4& b1) {
-    return __popc(a0.x ^ b0.x) + __popc(a0.y ^ b0.y) + __popc(a0.z ^ b0.z) + __popc(a0.w ^ b0.w) +
-           __popc(a1.x ^ b1.x) + __popc(a1.y ^ b1.y) + __popc(a1.z ^ b1.z) + __popc(a1.w ^ b1.w);
-}
 
 __global__ void __launch_bounds__(kBfThreads) hamming_bf_kernel(const uint4* __restrict__ query, int nq, const uint4* __restrict__ train, int nt,
                                                                 int chunk, int32_t* __restrict__ p_idx, int32_t* __restrict__ p_best,
@@ -39,7 +35,7 @@ __global__ void __launch_bounds__(kBfThreads) hamming_bf_kernel(const uint4* __r
         __syncthreads();
 #pragma unroll 4
         for (int j = 0; j < cnt; ++j) {
-            const int d = hamming256(a0, a1, tile[2 * j], tile[2 * j + 1]);
+            const int d = descriptor_distance(a0, a1, tile[2 * j], tile[2 * j + 1]);
             if (d < best) { second = best; best = d; idx = t0 + j; }
             else if (d < second) second = d;
         }
@@ -68,7 +64,7 @@ __global__ void hamming_bf_merge_kernel(int nq, int nsplit, const int32_t* __res
 __global__ void hamming_pairs_kernel(const uint4* __restrict__ a, const uint4* __restrict__ b, int n, int32_t* __restrict__ out) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    out[i] = hamming256(__ldg(&a[2 * i]), __ldg(&a[2 * i + 1]), __ldg(&b[2 * i]), __ldg(&b[2 * i + 1]));
+    out[i] = descriptor_distance(__ldg(&a[2 * i]), __ldg(&a[2 * i + 1]), __ldg(&b[2 * i]), __ldg(&b[2 * i + 1]));
 }
 
 // scratch: 3 * nsplit * nq int32.  Returns the split count through *nsplit_out when scratch == nullptr (sizing query).
@@ -175,8 +171,7 @@ __global__ void __launch_bounds__(256) distinctive_kernel(const uint8_t* __restr
         int dist[64];
         for (int j = 0; j < n; ++j) {
             const uint4 b0 = __ldg(D + 2 * j), b1 = __ldg(D + 2 * j + 1);
-            dist[j] = __popc(a0.x ^ b0.x) + __popc(a0.y ^ b0.y) + __popc(a0.z ^ b0.z) + __popc(a0.w ^ b0.w) + __popc(a1.x ^ b1.x) + __popc(a1.y ^ b1.y) +
-                      __popc(a1.z ^ b1.z) + __popc(a1.w ^ b1.w);
+            dist[j] = descriptor_distance(a0, a1, b0, b1);
         }
         // k-th smallest: the value v with  #(dist < v) <= k < #(dist <= v)
         int median = 0;

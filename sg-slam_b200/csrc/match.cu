@@ -21,14 +21,12 @@
 
 #include "match_dev.cuh"
 #include "sgs_common.h"
-#include "sgs_logf.h"
 
 namespace sgs {
 
 constexpr int kMatchThreads = 256;
 constexpr int kGridCols = 64, kGridRows = 48;         // FRAME_GRID_COLS / ROWS, include/Frame.h:39-40
 constexpr int kGridCells = kGridCols * kGridRows;
-constexpr int kThHigh = 100, kThLow = 50, kHistoLen = 30;   // src/ORBmatcher.cc:37-39
 constexpr uint32_t kNoKey = 0xFFFFFFFFu;
 
 struct FrameSmem {
@@ -39,7 +37,6 @@ struct FrameSmem {
     uint8_t* tent;       // tentative claims of the chunk being resolved (lane + 1, 0 = none)
     int32_t* cell_start; // [kGridCells + 1]
     int32_t* cursor;     // [kGridCells] scatter cursors
-    int n;
 };
 
 __host__ __device__ inline size_t frame_smem_bytes(int cap) {
@@ -60,14 +57,36 @@ __device__ __forceinline__ void carve(uint8_t* base, int cap, FrameSmem& s) {
     s.tent = base;
 }
 
-// Frame::PosInGrid (src/Frame.cc:409-419): round() is half away from zero
-__device__ __forceinline__ int grid_round(float v) { return (int)roundf(v); }
+struct GridScale { float w_inv, h_inv; };
+
+// Frame::mfGridElementWidthInv / mfGridElementHeightInv (src/Frame.cc:183-184)
+__device__ __forceinline__ GridScale grid_scale(const MatchCam& cam) {
+    return {__fdiv_rn((float)kGridCols, __fsub_rn(cam.max_x, cam.min_x)), __fdiv_rn((float)kGridRows, __fsub_rn(cam.max_y, cam.min_y))};
+}
+
+// Frame::PosInGrid (src/Frame.cc:409-419): round() is half away from zero; cell = ix * kGridRows + iy
+__device__ __forceinline__ bool pos_in_grid(const MatchCam& cam, GridScale g, float x, float y, int& cell) {
+    const int px = (int)roundf(__fmul_rn(__fsub_rn(x, cam.min_x), g.w_inv));
+    const int py = (int)roundf(__fmul_rn(__fsub_rn(y, cam.min_y), g.h_inv));
+    cell = px * kGridRows + py;
+    return px >= 0 && px < kGridCols && py >= 0 && py < kGridRows;
+}
+
+// The cells Frame::GetFeaturesInArea (src/Frame.cc:354-407) visits for the window of half-size r around (x, y): columns min_cx..max_cx,
+// rows min_cy..max_cy.  False when the window misses the grid.
+__device__ __forceinline__ bool feature_window(const MatchCam& cam, GridScale g, float x, float y, float r, int& min_cx, int& max_cx, int& min_cy,
+                                               int& max_cy) {
+    min_cx = max(0, (int)floorf(__fmul_rn(__fsub_rn(__fsub_rn(x, cam.min_x), r), g.w_inv)));
+    max_cx = min(kGridCols - 1, (int)ceilf(__fmul_rn(__fadd_rn(__fsub_rn(x, cam.min_x), r), g.w_inv)));
+    min_cy = max(0, (int)floorf(__fmul_rn(__fsub_rn(__fsub_rn(y, cam.min_y), r), g.h_inv)));
+    max_cy = min(kGridRows - 1, (int)ceilf(__fmul_rn(__fadd_rn(__fsub_rn(y, cam.min_y), r), g.h_inv)));
+    return min_cx < kGridCols && max_cx >= 0 && min_cy < kGridRows && max_cy >= 0;
+}
 
 // counting sort by cell; entries of a cell end up in ascending keypoint index (== push_back order of AssignFeaturesToGrid)
 __device__ void build_frame_grid(const MatchCam& cam, const sgs_keypoint* __restrict__ kps, const float* __restrict__ uright, int n, FrameSmem& s) {
     __shared__ int s_scan[kMatchThreads];
-    const float w_inv = __fdiv_rn((float)kGridCols, __fsub_rn(cam.max_x, cam.min_x));   // Frame.cc:183-184
-    const float h_inv = __fdiv_rn((float)kGridRows, __fsub_rn(cam.max_y, cam.min_y));
+    const GridScale g = grid_scale(cam);
     const int tid = threadIdx.x;
     for (int c = tid; c <= kGridCells; c += kMatchThreads) s.cell_start[c] = 0;
     __syncthreads();
@@ -75,9 +94,8 @@ __device__ void build_frame_grid(const MatchCam& cam, const sgs_keypoint* __rest
     for (int i = tid; i < n; i += kMatchThreads) {
         const sgs_keypoint kp = kps[i];
         s.kx[i] = kp.x; s.ky[i] = kp.y; s.oct[i] = (uint8_t)kp.octave; s.ur[i] = uright ? uright[i] : -1.f;
-        const int px = grid_round(__fmul_rn(__fsub_rn(kp.x, cam.min_x), w_inv));
-        const int py = grid_round(__fmul_rn(__fsub_rn(kp.y, cam.min_y), h_inv));
-        if (px >= 0 && px < kGridCols && py >= 0 && py < kGridRows) atomicAdd(&s.cell_start[px * kGridRows + py + 1], 1);
+        int cell;
+        if (pos_in_grid(cam, g, kp.x, kp.y, cell)) atomicAdd(&s.cell_start[cell + 1], 1);
     }
     __syncthreads();
     // inclusive scan of cell_start[1..kGridCells] (12 cells per thread + block scan of the partial sums)
@@ -103,9 +121,8 @@ __device__ void build_frame_grid(const MatchCam& cam, const sgs_keypoint* __rest
     __syncthreads();
     // scatter (unordered inside a cell), then order each cell's few entries by keypoint index
     for (int i = tid; i < n; i += kMatchThreads) {
-        const int px = grid_round(__fmul_rn(__fsub_rn(s.kx[i], cam.min_x), w_inv));
-        const int py = grid_round(__fmul_rn(__fsub_rn(s.ky[i], cam.min_y), h_inv));
-        if (px >= 0 && px < kGridCols && py >= 0 && py < kGridRows) s.order[atomicAdd(&s.cursor[px * kGridRows + py], 1)] = (uint16_t)i;
+        int cell;
+        if (pos_in_grid(cam, g, s.kx[i], s.ky[i], cell)) s.order[atomicAdd(&s.cursor[cell], 1)] = (uint16_t)i;
     }
     __syncthreads();
     for (int c = tid; c < kGridCells; c += kMatchThreads) {
@@ -137,11 +154,6 @@ __device__ __forceinline__ void topk_insert(TopK& t, uint32_t k) {   // insertio
     }
 }
 
-__device__ __forceinline__ int popc256(const uint4& a0, const uint4& a1, const uint4& b0, const uint4& b1) {
-    return __popc(a0.x ^ b0.x) + __popc(a0.y ^ b0.y) + __popc(a0.z ^ b0.z) + __popc(a0.w ^ b0.w) +
-           __popc(a1.x ^ b1.x) + __popc(a1.y ^ b1.y) + __popc(a1.z ^ b1.z) + __popc(a1.w ^ b1.w);
-}
-
 // Frame::GetFeaturesInArea + the candidate loop shared by both matchers.  A group of `gsize` lanes (1 or kGroup) shares one
 // window: lane `gl` of the group takes the entries j = beg+gl, beg+gl+gsize, ... of every cell column; the caller min-reduces
 // the (dist, position) keys across the group, which gives exactly the sequential loop's best / second best.
@@ -152,16 +164,8 @@ __device__ TopK scan_window(const MatchCam& cam, const FrameSmem& s, const uint4
                             int min_level, int max_level, const uint4& d0, const uint4& d1, bool use_claims, float ur_pred, float ur_tol,
                             int* ncand, int gl = 0, int gsize = 1) {
     TopK t; topk_init(t);
-    const float w_inv = __fdiv_rn((float)kGridCols, __fsub_rn(cam.max_x, cam.min_x));
-    const float h_inv = __fdiv_rn((float)kGridRows, __fsub_rn(cam.max_y, cam.min_y));
-    const int min_cx = max(0, (int)floorf(__fmul_rn(__fsub_rn(__fsub_rn(x, cam.min_x), r), w_inv)));
-    if (min_cx >= kGridCols) return t;
-    const int max_cx = min(kGridCols - 1, (int)ceilf(__fmul_rn(__fadd_rn(__fsub_rn(x, cam.min_x), r), w_inv)));
-    if (max_cx < 0) return t;
-    const int min_cy = max(0, (int)floorf(__fmul_rn(__fsub_rn(__fsub_rn(y, cam.min_y), r), h_inv)));
-    if (min_cy >= kGridRows) return t;
-    const int max_cy = min(kGridRows - 1, (int)ceilf(__fmul_rn(__fadd_rn(__fsub_rn(y, cam.min_y), r), h_inv)));
-    if (max_cy < 0) return t;
+    int min_cx, max_cx, min_cy, max_cy;
+    if (!feature_window(cam, grid_scale(cam), x, y, r, min_cx, max_cx, min_cy, max_cy)) return t;
     const bool check_levels = (min_level > 0) || (max_level >= 0);
     int cnt = 0;
     for (int ix = min_cx; ix <= max_cx; ++ix) {
@@ -183,7 +187,7 @@ __device__ TopK scan_window(const MatchCam& cam, const FrameSmem& s, const uint4
                 const float er = fabsf(__fsub_rn(ur_pred, ur));
                 if (er > ur_tol) continue;
             }
-            const uint32_t k = ((uint32_t)popc256(d0, d1, __ldg(&cur_desc[2 * idx]), __ldg(&cur_desc[2 * idx + 1])) << 16) | (uint32_t)j;
+            const uint32_t k = ((uint32_t)descriptor_distance(d0, d1, __ldg(&cur_desc[2 * idx]), __ldg(&cur_desc[2 * idx + 1])) << 16) | (uint32_t)j;
             topk_insert(t, k);
             ++t.ngated;
         }
@@ -205,19 +209,6 @@ __device__ __forceinline__ TopK group_topk(TopK t) {   // merge over the kGroup 
         for (int i = 0; i < kTopK; ++i) topk_insert(t, other[i]);
     }
     return t;
-}
-
-__device__ __forceinline__ void three_maxima(const int* hist, int& i1, int& i2, int& i3) {  // ORBmatcher.cc:1603-1644
-    int m1 = 0, m2 = 0, m3 = 0;
-    i1 = i2 = i3 = -1;
-    for (int i = 0; i < kHistoLen; ++i) {
-        const int sz = hist[i];
-        if (sz > m1) { m3 = m2; m2 = m1; m1 = sz; i3 = i2; i2 = i1; i1 = i; }
-        else if (sz > m2) { m3 = m2; m2 = sz; i3 = i2; i2 = i; }
-        else if (sz > m3) { m3 = sz; i3 = i; }
-    }
-    if ((float)m2 < __fmul_rn(0.1f, (float)m1)) { i2 = -1; i3 = -1; }
-    else if ((float)m3 < __fmul_rn(0.1f, (float)m1)) { i3 = -1; }
 }
 
 // First two candidates of a point's list whose keypoints are not claimed (claims only ever remove candidates, so this is what
@@ -317,6 +308,14 @@ __device__ int resolve_chunk(FrameSmem& s, Policy& pol, bool have_point, const u
     return accepted;
 }
 
+// end of both projection matchers: the frame's |vIndices| total (summed over the block) and its match count
+__device__ __forceinline__ void write_totals(int ncand, int nmatch, unsigned long long* ncand_out, int32_t* nmatches_out) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) ncand += __shfl_xor_sync(0xffffffffu, ncand, o);
+    if ((threadIdx.x & 31) == 0 && ncand) atomicAdd(ncand_out, (unsigned long long)ncand);
+    if (threadIdx.x == 0) *nmatches_out = nmatch;
+}
+
 // ---------------------------------------------------------------------------------------------------------------------
 struct LastPolicy {
     const LastFrameArgs& A; FrameSmem& s; const uint4* cur_desc; const sgs_keypoint* kps; int32_t* cur_mp; int* hist; int* n_event;
@@ -332,10 +331,7 @@ struct LastPolicy {
     }
     __device__ void record(int target) const {
         if (!A.check_ori) return;
-        float rot = __fsub_rn(A.last_angle[lo + point], kps[target].angle);      // :1438-1443
-        if (rot < 0.f) rot = __fadd_rn(rot, 360.f);
-        int bin = (int)roundf(__fmul_rn(rot, (float)kHistoLen / 360.0f));
-        if (bin == kHistoLen) bin = 0;
+        const int bin = rotation_bin(A.last_angle[lo + point], kps[target].angle);      // :1438-1443
         atomicAdd(&hist[bin], 1);
         A.events[lo + atomicAdd(n_event, 1)] = (bin << 16) | target;
     }
@@ -356,7 +352,6 @@ __global__ void __launch_bounds__(kMatchThreads) match_lastframe_kernel(const __
     const int nlast = min(A.last_n[f], A.last_cap);
     FrameSmem s;
     carve(smem, A.cur_cap, s);
-    s.n = n;
     const sgs_keypoint* kps = A.cur_kps + (int64_t)f * A.cur_cap;
     const uint4* cur_desc = reinterpret_cast<const uint4*>(A.cur_desc + (int64_t)f * A.cur_cap * 32);
     int32_t* cur_mp = A.cur_mp + (int64_t)f * A.cur_cap;
@@ -365,8 +360,7 @@ __global__ void __launch_bounds__(kMatchThreads) match_lastframe_kernel(const __
     if (threadIdx.x == 0) {
         s_nmatch = 0; s_nevent = 0;
         // Rcw, tcw, twc = -Rcw^T tcw, tlc = Rlw twc + tlw (:1342-1351).  cv::gemm on CV_32F: the transposed product takes the general path
-        // (double accumulator, one rounding); a plain 3x3 * 3x1 (+ C) takes OpenCV's small-matrix path: float products summed in float,
-        // left to right, then (float)((double)sum + (double)c).  Pinned against cv2.gemm (tests/golden/make_golden_frustum.py).
+        // (double accumulator, one rounding); the plain product takes the small-matrix path (gemm3_row).
         const float* Tc = A.tcw_cur + 16 * f; const float* Tl = A.kf_mode ? Tc : A.tcw_last + 16 * f;
         float twc[3];
         for (int r = 0; r < 3; ++r) {
@@ -374,8 +368,7 @@ __global__ void __launch_bounds__(kMatchThreads) match_lastframe_kernel(const __
             for (int k = 0; k < 3; ++k) acc = __dadd_rn(acc, __dmul_rn((double)(-Tc[4 * k + r]), (double)Tc[4 * k + 3]));
             twc[r] = (float)acc;
         }
-        const float acc = __fadd_rn(__fadd_rn(__fmul_rn(Tl[8], twc[0]), __fmul_rn(Tl[9], twc[1])), __fmul_rn(Tl[10], twc[2]));
-        const float tlc2 = (float)__dadd_rn((double)acc, (double)Tl[11]);
+        const float tlc2 = gemm3_row(Tl[8], Tl[9], Tl[10], twc, Tl[11]);
         const float mb = __fdiv_rn(A.cam.bf, A.cam.fx);       // Frame.cc:196
         for (int r = 0; r < 3; ++r) { for (int c = 0; c < 3; ++c) s_pose[3 * r + c] = Tc[4 * r + c]; s_pose[9 + r] = Tc[4 * r + 3]; }
         s_pose[12] = (!A.kf_mode && tlc2 > mb && !A.mono) ? 1.f : 0.f;
@@ -403,10 +396,7 @@ __global__ void __launch_bounds__(kMatchThreads) match_lastframe_kernel(const __
             const float* X = A.last_xyz + 3 * (lo + i);
             float xc[3];
 #pragma unroll
-            for (int r = 0; r < 3; ++r) {      // Rcw * x3Dw + tcw: small-matrix gemm path (float accumulation)
-                const float acc = __fadd_rn(__fadd_rn(__fmul_rn(s_pose[3 * r], X[0]), __fmul_rn(s_pose[3 * r + 1], X[1])), __fmul_rn(s_pose[3 * r + 2], X[2]));
-                xc[r] = (float)__dadd_rn((double)acc, (double)s_pose[9 + r]);
-            }
+            for (int r = 0; r < 3; ++r) xc[r] = gemm3_row(s_pose[3 * r], s_pose[3 * r + 1], s_pose[3 * r + 2], X, s_pose[9 + r]);   // Rcw * x3Dw + tcw
             const float invz = (float)__ddiv_rn(1.0, (double)xc[2]);                       // :1369 / :1506
             if (A.kf_mode || !(invz < 0.f)) {
                 const float u = __fadd_rn(__fmul_rn(__fmul_rn(A.cam.fx, xc[0]), invz), A.cam.cx);
@@ -419,8 +409,7 @@ __global__ void __launch_bounds__(kMatchThreads) match_lastframe_kernel(const __
                         const float dist = (float)sqrt(((double)px * px + (double)py * py) + (double)pz * pz);
                         const float maxd = A.kf_max_dist[lo + i];
                         ok = !(dist < __fmul_rn(0.8f, A.kf_min_dist[lo + i]) || dist > __fmul_rn(1.2f, maxd));
-                        oct = (int)ceilf(__fdiv_rn(glibc_logf(__fdiv_rn(maxd, dist)), A.log_sf));
-                        oct = oct < 0 ? 0 : (oct >= A.cam.nlevels ? A.cam.nlevels - 1 : oct);
+                        oct = predict_scale(maxd, dist, A.log_sf, A.cam.nlevels);
                         mn = oct - 1; mx = oct + 1;
                     } else {
                         oct = A.last_octave[lo + i];
@@ -458,26 +447,15 @@ __global__ void __launch_bounds__(kMatchThreads) match_lastframe_kernel(const __
         if (threadIdx.x == 0) s_nmatch = nmatch;
     }
     __syncthreads();
-    if (A.check_ori) {                                             // :1451-1470, order independent
-        int i1, i2, i3;
-        three_maxima(hist, i1, i2, i3);
-        int removed = 0;
-        for (int e = threadIdx.x; e < s_nevent; e += blockDim.x) {
-            const int ev = A.events[lo + e];
-            const int bin = ev >> 16, idx = ev & 0xFFFF;
-            if (bin != i1 && bin != i2 && bin != i3) { cur_mp[idx] = -1; ++removed; }
-        }
+    if (A.check_ori) {                                             // :1451-1470
+        int removed = drop_outside_main_bins(hist, A.events + lo, s_nevent, cur_mp);
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) removed += __shfl_xor_sync(0xffffffffu, removed, o);
         __syncthreads();
         if ((threadIdx.x & 31) == 0 && removed) atomicSub(&s_nmatch, removed);
     }
     __syncthreads();
-    // totals
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) ncand += __shfl_xor_sync(0xffffffffu, ncand, o);
-    if ((threadIdx.x & 31) == 0 && ncand) atomicAdd(&A.ncand[f], (unsigned long long)ncand);
-    if (threadIdx.x == 0) A.nmatches[f] = s_nmatch;
+    write_totals(ncand, s_nmatch, &A.ncand[f], &A.nmatches[f]);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -526,7 +504,6 @@ __global__ void __launch_bounds__(kMatchThreads) match_localmap_kernel(const __g
     const int nmp = min(A.mp_n[f], A.mp_cap);
     FrameSmem s;
     carve(smem, A.cur_cap, s);
-    s.n = n;
     const sgs_keypoint* kps = A.cur_kps + (int64_t)f * A.cur_cap;
     const uint4* cur_desc = reinterpret_cast<const uint4*>(A.cur_desc + (int64_t)f * A.cur_cap * 32);
     int32_t* f_mp = A.f_mp + (int64_t)f * A.cur_cap;
@@ -573,21 +550,7 @@ __global__ void __launch_bounds__(kMatchThreads) match_localmap_kernel(const __g
         if (threadIdx.x == 0) s_nmatch = nmatch;
     }
     __syncthreads();
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) ncand += __shfl_xor_sync(0xffffffffu, ncand, o);
-    if ((threadIdx.x & 31) == 0 && ncand) atomicAdd(&A.ncand[f], (unsigned long long)ncand);
-    if (threadIdx.x == 0) A.nmatches[f] = s_nmatch;
-}
-
-size_t match_smem_bytes(int cap) { return frame_smem_bytes(cap); }
-
-int launch_match_lastframe(const LastFrameArgs& A, int nframes, cudaStream_t st) {
-    const size_t smem = match_smem_bytes(A.cur_cap);
-    if (smem > 200 * 1024 || A.cur_cap > 65535) { set_error("match: cur_cap %d too large for shared memory", A.cur_cap); return SGS_ERR_UNSUPPORTED; }
-    SGS_CUDA_TRY(cudaFuncSetAttribute(match_lastframe_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    match_lastframe_kernel<<<nframes, kMatchThreads, smem, st>>>(A);
-    SGS_CUDA_TRY(cudaGetLastError());
-    return SGS_OK;
+    write_totals(ncand, s_nmatch, &A.ncand[f], &A.nmatches[f]);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -601,14 +564,12 @@ __global__ void __launch_bounds__(kMatchThreads) fuse_search_kernel(const __grid
     carve(smem, A.kf_cap, s);
     const int f = blockIdx.x;
     const int n = min(A.kf_n[f], A.kf_cap), nmp = min(A.mp_n[f], A.mp_cap);
-    s.n = n;
     const sgs_keypoint* kps = A.kf_kps + (int64_t)f * A.kf_cap;
     const uint4* kf_desc = reinterpret_cast<const uint4*>(A.kf_desc + (int64_t)f * A.kf_cap * 32);
     build_frame_grid(A.cam, kps, A.kf_uright + (int64_t)f * A.kf_cap, n, s);
     const float* T = A.tcw + 16 * (int64_t)f; const float* O = A.ow + 3 * (int64_t)f;
     const int64_t lo = (int64_t)f * A.mp_cap;
-    const float w_inv = __fdiv_rn((float)kGridCols, __fsub_rn(A.cam.max_x, A.cam.min_x));
-    const float h_inv = __fdiv_rn((float)kGridRows, __fsub_rn(A.cam.max_y, A.cam.min_y));
+    const GridScale g = grid_scale(A.cam);
     const int gl = threadIdx.x & (kGroup - 1), ngroups = blockDim.x / kGroup;
     // variant 3 (SearchByProjection(KeyFrame*, Scw, vpPoints, vpMatched, th)): the reference visits the points in order and a feature claimed by an
     // earlier point is invisible to later ones.  A wave of ngroups points searches in parallel against the claims made so far; one thread then walks
@@ -628,18 +589,12 @@ __global__ void __launch_bounds__(kMatchThreads) fuse_search_kernel(const __grid
             const float* X = A.mp_xyz + 3 * (lo + i);
             float pc[3];
 #pragma unroll
-            for (int r = 0; r < 3; ++r) {      // Rcw * p3Dw + tcw: small-matrix gemm path (float accumulation)
-                const float acc = __fadd_rn(__fadd_rn(__fmul_rn(T[4 * r], X[0]), __fmul_rn(T[4 * r + 1], X[1])), __fmul_rn(T[4 * r + 2], X[2]));
-                pc[r] = (float)__dadd_rn((double)acc, (double)T[4 * r + 3]);
-            }
+            for (int r = 0; r < 3; ++r) pc[r] = gemm3_row(T[4 * r], T[4 * r + 1], T[4 * r + 2], X, T[4 * r + 3]);   // Rcw * p3Dw + tcw
             if (A.sim3_variant == 2) {          // p3Dc2 = sR21 * p3Dc1 + t21
                 const float* S = A.xform2 + 12 * (int64_t)f;
                 float q[3];
 #pragma unroll
-                for (int r = 0; r < 3; ++r) {
-                    const float acc = __fadd_rn(__fadd_rn(__fmul_rn(S[3 * r], pc[0]), __fmul_rn(S[3 * r + 1], pc[1])), __fmul_rn(S[3 * r + 2], pc[2]));
-                    q[r] = (float)__dadd_rn((double)acc, (double)S[9 + r]);
-                }
+                for (int r = 0; r < 3; ++r) q[r] = gemm3_row(S[3 * r], S[3 * r + 1], S[3 * r + 2], pc, S[9 + r]);
                 pc[0] = q[0]; pc[1] = q[1]; pc[2] = q[2];
             }
             bool ok = !(pc[2] < 0.0f);
@@ -655,14 +610,10 @@ __global__ void __launch_bounds__(kMatchThreads) fuse_search_kernel(const __grid
             const float* N = A.mp_normal + 3 * (lo + i);
             ok = ok && (cam2 || !((((double)px * N[0] + (double)py * N[1]) + (double)pz * N[2]) < 0.5 * (double)dist));
             if (ok) {
-                int lvl = (int)ceilf(__fdiv_rn(glibc_logf(__fdiv_rn(maxd, dist)), A.log_sf));
-                lvl = lvl < 0 ? 0 : (lvl >= A.cam.nlevels ? A.cam.nlevels - 1 : lvl);
+                const int lvl = predict_scale(maxd, dist, A.log_sf, A.cam.nlevels);
                 const float r = __fmul_rn(A.th, A.cam.scale[lvl]);
-                const int min_cx = max(0, (int)floorf(__fmul_rn(__fsub_rn(__fsub_rn(u, A.cam.min_x), r), w_inv)));
-                const int max_cx = min(kGridCols - 1, (int)ceilf(__fmul_rn(__fadd_rn(__fsub_rn(u, A.cam.min_x), r), w_inv)));
-                const int min_cy = max(0, (int)floorf(__fmul_rn(__fsub_rn(__fsub_rn(v, A.cam.min_y), r), h_inv)));
-                const int max_cy = min(kGridRows - 1, (int)ceilf(__fmul_rn(__fadd_rn(__fsub_rn(v, A.cam.min_y), r), h_inv)));
-                if (min_cx < kGridCols && max_cx >= 0 && min_cy < kGridRows && max_cy >= 0) {
+                int min_cx, max_cx, min_cy, max_cy;
+                if (feature_window(A.cam, g, u, v, r, min_cx, max_cx, min_cy, max_cy)) {
                     const uint4* dm = reinterpret_cast<const uint4*>(A.mp_desc + 32 * (lo + i));
                     const uint4 d0 = __ldg(dm), d1 = __ldg(dm + 1);
                     for (int ix = min_cx; ix <= max_cx; ++ix) {
@@ -684,7 +635,7 @@ __global__ void __launch_bounds__(kMatchThreads) fuse_search_kernel(const __grid
                                 const float e2 = __fadd_rn(__fmul_rn(ex, ex), __fmul_rn(ey, ey));
                                 if ((double)__fmul_rn(e2, A.inv_sigma2[o]) > 5.99) continue;
                             }
-                            const uint32_t k = ((uint32_t)popc256(d0, d1, __ldg(&kf_desc[2 * idx]), __ldg(&kf_desc[2 * idx + 1])) << 16) | (uint32_t)j;
+                            const uint32_t k = ((uint32_t)descriptor_distance(d0, d1, __ldg(&kf_desc[2 * idx]), __ldg(&kf_desc[2 * idx + 1])) << 16) | (uint32_t)j;
                             best = min(best, k);
                         }
                     }
@@ -727,15 +678,6 @@ __global__ void __launch_bounds__(kMatchThreads) fuse_search_kernel(const __grid
     }
 }
 
-int launch_fuse_search(const FuseArgs& A, int nframes, cudaStream_t st) {
-    const size_t smem = frame_smem_bytes(A.kf_cap);
-    if (smem > 200 * 1024 || A.kf_cap > 65535) { set_error("fuse: kf_cap %d too large for shared memory", A.kf_cap); return SGS_ERR_UNSUPPORTED; }
-    SGS_CUDA_TRY(cudaFuncSetAttribute(fuse_search_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    fuse_search_kernel<<<nframes, kMatchThreads, smem, st>>>(A);
-    SGS_CUDA_TRY(cudaGetLastError());
-    return SGS_OK;
-}
-
 // ORBmatcher::SearchForInitialization (src/ORBmatcher.cc:407-522), one block per (F1, F2) pair.  The reference loop is order dependent (a feature of
 // F2 remembers the best distance that claimed it, a better later keypoint steals it), so the keypoints of F1 are visited one after the other; the
 // block shares the candidate scan of each: every thread folds its candidates into (best key, second-best distance), the pairs are merged with the
@@ -761,7 +703,6 @@ __global__ void __launch_bounds__(kMatchThreads) search_init_kernel(const __grid
     __shared__ int s_nm;
     const int f = blockIdx.x, tid = threadIdx.x;
     const int n1 = min(A.f1_n[f], A.f1_cap), n2 = min(A.f2_n[f], A.f2_cap);
-    s.n = n2;
     const sgs_keypoint* k1 = A.f1_kps + (int64_t)f * A.f1_cap;
     const sgs_keypoint* k2 = A.f2_kps + (int64_t)f * A.f2_cap;
     const uint4* d1 = reinterpret_cast<const uint4*>(A.f1_desc + (int64_t)f * A.f1_cap * 32);
@@ -774,18 +715,13 @@ __global__ void __launch_bounds__(kMatchThreads) search_init_kernel(const __grid
     if (tid < kHistoLen) hist[tid] = 0;
     if (tid == 0) s_nm = 0;
     __syncthreads();
-    const float w_inv = __fdiv_rn((float)kGridCols, __fsub_rn(A.cam.max_x, A.cam.min_x));
-    const float h_inv = __fdiv_rn((float)kGridRows, __fsub_rn(A.cam.max_y, A.cam.min_y));
+    const GridScale g = grid_scale(A.cam);
     const float r = (float)A.window;
     for (int i1 = 0; i1 < n1; ++i1) {
         if (k1[i1].octave > 0) continue;                                                    // level1 > 0 (:424-426), block-uniform
         const float x = prev[2 * i1], y = prev[2 * i1 + 1];
-        // Frame::GetFeaturesInArea(x, y, windowSize, 0, 0) (src/Frame.cc:354-407)
-        const int min_cx = max(0, (int)floorf(__fmul_rn(__fsub_rn(__fsub_rn(x, A.cam.min_x), r), w_inv)));
-        const int max_cx = min(kGridCols - 1, (int)ceilf(__fmul_rn(__fadd_rn(__fsub_rn(x, A.cam.min_x), r), w_inv)));
-        const int min_cy = max(0, (int)floorf(__fmul_rn(__fsub_rn(__fsub_rn(y, A.cam.min_y), r), h_inv)));
-        const int max_cy = min(kGridRows - 1, (int)ceilf(__fmul_rn(__fadd_rn(__fsub_rn(y, A.cam.min_y), r), h_inv)));
-        if (min_cx >= kGridCols || max_cx < 0 || min_cy >= kGridRows || max_cy < 0) continue;
+        int min_cx, max_cx, min_cy, max_cy;                                                 // GetFeaturesInArea(x, y, windowSize, 0, 0)
+        if (!feature_window(A.cam, g, x, y, r, min_cx, max_cx, min_cy, max_cy)) continue;
         const uint4 a0 = __ldg(&d1[2 * i1]), a1 = __ldg(&d1[2 * i1 + 1]);
         BestTwo t;
         t.best = kNoKey; t.second = 0xFFFFFFFFu;
@@ -795,7 +731,7 @@ __global__ void __launch_bounds__(kMatchThreads) search_init_kernel(const __grid
                 const int idx = s.order[j];
                 if (s.oct[idx] > 0) continue;                                               // maxLevel = 0
                 if (!(fabsf(__fsub_rn(s.kx[idx], x)) < r && fabsf(__fsub_rn(s.ky[idx], y)) < r)) continue;
-                const uint32_t d = (uint32_t)popc256(a0, a1, __ldg(&d2[2 * idx]), __ldg(&d2[2 * idx + 1]));
+                const uint32_t d = (uint32_t)descriptor_distance(a0, a1, __ldg(&d2[2 * idx]), __ldg(&d2[2 * idx + 1]));
                 if (mdist[idx] <= (int)d) continue;                                         // if(vMatchedDistance[i2]<=dist) continue;  (:447)
                 const uint32_t key = (d << 16) | (uint32_t)j;
                 if (key < t.best) { if (t.best != kNoKey) t.second = min(t.second, t.best >> 16); t.best = key; }
@@ -820,10 +756,7 @@ __global__ void __launch_bounds__(kMatchThreads) search_init_kernel(const __grid
                     if (m21[idx2] >= 0) { m12[m21[idx2]] = -1; s_nm = s_nm - 1; }
                     m12[i1] = idx2; m21[idx2] = i1; mdist[idx2] = best_d; s_nm = s_nm + 1;
                     if (A.check_ori) {
-                        float rot = __fsub_rn(k1[i1].angle, k2[idx2].angle);
-                        if (rot < 0.0f) rot = __fadd_rn(rot, 360.0f);
-                        int bin = (int)roundf(__fmul_rn(rot, (float)kHistoLen / 360.0f));
-                        if (bin == kHistoLen) bin = 0;
+                        const int bin = rotation_bin(k1[i1].angle, k2[idx2].angle);
                         hist[bin] = hist[bin] + 1; bin_of[i1] = (int8_t)bin;
                     }
                 }
@@ -848,22 +781,29 @@ __global__ void __launch_bounds__(kMatchThreads) search_init_kernel(const __grid
     if (tid == 0 && A.nmatches) A.nmatches[f] = s_nm;
 }
 
-int launch_search_init(const InitArgs& A, int nframes, cudaStream_t st) {
-    const size_t smem = frame_smem_bytes(A.f2_cap) + (size_t)A.f2_cap * 8 + (size_t)((A.f1_cap + 15) & ~15);
-    if (smem > 200 * 1024 || A.f2_cap > 65535 || A.f1_cap > 65535) { set_error("search for initialisation: capacities %d / %d too large for shared memory", A.f1_cap, A.f2_cap); return SGS_ERR_UNSUPPORTED; }
-    SGS_CUDA_TRY(cudaFuncSetAttribute(search_init_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    search_init_kernel<<<nframes, kMatchThreads, smem, st>>>(A);
+// One block of kMatchThreads per frame.  The frame grid keeps keypoint indices in 16 bits, so no capacity may exceed 65535, and `smem` bytes
+// of dynamic shared memory hold it (plus the kernel's own per-keypoint arrays).
+template <class Args>
+static int launch_per_frame(void (*kernel)(Args), const Args& A, size_t smem, int cap, int nframes, cudaStream_t st) {
+    if (smem > 200 * 1024 || cap > 65535) { set_error("matcher: capacity %d too large for shared memory", cap); return SGS_ERR_UNSUPPORTED; }
+    SGS_CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    kernel<<<nframes, kMatchThreads, smem, st>>>(A);
     SGS_CUDA_TRY(cudaGetLastError());
     return SGS_OK;
 }
 
-int launch_match_localmap(const LocalMapArgs& A, int nframes, cudaStream_t st) {
-    const size_t smem = match_smem_bytes(A.cur_cap);
-    if (smem > 200 * 1024 || A.cur_cap > 65535) { set_error("match: cur_cap %d too large for shared memory", A.cur_cap); return SGS_ERR_UNSUPPORTED; }
-    SGS_CUDA_TRY(cudaFuncSetAttribute(match_localmap_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    match_localmap_kernel<<<nframes, kMatchThreads, smem, st>>>(A);
-    SGS_CUDA_TRY(cudaGetLastError());
-    return SGS_OK;
+int launch_matcher(const LastFrameArgs& A, int nframes, cudaStream_t st) {
+    return launch_per_frame(match_lastframe_kernel, A, frame_smem_bytes(A.cur_cap), A.cur_cap, nframes, st);
+}
+int launch_matcher(const LocalMapArgs& A, int nframes, cudaStream_t st) {
+    return launch_per_frame(match_localmap_kernel, A, frame_smem_bytes(A.cur_cap), A.cur_cap, nframes, st);
+}
+int launch_matcher(const FuseArgs& A, int nframes, cudaStream_t st) {
+    return launch_per_frame(fuse_search_kernel, A, frame_smem_bytes(A.kf_cap), A.kf_cap, nframes, st);
+}
+int launch_matcher(const InitArgs& A, int nframes, cudaStream_t st) {     // + vMatchedDistance, vnMatches21 and the rotation bins of F1
+    const size_t smem = frame_smem_bytes(A.f2_cap) + (size_t)A.f2_cap * 8 + (size_t)((A.f1_cap + 15) & ~15);
+    return launch_per_frame(search_init_kernel, A, smem, max(A.f1_cap, A.f2_cap), nframes, st);
 }
 
 }  // namespace sgs

@@ -22,7 +22,7 @@ struct sgs_matcher {
 
 namespace {
 
-int pow2_at_least(int v) { int p = 1; while (p < v) p <<= 1; return p; }
+using MatcherPtr = std::unique_ptr<sgs_matcher, void (*)(sgs_matcher*)>;     // the scratch handle of a single-frame call
 
 MatchCam to_cam(const sgs_camera& c) {
     MatchCam m;
@@ -39,6 +39,18 @@ sgs_camera view_cam(const sgs_frame_view* v) {
     c.fx = v->fx; c.fy = v->fy; c.cx = v->cx; c.cy = v->cy; c.bf = v->bf; c.nlevels = v->nlevels;
     for (int i = 0; i < v->nlevels && i < kMaxLevels; ++i) c.scale_factors[i] = v->scale_factors[i];
     return c;
+}
+
+// the fields both variants of SearchByProjection(Frame&, ...) take from the matcher and from the current frames of their batch
+template <class Batch>
+LastFrameArgs projection_args(const sgs_matcher* m, const Batch* a) {
+    LastFrameArgs A{};
+    A.cam = to_cam(a->cam);
+    A.cur_kps = a->cur_kps; A.cur_desc = a->cur_desc; A.cur_uright = a->cur_uright; A.cur_n = a->cur_n; A.cur_cap = m->cur_cap;
+    A.last_cap = m->point_cap; A.tcw_cur = a->tcw_cur; A.th = a->th; A.check_ori = a->check_orientation;
+    A.cur_mp = a->cur_mp; A.nmatches = a->nmatches; A.ncand = (unsigned long long*)a->ncand;
+    A.pre = m->d_pre; A.events = m->d_events;
+    return A;
 }
 
 // the frame a projection matcher or the fuse search runs on: keypoints, descriptors, right coordinates and count
@@ -70,18 +82,12 @@ SGS_API void sgs_matcher_destroy(sgs_matcher* m) { delete m; }
 SGS_API int sgs_match_project_lastframe_batch_device(sgs_matcher* m, const sgs_lastframe_batch* a, int nframes, void* stream) {
     if (!m || !a) { set_error("sgs_match_project_lastframe_batch_device: NULL"); return SGS_ERR_INVALID; }
     if (nframes < 1 || nframes > m->max_frames) { set_error("nframes outside [1,max_frames]"); return SGS_ERR_INVALID; }
-    LastFrameArgs A;
-    A.cam = to_cam(a->cam);
-    A.cur_kps = a->cur_kps; A.cur_desc = a->cur_desc; A.cur_uright = a->cur_uright; A.cur_n = a->cur_n;
-    A.cur_cap = m->cur_cap; A.cur_cap_pow2 = pow2_at_least(m->cur_cap);
+    LastFrameArgs A = projection_args(m, a);
     A.last_xyz = a->last_xyz; A.last_desc = a->last_desc; A.last_flags = a->last_flags; A.last_octave = a->last_octave;
-    A.last_angle = a->last_angle; A.last_n = a->last_n; A.last_cap = m->point_cap;
-    A.tcw_cur = a->tcw_cur; A.tcw_last = a->tcw_last; A.th = a->th; A.mono = a->mono; A.check_ori = a->check_orientation;
-    A.cur_mp = a->cur_mp; A.cur_mp_obs_in = a->cur_mp_obs_in; A.nmatches = a->nmatches; A.ncand = (unsigned long long*)a->ncand;
-    A.kf_mode = 0; A.orb_dist = 100; A.log_sf = 0.f; A.kf_min_dist = A.kf_max_dist = nullptr;      // TH_HIGH, src/ORBmatcher.cc:37
-    A.frame_enable = a->frame_enable;
-    A.pre = m->d_pre; A.events = m->d_events;
-    return launch_match_lastframe(A, nframes, (cudaStream_t)stream);
+    A.last_angle = a->last_angle; A.last_n = a->last_n; A.tcw_last = a->tcw_last; A.mono = a->mono;
+    A.cur_mp_obs_in = a->cur_mp_obs_in; A.frame_enable = a->frame_enable;
+    A.kf_mode = 0; A.orb_dist = kThHigh;
+    return launch_matcher(A, nframes, (cudaStream_t)stream);
 }
 
 SGS_API int sgs_fuse_search_batch_device(const sgs_fuse_batch* a, int nframes, void* stream) {
@@ -101,7 +107,7 @@ SGS_API int sgs_fuse_search_batch_device(const sgs_fuse_batch* a, int nframes, v
         set_error("sgs_fuse_search_batch_device: bad variant"); return SGS_ERR_INVALID; }
     A.best_idx = a->best_idx; A.best_dist = a->best_dist;
     A.kf_matched = a->kf_matched; A.nmatches = a->nmatches;
-    return launch_fuse_search(A, nframes, (cudaStream_t)stream);
+    return launch_matcher(A, nframes, (cudaStream_t)stream);
 }
 
 SGS_API int sgs_match_project_keyframe_batch_device(sgs_matcher* m, const sgs_keyframe_batch* a, int nframes, void* stream) {
@@ -110,18 +116,10 @@ SGS_API int sgs_match_project_keyframe_batch_device(sgs_matcher* m, const sgs_ke
     if (!a->cur_kps || !a->cur_desc || !a->cur_n || !a->kf_xyz || !a->kf_desc || !a->kf_valid || !a->kf_angle || !a->kf_min_dist || !a->kf_max_dist ||
         !a->kf_n || !a->tcw_cur || !a->cur_mp || !a->nmatches || !a->ncand || !a->cur_uright) { set_error("sgs_match_project_keyframe_batch_device: NULL array"); return SGS_ERR_INVALID; }
     if (a->cam.nlevels < 2 || !(a->cam.scale_factors[1] > 1.f)) { set_error("sgs_match_project_keyframe_batch_device: camera scale table missing"); return SGS_ERR_INVALID; }
-    LastFrameArgs A;
-    A.cam = to_cam(a->cam);
-    A.cur_kps = a->cur_kps; A.cur_desc = a->cur_desc; A.cur_uright = a->cur_uright; A.cur_n = a->cur_n;
-    A.cur_cap = m->cur_cap; A.cur_cap_pow2 = pow2_at_least(m->cur_cap);
-    A.last_xyz = a->kf_xyz; A.last_desc = a->kf_desc; A.last_flags = a->kf_valid; A.last_octave = nullptr;
-    A.last_angle = a->kf_angle; A.last_n = a->kf_n; A.last_cap = m->point_cap;
-    A.tcw_cur = a->tcw_cur; A.tcw_last = nullptr; A.th = a->th; A.mono = 1; A.check_ori = a->check_orientation;
-    A.cur_mp = a->cur_mp; A.cur_mp_obs_in = nullptr; A.nmatches = a->nmatches; A.ncand = (unsigned long long*)a->ncand;
+    LastFrameArgs A = projection_args(m, a);
+    A.last_xyz = a->kf_xyz; A.last_desc = a->kf_desc; A.last_flags = a->kf_valid; A.last_angle = a->kf_angle; A.last_n = a->kf_n; A.mono = 1;
     A.kf_mode = 1; A.orb_dist = a->orb_dist; A.log_sf = logf(a->cam.scale_factors[1]); A.kf_min_dist = a->kf_min_dist; A.kf_max_dist = a->kf_max_dist;
-    A.frame_enable = nullptr;
-    A.pre = m->d_pre; A.events = m->d_events;
-    return launch_match_lastframe(A, nframes, (cudaStream_t)stream);
+    return launch_matcher(A, nframes, (cudaStream_t)stream);
 }
 
 SGS_API int sgs_match_project_localmap_batch_device(sgs_matcher* m, const sgs_localmap_batch* a, int nframes, void* stream) {
@@ -130,13 +128,13 @@ SGS_API int sgs_match_project_localmap_batch_device(sgs_matcher* m, const sgs_lo
     LocalMapArgs A;
     A.cam = to_cam(a->cam);
     A.cur_kps = a->cur_kps; A.cur_desc = a->cur_desc; A.cur_uright = a->cur_uright; A.cur_n = a->cur_n;
-    A.cur_cap = m->cur_cap; A.cur_cap_pow2 = pow2_at_least(m->cur_cap);
+    A.cur_cap = m->cur_cap;
     A.mp_inview = a->mp_inview; A.proj_x = a->proj_x; A.proj_y = a->proj_y; A.proj_xr = a->proj_xr; A.level = a->level;
     A.view_cos = a->view_cos; A.mp_desc = a->mp_desc; A.mp_obs = a->mp_obs; A.mp_n = a->mp_n; A.mp_cap = m->point_cap;
     A.th = a->th; A.nnratio = a->nnratio; A.id_base = a->id_base;
     A.f_mp = a->f_mp; A.f_mp_obs = a->f_mp_obs; A.nmatches = a->nmatches; A.ncand = (unsigned long long*)a->ncand;
     A.pre = m->d_lpre;
-    return launch_match_localmap(A, nframes, (cudaStream_t)stream);
+    return launch_matcher(A, nframes, (cudaStream_t)stream);
 }
 
 SGS_API int sgs_match_project_lastframe(const sgs_frame_view* cur, const float* tcw_cur, const float* tcw_last, int nlast,
@@ -149,10 +147,10 @@ SGS_API int sgs_match_project_lastframe(const sgs_frame_view* cur, const float* 
     if (!last_has_mp || !last_xyz || !last_desc || !last_obs || !last_octave || !last_angle || !cur_mp_inout || !cur->keys_un || !cur->u_right || !cur->desc) {
         set_error("sgs_match_project_lastframe: NULL array"); return SGS_ERR_INVALID;
     }
-    sgs_matcher* m = nullptr;
-    int rc = sgs_matcher_create(device, 1, cur->n, nlast, &m);
+    sgs_matcher* h = nullptr;
+    int rc = sgs_matcher_create(device, 1, cur->n, nlast, &h);
     if (rc != SGS_OK) return rc;
-    struct Guard { sgs_matcher* m; ~Guard() { sgs_matcher_destroy(m); } } guard{m};
+    const MatcherPtr m{h, sgs_matcher_destroy};
     const int n = cur->n;
     std::vector<uint8_t> flags(nlast);
     for (int i = 0; i < nlast; ++i) flags[i] = (uint8_t)((last_has_mp[i] ? 1 : 0) | (last_obs[i] ? 2 : 0));
@@ -168,7 +166,7 @@ SGS_API int sgs_match_project_lastframe(const sgs_frame_view* cur, const float* 
     S.in(&b.cur_mp, cur_mp_inout, n); S.opt(&b.cur_mp_obs_in, cur_mp_obs_in, n);
     S.out(&b.nmatches, 1); S.zeroed(&b.ncand, 1);
     if (S.commit() != SGS_OK) return SGS_ERR_CUDA;
-    rc = sgs_match_project_lastframe_batch_device(m, &b, 1, nullptr);
+    rc = sgs_match_project_lastframe_batch_device(m.get(), &b, 1, nullptr);
     if (rc != SGS_OK) return rc;
     S.check(cudaDeviceSynchronize());
     int32_t nm_h = 0;
@@ -186,10 +184,10 @@ SGS_API int sgs_match_project_keyframe(const sgs_frame_view* cur, const float* t
     if (!kf_valid || !kf_xyz || !kf_desc || !kf_angle || !kf_min_dist || !kf_max_dist || !cur_mp_inout || !cur->keys_un || !cur->u_right || !cur->desc) {
         set_error("sgs_match_project_keyframe: NULL array"); return SGS_ERR_INVALID;
     }
-    sgs_matcher* m = nullptr;
-    int rc = sgs_matcher_create(device, 1, cur->n, nkf, &m);
+    sgs_matcher* h = nullptr;
+    int rc = sgs_matcher_create(device, 1, cur->n, nkf, &h);
     if (rc != SGS_OK) return rc;
-    struct Guard { sgs_matcher* m; ~Guard() { sgs_matcher_destroy(m); } } guard{m};
+    const MatcherPtr m{h, sgs_matcher_destroy};
     const int n = cur->n;
     std::vector<uint8_t> flags(nkf);
     for (int i = 0; i < nkf; ++i) flags[i] = kf_valid[i] ? 1 : 0;
@@ -204,7 +202,7 @@ SGS_API int sgs_match_project_keyframe(const sgs_frame_view* cur, const float* t
     S.in(&b.kf_n, &nkf, 1); S.in(&b.tcw_cur, tcw_cur, 16); S.in(&b.cur_mp, cur_mp_inout, n);
     S.out(&b.nmatches, 1); S.zeroed(&b.ncand, 1);
     if (S.commit() != SGS_OK) return SGS_ERR_CUDA;
-    rc = sgs_match_project_keyframe_batch_device(m, &b, 1, nullptr);
+    rc = sgs_match_project_keyframe_batch_device(m.get(), &b, 1, nullptr);
     if (rc != SGS_OK) return rc;
     S.check(cudaDeviceSynchronize());
     int32_t nm_h = 0;
@@ -258,7 +256,7 @@ SGS_API int sgs_search_for_initialization_batch_device(const sgs_init_batch* a, 
     A.f1_kps = a->f1_kps; A.f1_desc = a->f1_desc; A.f1_n = a->f1_n; A.f1_cap = a->f1_cap;
     A.f2_kps = a->f2_kps; A.f2_desc = a->f2_desc; A.f2_n = a->f2_n; A.f2_cap = a->f2_cap;
     A.prev_xy = a->prev_xy; A.window = a->window_size; A.nnratio = a->nnratio; A.check_ori = a->check_orientation; A.match12 = a->match12; A.nmatches = a->nmatches;
-    return launch_search_init(A, nframes, (cudaStream_t)stream);
+    return launch_matcher(A, nframes, (cudaStream_t)stream);
 }
 
 SGS_API int sgs_search_for_initialization(const sgs_frame_view* f1, const sgs_frame_view* f2, float* prev_xy, int window_size, float nnratio, int check_orientation,
@@ -340,10 +338,10 @@ SGS_API int sgs_match_project_localmap(const sgs_frame_view* f, int nmp, const u
     if (!mp_inview || !proj_x || !proj_y || !proj_xr || !level || !view_cos || !mp_desc || !mp_obs || !f_mp_inout || !f_mp_obs_inout) {
         set_error("sgs_match_project_localmap: NULL array"); return SGS_ERR_INVALID;
     }
-    sgs_matcher* m = nullptr;
-    int rc = sgs_matcher_create(device, 1, f->n, nmp, &m);
+    sgs_matcher* h = nullptr;
+    int rc = sgs_matcher_create(device, 1, f->n, nmp, &h);
     if (rc != SGS_OK) return rc;
-    struct Guard { sgs_matcher* m; ~Guard() { sgs_matcher_destroy(m); } } guard{m};
+    const MatcherPtr m{h, sgs_matcher_destroy};
     const int n = f->n;
     const size_t M = (size_t)nmp;
     sgs_localmap_batch b;
@@ -357,7 +355,7 @@ SGS_API int sgs_match_project_localmap(const sgs_frame_view* f, int nmp, const u
     S.in(&b.f_mp, f_mp_inout, n); S.in(&b.f_mp_obs, f_mp_obs_inout, n);
     S.out(&b.nmatches, 1); S.zeroed(&b.ncand, 1);
     if (S.commit() != SGS_OK) return SGS_ERR_CUDA;
-    rc = sgs_match_project_localmap_batch_device(m, &b, 1, nullptr);
+    rc = sgs_match_project_localmap_batch_device(m.get(), &b, 1, nullptr);
     if (rc != SGS_OK) return rc;
     S.check(cudaDeviceSynchronize());
     int32_t nm_h = 0;

@@ -3,6 +3,7 @@
 #pragma once
 #include <cuda_runtime.h>
 
+#include "match_rules.cuh"
 #include "sgs_common.h"
 
 namespace sgs {
@@ -30,7 +31,7 @@ struct LastFrameArgs {
     MatchCam cam;
     // current frames
     const sgs_keypoint* cur_kps; const uint8_t* cur_desc; const float* cur_uright; const int32_t* cur_n;
-    int32_t cur_cap, cur_cap_pow2;
+    int32_t cur_cap;
     // last-frame map points
     const float* last_xyz; const uint8_t* last_desc; const uint8_t* last_flags;  // bit0: has map point & !outlier, bit1: Observations()>0
     const int32_t* last_octave; const float* last_angle; const int32_t* last_n; int32_t last_cap;
@@ -49,7 +50,7 @@ struct LastFrameArgs {
 struct LocalMapArgs {
     MatchCam cam;
     const sgs_keypoint* cur_kps; const uint8_t* cur_desc; const float* cur_uright; const int32_t* cur_n;
-    int32_t cur_cap, cur_cap_pow2;
+    int32_t cur_cap;
     const uint8_t* mp_inview; const float* proj_x; const float* proj_y; const float* proj_xr; const int32_t* level;
     const float* view_cos; const uint8_t* mp_desc; const uint8_t* mp_obs; const int32_t* mp_n; int32_t mp_cap;
     float th, nnratio; int32_t id_base;
@@ -81,9 +82,10 @@ struct InitArgs {                 // ORBmatcher::SearchForInitialization(F1, F2,
     int32_t* match12; int32_t* nmatches;
 };
 
-int launch_match_lastframe(const LastFrameArgs& A, int nframes, cudaStream_t st);
-int launch_search_init(const InitArgs& A, int nframes, cudaStream_t st);
-int launch_fuse_search(const FuseArgs& A, int nframes, cudaStream_t st);
-int launch_match_localmap(const LocalMapArgs& A, int nframes, cudaStream_t st);
+// one block per frame of the matcher that takes these arguments; SGS_ERR_UNSUPPORTED when its frame grid does not fit in shared memory
+int launch_matcher(const LastFrameArgs& A, int nframes, cudaStream_t st);
+int launch_matcher(const LocalMapArgs& A, int nframes, cudaStream_t st);
+int launch_matcher(const FuseArgs& A, int nframes, cudaStream_t st);
+int launch_matcher(const InitArgs& A, int nframes, cudaStream_t st);
 
 }  // namespace sgs
