@@ -465,9 +465,12 @@ SGS_API int sgs_dynreject(const float* cur_xy, const float* prev_xy, int n, cons
 /* Fused device-side variant used by the batched pipeline: computes the verdicts and applies them as an ORDERED compaction
  * of keypoints and descriptor rows (the erase loop :563-597) for `nframes` frames resident on the device.
  *   in : d_kps [F][cap], d_desc [F][cap][32], d_counts [F], d_prev_xy [F][cap][2], d_F [F][9] (double; a NaN in F[0] marks
- *        an empty matrix), d_boxes [F][max_boxes], d_nboxes [F], d_have_dyn [F] (uint8)
+ *        an empty matrix), d_boxes [F][max_boxes], d_nboxes [F], d_have_dyn [F] (uint8); a frame uses its first
+ *        d_counts[f] keypoints and d_nboxes[f] boxes, each clamped to [0, cap] and [0, max_boxes]
  *   out: d_kps_out / d_desc_out / d_counts_out (same shapes; when the restore-all branch fires the frame is copied
- *        unchanged), d_keep [F][cap] (per-point verdicts, may be NULL) */
+ *        unchanged), d_keep [F][cap] (per-point verdicts, may be NULL); rows at and past d_counts_out[f] and verdicts
+ *        past the clamped count are not written.  cap * 4 bytes must fit in 160 KB of shared memory, else
+ *        SGS_ERR_UNSUPPORTED and nothing is enqueued. */
 SGS_API int sgs_dynreject_batch_device(const sgs_keypoint* d_kps, const uint8_t* d_desc, const int32_t* d_counts, int cap,
                                        int nframes, const float* d_prev_xy, const double* d_F, const sgs_rect* d_boxes,
                                        const int32_t* d_nboxes, int max_boxes, const uint8_t* d_have_dyn, int nfeatures,

@@ -132,6 +132,22 @@ REF_API int ref_frame_is_in_frustum(const float* Tcw, float viewing_cos_limit, i
     return cnt;
 }
 
+// The two per-keypoint tests of the rejection on their own: Frame::CheckEpiLineDistToRmDynamicPoint(kp, prev, F (9, row major), threshold) and
+// Frame::isInDynamicRegion(kp, boxes (x, y, w, h)), the KeyPoint overloads the erase loop calls.  Neither reads the Frame's members.
+REF_API int ref_frame_check_epi_line_dist(float x, float y, float px, float py, const double* F9, double threshold) {
+    Frame fr;
+    cv::KeyPoint kp; kp.pt = cv::Point2f(x, y);
+    cv::Mat F(3, 3, CV_64F);
+    for (int i = 0; i < 9; ++i) F.at<double>(i / 3, i % 3) = F9[i];
+    return fr.CheckEpiLineDistToRmDynamicPoint(kp, cv::Point2f(px, py), F, threshold) ? 1 : 0;
+}
+
+REF_API int ref_frame_is_in_dynamic_region(float x, float y, const float* boxes, int nboxes) {
+    Frame fr;
+    cv::KeyPoint kp; kp.pt = cv::Point2f(x, y);
+    return fr.isInDynamicRegion(kp, rects(boxes, nboxes)) ? 1 : 0;
+}
+
 // ---- allocation order = address order (see orbextractor_ref_driver.cpp: DistributeOctTree breaks size ties by node ADDRESS; quirk Q1) -------------------------
 #include <cstdlib>
 namespace {

@@ -60,7 +60,7 @@ __global__ void __launch_bounds__(kDynThreads) dynreject_batch_kernel(const sgs_
     extern __shared__ int32_t s_pos[];   // [cap] exclusive positions (or -1)
     __shared__ double sF[9];
     const int f = blockIdx.x;
-    const int n = min(counts[f], cap);
+    const int n = max(0, min(counts[f], cap));   // a negative count is an empty frame: counts_out 0 even when the restore guard fires
     const int64_t base = (int64_t)f * cap;
     if (threadIdx.x < 9) sF[threadIdx.x] = Fm[9 * f + threadIdx.x];
     __syncthreads();
