@@ -339,7 +339,7 @@ typedef struct sgs_settings {
 SGS_API int sgs_settings_load(const char* path, sgs_settings* out);
 
 /* ------------------------------------------------------------------------------------
- * Bag of words (tracking fallback, Tracking::TrackReferenceKeyFrame src/Tracking.cc:858-904):
+ * Bag of words (tracking fallback, Tracking::TrackReferenceKeyFrame src/Tracking.cc:796-838):
  *   sgs_vocabulary_create       : the DBoW2 tree as flat arrays -- parent[i] of node i in node-id order (node 0 = root; DBoW2 appends children
  *                                 to their parent in that order, TemplatedVocabulary.h:1351-1420 / 1467-1508), node descriptors [nnodes][32],
  *                                 node weights (leaves: the TF-IDF word weight).  Word ids number the leaves in node-id order.
@@ -649,6 +649,52 @@ typedef struct sgs_posechain_batch {
     int32_t* stats;                   /* [F][8] */
 } sgs_posechain_batch;
 SGS_API int sgs_tracker_pose_chain_device(sgs_tracker* t, const sgs_posechain_batch* args, int nframes, void* stream);
+/* Local-map ids the last sgs_tracker_pose_chain_device call's first discard dropped (the outliers of TrackWithMotionModel's PoseOptimization, whose
+ * mnLastFrameSeen :951 sets): [max_batch][mp_cap of that call], 1 = dropped.  Rows with stats[2] < 20 hold none (the reference returns at :933 before
+ * the discard).  Valid until the next pose chain call on the handle; the seen_in of sgs_tracker_refkf_chain_device.  SGS_ERR_INVALID before the first. */
+SGS_API int sgs_tracker_motion_discards_device(const sgs_tracker* t, const uint8_t** d_mask);
+
+/* ------------------------------------------------------------------------------------
+ * The other way Tracking::Track() gets an initial pose, Tracking::TrackReferenceKeyFrame (src/Tracking.cc:796-838), followed by TrackLocalMap, on the
+ * device-resident frame of the last track or step call (the compacted keypoints, or mvKeysUn after an RGB-D step, descriptors, mvuRight, counts), for
+ * the rows the caller enables: the second frame of a sequence (empty mVelocity), the two frames after a relocalisation, a failed motion model
+ * (:349-358).  Per enabled row:
+ *   Frame::ComputeBoW (levelsup 4); ORBmatcher(0.7, true).SearchByBoW(mpReferenceKF, mCurrentFrame) -- a key-frame feature takes part when its map point
+ *   is present and not bad; below 15 matches the row stops (stats 0..1 written, everything else left as it was); PoseOptimization from tcw_last with
+ *   the key frame's points; outliers discarded (nmatches--, nmatchesMap, marked seen in the frame); then TrackLocalMap exactly as the pose chain runs it,
+ *   with the seen_in points left out of the local search as well.
+ * UpdateLocalMap stays with the caller, as for the pose chain.  Ids in f_mp: 0 .. point_cap-1 = key-frame feature, point_cap + j = local-map point j.
+ * stats [F][8]: 0 nmatches of SearchByBoW (-1: kf_n outside [0, point_cap], nothing else written), 1 reached 15 and the rest ran (0/1), 2 unused (0),
+ *   3..7 as the pose chain (nmatches after the discard, nmatchesMap, nToMatch, matches added by the local search, mnMatchesInliers).
+ *   TrackReferenceKeyFrame returned true <=> stats[1] && stats[4] >= 10; rows that pass the gate run TrackLocalMap whatever that verdict.
+ * Limits: nframes <= the frames of the last track or step call; point_cap and the tracker's keypoint cap at most 8192 (SearchByBoW's limit,
+ * SGS_ERR_UNSUPPORTED); kf_desc 16-byte aligned.  Refused calls (SGS_ERR_INVALID / SGS_ERR_UNSUPPORTED) enqueue nothing.  Enqueued on `stream`
+ * (NULL: the tracker's stream), no synchronisation.  A batch that mixes th_local 3 and 5 makes two calls with complementary frame_enable.
+ * ------------------------------------------------------------------------------------ */
+typedef struct sgs_refkf_batch {
+    /* reference key frame of every frame, [F][point_cap] (x3 / x32) like the last-frame arrays of the track calls */
+    const int32_t* kf_node; const double* kf_weight;   /* its FeatureVector: sgs_bow_transform_batch_device on its descriptors, levelsup 4 */
+    const uint8_t* kf_desc; const float* kf_angle;     /* pKF->mDescriptors, mvKeysUn[i].angle */
+    const float* kf_xyz;                               /* GetWorldPos() of the map point of feature i */
+    const uint8_t* kf_flags;                           /* bit 0 map point present, bit 1 Observations() > 0, bit 2 isBad() */
+    const int32_t* kf_n;                               /* [F] */
+    const int32_t* kf_local_id;                        /* index of feature i's map point in this frame's local-map list, -1 = not in it (may be NULL) */
+    const float* tcw_last;                             /* [F][16] mLastFrame.mTcw at the call (:812; after UpdateLastFrame when the motion model ran first) */
+    const uint8_t* frame_enable;                       /* [F] may be NULL = all; 0 = row untouched */
+    const uint8_t* seen_in;                            /* [F][mp_cap] may be NULL: local-map points whose mnLastFrameSeen is already this frame
+                                                          (sgs_tracker_motion_discards_device after a failed motion model) */
+    /* local map of every frame, [F][mp_cap], and the local search: as in sgs_posechain_batch */
+    const float* mp_xyz; const float* mp_normal; const float* mp_min_dist; const float* mp_max_dist; const uint8_t* mp_desc;
+    const uint8_t* mp_valid; const uint8_t* mp_obs; const int32_t* mp_n; int32_t mp_cap;
+    float th_local, nnratio_local;                     /* 3 (RGB-D), 5 right after a relocalisation (:1304-1309); 0.8 */
+    float inv_level_sigma2[16];
+    /* outputs (device), written only for rows that pass the gate (stats for every enabled row) */
+    float* tcw_refkf; float* tcw_final;                /* [F][16] after TrackReferenceKeyFrame's PoseOptimization / after TrackLocalMap */
+    int32_t* f_mp;                                     /* [F][cap] */
+    uint8_t* outlier;                                  /* [F][cap] mvbOutlier after the second PoseOptimization */
+    int32_t* stats;                                    /* [F][8] */
+} sgs_refkf_batch;
+SGS_API int sgs_tracker_refkf_chain_device(sgs_tracker* t, const sgs_vocabulary* voc, const sgs_refkf_batch* args, int nframes, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------------------------
  * Object detector: Detector2D (src/Detector2D.cc:16-89, include/Detector2D.h:29-80) -- ncnn forward of the MobileNetV3-SSDLite graph

@@ -124,6 +124,7 @@ __global__ void __launch_bounds__(kBowThreads) bow_search_kernel(const BowArgs A
     const int64_t oo = A.pair_mode ? ko : fo;                      // the result is indexed by the first side in pair mode
     for (int j = tid; j < A.f_cap; j += blockDim.x) taken[j] = 0;
     for (int j = tid; j < (A.pair_mode ? A.kf_cap : A.f_cap); j += blockDim.x) A.match_f[oo + j] = -1;
+    if (nk_all == 0 || nf_all == 0) { if (tid == 0) A.nmatches[f] = 0; return; }      // an empty side matches nothing: no sort (rows a caller switched off by a zero count)
     __syncthreads();
     bow_bitonic(kkey, A.kf_pow2);
     bow_bitonic(fkey, A.f_pow2);

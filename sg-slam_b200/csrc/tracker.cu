@@ -75,6 +75,15 @@ struct sgs_tracker {
     double* d_po_err = nullptr; uint8_t* d_po_level = nullptr;
     uint8_t* d_inview = nullptr; float* d_projx = nullptr; float* d_projy = nullptr; float* d_projxr = nullptr; int32_t* d_level = nullptr; float* d_viewcos = nullptr;
     unsigned long long* d_ncand2 = nullptr;
+    // the local-map ids of the outliers the last pose chain's first discard dropped, [max_batch][mp_cap of that call]; sized by the pose chain only, so
+    // that a sgs_tracker_refkf_chain_device call reading it as seen_in never reallocates it
+    uint8_t* d_mdisc = nullptr; int mdisc_cap = 0;
+    // sgs_tracker_refkf_chain_device, sized on first use: the frame's BoW (word, weight, node) and keypoint angles [B][cap], the key frame's valid flags
+    // [B][point_cap], the matches [B][cap], per row the counts (keypoints, key-frame features, local-map points; 0 = no work), the BoW nmatches, the
+    // run flag and the two poses
+    int32_t* d_rk_word = nullptr; double* d_rk_weight = nullptr; int32_t* d_rk_node = nullptr; float* d_rk_ang = nullptr; uint8_t* d_rk_valid = nullptr;
+    int32_t* d_rk_mp = nullptr; int32_t* d_rk_n = nullptr; int32_t* d_rk_kfn = nullptr; int32_t* d_rk_mpn = nullptr; int32_t* d_rk_nm = nullptr;
+    uint8_t* d_rk_run = nullptr; float* d_rk_T1 = nullptr; float* d_rk_T2 = nullptr;
     StreamState ss;                             // the RGB-D stream steps
 };
 
@@ -117,14 +126,20 @@ __global__ void chain_merge_counts_kernel(const uint8_t* __restrict__ enable, co
     if (enable[f]) nm[f] = nm2[f];
     stats[8 * f + 2] = nm[f];
 }
-// :940-957 discard the outliers of the first PoseOptimization; SearchLocalPoints' first loop (:1265-1281): every map point matched in the frame --
-// the discarded ones too, their mnLastFrameSeen was set at :951 -- is marked as seen, bad ones lose their slot (last_flags bit 2 = isBad()).
+// :940-957 discard the outliers of the first PoseOptimization (TrackReferenceKeyFrame: :816-835); SearchLocalPoints' first loop (:1265-1281): every map
+// point matched in the frame -- the discarded ones too, their mnLastFrameSeen was set at :951 / :831 -- is marked as seen, bad ones lose their slot
+// (flags bit 2 = isBad()).  flags / local_id: [F][point_cap] of the points the ids below point_cap name.  run (NULL = every row): 0 = the row is left
+// as it is.  discards (NULL: not kept): the local-map ids of the dropped outliers, for rows with nm >= 20 -- below that TrackWithMotionModel returns at
+// :933 before its discard.
 __global__ void __launch_bounds__(256) chain_discard_kernel(const int32_t* __restrict__ n_cur, int cap, int point_cap, const uint8_t* __restrict__ last_flags,
                                                             const int32_t* __restrict__ last_local_id, int mp_cap, int32_t* __restrict__ mp, uint8_t* __restrict__ outlier,
-                                                            uint8_t* __restrict__ obs, uint8_t* __restrict__ seen, const int32_t* __restrict__ nm, int32_t* __restrict__ stats) {
+                                                            uint8_t* __restrict__ obs, uint8_t* __restrict__ seen, const int32_t* __restrict__ nm, int32_t* __restrict__ stats,
+                                                            const uint8_t* __restrict__ run, uint8_t* __restrict__ discards) {
     __shared__ int s_drop, s_map;
     const int f = blockIdx.x;
+    if (run && !run[f]) return;
     const int n = min(n_cur[f], cap);
+    const bool keep_discards = discards && nm[f] >= 20;
     if (threadIdx.x == 0) { s_drop = 0; s_map = 0; }
     __syncthreads();
     int drop = 0, nmap = 0;
@@ -135,9 +150,12 @@ __global__ void __launch_bounds__(256) chain_discard_kernel(const int32_t* __res
         if (id >= 0) {
             const uint8_t fl = last_flags[(int64_t)f * point_cap + id];
             const int lid = last_local_id ? last_local_id[(int64_t)f * point_cap + id] : -1;
-            if (lid >= 0 && lid < mp_cap) seen[(int64_t)f * mp_cap + lid] = 1;
-            if (outlier[k]) { id = -1; outlier[k] = 0; ++drop; }
-            else {
+            const bool local = lid >= 0 && lid < mp_cap;
+            if (local) seen[(int64_t)f * mp_cap + lid] = 1;
+            if (outlier[k]) {
+                if (local && keep_discards) discards[(int64_t)f * mp_cap + lid] = 1;
+                id = -1; outlier[k] = 0; ++drop;
+            } else {
                 if (fl & 2) ++nmap;
                 if (fl & 4) id = -1;                       // isBad(): removed by SearchLocalPoints, after the counts of TrackWithMotionModel
                 else ob = (fl >> 1) & 1;
@@ -150,18 +168,21 @@ __global__ void __launch_bounds__(256) chain_discard_kernel(const int32_t* __res
     __syncthreads();
     if (threadIdx.x == 0) { stats[8 * f + 3] = nm[f] - s_drop; stats[8 * f + 4] = s_map; }
 }
-// SearchLocalPoints' second loop (:1286-1300): points seen in this frame or bad are skipped before isInFrustum; nToMatch
+// SearchLocalPoints' second loop (:1286-1300): points seen in this frame (seen, or seen_in: marked before this chain, may be NULL) or bad are skipped
+// before isInFrustum; nToMatch
 __global__ void __launch_bounds__(256) chain_mask_kernel(const int32_t* __restrict__ mp_n, int mp_cap, const uint8_t* __restrict__ mp_valid, const uint8_t* __restrict__ seen,
-                                                         uint8_t* __restrict__ inview, int32_t* __restrict__ stats) {
+                                                         const uint8_t* __restrict__ seen_in, uint8_t* __restrict__ inview, int32_t* __restrict__ stats,
+                                                         const uint8_t* __restrict__ run) {
     __shared__ int s_cnt;
     const int f = blockIdx.x;
+    if (run && !run[f]) return;
     const int n = min(mp_n[f], mp_cap);
     if (threadIdx.x == 0) s_cnt = 0;
     __syncthreads();
     int c = 0;
     for (int j = threadIdx.x; j < mp_cap; j += blockDim.x) {
         const int64_t k = (int64_t)f * mp_cap + j;
-        const uint8_t v = (j < n && inview[k] && mp_valid[k] && !seen[k]) ? 1 : 0;
+        const uint8_t v = (j < n && inview[k] && mp_valid[k] && !seen[k] && !(seen_in && seen_in[k])) ? 1 : 0;
         inview[k] = v; c += v;
     }
     atomicAdd(&s_cnt, c);
@@ -170,9 +191,11 @@ __global__ void __launch_bounds__(256) chain_mask_kernel(const int32_t* __restri
 }
 // :982-996 mnMatchesInliers (mbOnlyTracking == false): map point && !outlier && Observations() > 0
 __global__ void __launch_bounds__(256) chain_final_kernel(const int32_t* __restrict__ n_cur, int cap, const int32_t* __restrict__ mp, const uint8_t* __restrict__ outlier,
-                                                          const uint8_t* __restrict__ obs, const int32_t* __restrict__ nml, int32_t* __restrict__ f_mp, int32_t* __restrict__ stats) {
+                                                          const uint8_t* __restrict__ obs, const int32_t* __restrict__ nml, int32_t* __restrict__ f_mp, int32_t* __restrict__ stats,
+                                                          const uint8_t* __restrict__ run) {
     __shared__ int s_cnt;
     const int f = blockIdx.x;
+    if (run && !run[f]) return;
     const int n = min(n_cur[f], cap);
     if (threadIdx.x == 0) s_cnt = 0;
     __syncthreads();
@@ -186,6 +209,52 @@ __global__ void __launch_bounds__(256) chain_final_kernel(const int32_t* __restr
     atomicAdd(&s_cnt, c);
     __syncthreads();
     if (threadIdx.x == 0) { stats[8 * f + 6] = nml[f]; stats[8 * f + 7] = s_cnt; }
+}
+// ---- glue of sgs_tracker_refkf_chain_device (Tracking::TrackReferenceKeyFrame, src/Tracking.cc:796-838) ------------------------------------------
+// Per row before ComputeBoW: enabled (frame_enable NULL = all) rows with 0 <= kf_n <= point_cap run; the others get zero counts, so that the BoW
+// transform and matcher exit at once.  A running row gets its key-frame features' SearchByBoW validity (map point present && !isBad(), :176-178 of
+// src/ORBmatcher.cc) and its keypoint angles (mvKeysUn[i].angle == mvKeys[i].angle); an enabled row with kf_n out of range gets stats[0] = -1.
+__global__ void __launch_bounds__(256) refkf_prep_kernel(const uint8_t* __restrict__ enable, const int32_t* __restrict__ n_cur, int cap, const int32_t* __restrict__ kf_n,
+                                                         int point_cap, const uint8_t* __restrict__ kf_flags, const sgs_keypoint* __restrict__ kps,
+                                                         int32_t* __restrict__ n_out, int32_t* __restrict__ kfn_out, uint8_t* __restrict__ run,
+                                                         uint8_t* __restrict__ kf_valid, float* __restrict__ angle, int32_t* __restrict__ stats) {
+    const int f = blockIdx.x;
+    const bool en = !enable || enable[f];
+    const int kn = kf_n[f];
+    const bool ok = en && kn >= 0 && kn <= point_cap;
+    const int n = ok ? min(n_cur[f], cap) : 0;
+    if (threadIdx.x == 0) {
+        n_out[f] = n; kfn_out[f] = ok ? kn : 0; run[f] = ok ? 1 : 0;
+        if (en && !ok) for (int q = 0; q < 8; ++q) stats[8 * f + q] = q == 0 ? -1 : 0;
+    }
+    if (!ok) return;
+    for (int i = threadIdx.x; i < kn; i += blockDim.x) {
+        const uint8_t fl = kf_flags[(int64_t)f * point_cap + i];
+        kf_valid[(int64_t)f * point_cap + i] = ((fl & 1) && !(fl & 4)) ? 1 : 0;
+    }
+    for (int i = threadIdx.x; i < n; i += blockDim.x) angle[(int64_t)f * cap + i] = kps[(int64_t)f * cap + i].angle;
+}
+// :808-809: fewer than 15 BoW matches stops the row (stats 0..1 written, the rest 0); a row that passes gets its local-map count and cleared outlier flags
+// (mvbOutlier of keypoints without a map point stays false).  Rows that do not run get zero counts for the rest of the chain.
+__global__ void __launch_bounds__(256) refkf_gate_kernel(const int32_t* __restrict__ nm, const int32_t* __restrict__ mp_n, int cap, int32_t* __restrict__ n_cur,
+                                                         int32_t* __restrict__ mpn_out, uint8_t* __restrict__ run, uint8_t* __restrict__ outlier, int32_t* __restrict__ stats) {
+    const int f = blockIdx.x;
+    const bool en = run[f] != 0;
+    const bool pass = en && nm[f] >= 15;
+    __syncthreads();                                   // every thread has read run[f] before thread 0 rewrites it
+    if (threadIdx.x == 0) {
+        mpn_out[f] = pass ? mp_n[f] : 0;
+        if (!pass) { n_cur[f] = 0; run[f] = 0; }
+        if (en) for (int q = 0; q < 8; ++q) stats[8 * f + q] = q == 0 ? nm[f] : q == 1 ? (pass ? 1 : 0) : 0;
+    }
+    if (pass) for (int i = threadIdx.x; i < cap; i += blockDim.x) outlier[(int64_t)f * cap + i] = 0;
+}
+// the poses of the rows that ran: after the first PoseOptimization (:814) and after TrackLocalMap
+__global__ void refkf_commit_kernel(const uint8_t* __restrict__ run, const float* __restrict__ T1, const float* __restrict__ T2, float* __restrict__ tcw_refkf,
+                                    float* __restrict__ tcw_final) {
+    const int f = blockIdx.x, q = threadIdx.x;
+    if (!run[f] || q >= 16) return;
+    tcw_refkf[16 * f + q] = T1[16 * f + q]; tcw_final[16 * f + q] = T2[16 * f + q];
 }
 // ---- the RGB-D stream steps (StreamState) ----------------------------------------------------------------------------------------------------
 // Per frame of a call, before LK: a first frame (its slot never held a frame, or new_stream[f]) tracks into its own image and has no previous frame;
@@ -524,6 +593,91 @@ int enqueue_step(sgs_tracker* t, sgs_detector* det, const StepFrames& fr, int nf
     return enqueue_track(t, nframes, t->d_prev, t->d_uright_in, t->d_Fgpu, t->d_boxes, t->d_nboxes, t->d_have, last, th, mono, check_orientation,
                          rgbd ? t->d_kpsun : nullptr, rgbd ? t->d_dz : nullptr, st);
 }
+
+// the chain scratch of sgs_tracker_pose_chain_device and sgs_tracker_refkf_chain_device, sized for (max_batch, mp_cap) on first use or a larger map
+int ensure_chain_scratch(sgs_tracker* t, const char* fn, int mp_cap) {
+    if (t->chain_mp_cap >= mp_cap) return SGS_OK;
+    const size_t B = t->max_batch, K = t->cap, M = mp_cap;
+    t->chain_mp_cap = 0;
+    t->mt_local.reset();
+    sgs_matcher* mt_local = nullptr;
+    const int rc = sgs_matcher_create(t->device, t->max_batch, t->cap, mp_cap, &mt_local);
+    t->mt_local.reset(mt_local);
+    if (rc != SGS_OK) return rc;
+    HandleResources& R = t->res;
+    // 16 bytes of slack past the end of every array, as in sgs_tracker_create
+    SGS_CUDA_TRY_AT(fn, R.regrow(&t->d_enable, B + 16)); SGS_CUDA_TRY_AT(fn, R.regrow(&t->d_nm2, B * 4 + 16)); SGS_CUDA_TRY_AT(fn, R.regrow(&t->d_obs, B * K + 16));
+    SGS_CUDA_TRY_AT(fn, R.regrow(&t->d_seen, B * M + 16)); SGS_CUDA_TRY_AT(fn, R.regrow(&t->d_ninl, B * 4 + 16)); SGS_CUDA_TRY_AT(fn, R.regrow(&t->d_nml, B * 4 + 16));
+    SGS_CUDA_TRY_AT(fn, R.regrow(&t->d_po_err, B * K * 24 + 16)); SGS_CUDA_TRY_AT(fn, R.regrow(&t->d_po_level, B * K + 16)); SGS_CUDA_TRY_AT(fn, R.regrow(&t->d_inview, B * M + 16));
+    SGS_CUDA_TRY_AT(fn, R.regrow(&t->d_projx, B * M * 4 + 16)); SGS_CUDA_TRY_AT(fn, R.regrow(&t->d_projy, B * M * 4 + 16)); SGS_CUDA_TRY_AT(fn, R.regrow(&t->d_projxr, B * M * 4 + 16));
+    SGS_CUDA_TRY_AT(fn, R.regrow(&t->d_level, B * M * 4 + 16)); SGS_CUDA_TRY_AT(fn, R.regrow(&t->d_viewcos, B * M * 4 + 16)); SGS_CUDA_TRY_AT(fn, R.regrow(&t->d_ncand2, B * 8 + 16));
+    t->chain_mp_cap = mp_cap;
+    return SGS_OK;
+}
+
+// The first PoseOptimization of both chains on the tracker's compacted frame: map point of keypoint i = points_xyz[mp[i]] (-1 none), counts n
+sgs_poseopt_batch first_optimization(const sgs_tracker* t, const float* tcw_in, const int32_t* n, const int32_t* mp, const float* points_xyz,
+                                     const float* inv_level_sigma2, float* tcw_out, uint8_t* outlier) {
+    sgs_poseopt_batch po;
+    std::memset(&po, 0, sizeof po);
+    po.cam = t->cam; po.tcw_in = tcw_in; po.kps = t->keys_un; po.uright = t->d_uright2; po.n = n; po.cap = t->cap;
+    po.mp_index = mp; po.points_xyz = points_xyz; po.point_cap = t->point_cap;
+    for (int l = 0; l < 16; ++l) po.inv_level_sigma2[l] = inv_level_sigma2[l];
+    po.tcw_out = tcw_out; po.outlier = outlier; po.ninliers = t->d_ninl; po.scratch_err = t->d_po_err; po.scratch_level = t->d_po_level;
+    return po;
+}
+
+// The local map of every frame and the local search's parameters: the mp_* / th_local / nnratio_local fields both chain structs share.  mp_n: [F]
+// local-map sizes (0: the row does no work).
+struct LocalMap {
+    const float* xyz; const float* normal; const float* min_dist; const float* max_dist; const uint8_t* desc; const uint8_t* valid; const uint8_t* obs;
+    const int32_t* n; int cap; float th, nnratio;
+};
+template <class Batch> LocalMap local_map(const Batch* a, const int32_t* mp_n) {
+    return {a->mp_xyz, a->mp_normal, a->mp_min_dist, a->mp_max_dist, a->mp_desc, a->mp_valid, a->mp_obs, mp_n, a->mp_cap, a->th_local, a->nnratio_local};
+}
+
+// The frame after the first PoseOptimization, as the TrackLocalMap half takes it, and where that half writes.
+struct FirstHalf {
+    const int32_t* n = nullptr;          // [F] keypoints (0: the row does no work)
+    const uint8_t* run = nullptr;        // [F] NULL = every row; 0 = the row's stats and f_mp are not written
+    const int32_t* nm = nullptr;         // [F] matches before the discard
+    const uint8_t* flags = nullptr; const int32_t* local_id = nullptr;   // [F][point_cap] for the ids below point_cap (local_id may be NULL)
+    const uint8_t* seen_in = nullptr;    // [F][mp_cap] may be NULL: local-map points already seen in the frame
+    uint8_t* discards = nullptr;         // [F][mp_cap] may be NULL: receives the local-map ids of the dropped outliers (rows with nm >= 20)
+    int32_t* mp = nullptr;               // [F][cap] in/out: the matches as ids
+    const float* tcw_first = nullptr; float* tcw_final = nullptr; int32_t* f_mp = nullptr; int32_t* stats = nullptr;
+};
+
+// Both chains after their first PoseOptimization `po` (its outlier flags are read): discard the outliers, SearchLocalPoints (frustum test with the new pose,
+// scale prediction, projection search), the second PoseOptimization, mnMatchesInliers.
+int enqueue_local_half(sgs_tracker* t, const LocalMap& lm_in, const FirstHalf& h, sgs_poseopt_batch po, int F, cudaStream_t st) {
+    const int cap = t->cap, M = lm_in.cap;
+    SGS_CUDA_TRY(cudaMemsetAsync(t->d_seen, 0, (size_t)F * M, st));
+    chain_discard_kernel<<<F, 256, 0, st>>>(h.n, cap, t->point_cap, h.flags, h.local_id, M, h.mp, po.outlier, t->d_obs, t->d_seen, h.nm, h.stats, h.run, h.discards);
+    sgs_frustum_batch fr;
+    std::memset(&fr, 0, sizeof fr);
+    fr.cam = t->cam; fr.tcw = h.tcw_first; fr.mp_xyz = lm_in.xyz; fr.mp_normal = lm_in.normal; fr.mp_min_dist = lm_in.min_dist; fr.mp_max_dist = lm_in.max_dist;
+    fr.mp_n = lm_in.n; fr.point_cap = M; fr.viewing_cos_limit = 0.5f;
+    fr.mp_inview = t->d_inview; fr.proj_x = t->d_projx; fr.proj_y = t->d_projy; fr.proj_xr = t->d_projxr; fr.level = t->d_level; fr.view_cos = t->d_viewcos;
+    int rc = sgs_frustum_batch_device(&fr, F, st);
+    if (rc != SGS_OK) return rc;
+    chain_mask_kernel<<<F, 256, 0, st>>>(lm_in.n, M, lm_in.valid, t->d_seen, h.seen_in, t->d_inview, h.stats, h.run);
+    sgs_localmap_batch lm;
+    std::memset(&lm, 0, sizeof lm);
+    lm.cam = t->cam; lm.cur_kps = t->keys_un; lm.cur_desc = t->d_desc2; lm.cur_uright = t->d_uright2; lm.cur_n = h.n;
+    lm.mp_inview = t->d_inview; lm.proj_x = t->d_projx; lm.proj_y = t->d_projy; lm.proj_xr = t->d_projxr; lm.level = t->d_level; lm.view_cos = t->d_viewcos;
+    lm.mp_desc = lm_in.desc; lm.mp_obs = lm_in.obs; lm.mp_n = lm_in.n; lm.th = lm_in.th; lm.nnratio = lm_in.nnratio; lm.id_base = t->point_cap;
+    lm.f_mp = h.mp; lm.f_mp_obs = t->d_obs; lm.nmatches = t->d_nml; lm.ncand = (uint64_t*)t->d_ncand2;
+    rc = sgs_match_project_localmap_batch_device(t->mt_local.get(), &lm, F, st);
+    if (rc != SGS_OK) return rc;
+    po.tcw_in = h.tcw_first; po.tcw_out = h.tcw_final; po.points2_xyz = lm_in.xyz; po.id_base2 = t->point_cap; po.point2_cap = M;
+    rc = sgs_pose_optimization_batch_device(&po, F, st);
+    if (rc != SGS_OK) return rc;
+    chain_final_kernel<<<F, 256, 0, st>>>(h.n, cap, h.mp, po.outlier, t->d_obs, t->d_nml, h.f_mp, h.stats, h.run);
+    SGS_CUDA_TRY(cudaGetLastError());
+    return SGS_OK;
+}
 }  // namespace
 
 extern "C" {
@@ -745,22 +899,12 @@ SGS_API int sgs_tracker_pose_chain_device(sgs_tracker* t, const sgs_posechain_ba
     if (a->mp_cap < 1) return bad(fn, "mp_cap < 1");
     SGS_CUDA_TRY(cudaSetDevice(t->device));
     cudaStream_t st = stream ? (cudaStream_t)stream : t->st;
-    const size_t B = t->max_batch, K = t->cap, M = a->mp_cap;
-    if (t->chain_mp_cap < a->mp_cap) {                       // scratch for this local-map capacity (first call, or a larger map)
-        t->chain_mp_cap = 0;
-        t->mt_local.reset();
-        sgs_matcher* mt_local = nullptr;
-        const int rc = sgs_matcher_create(t->device, t->max_batch, t->cap, a->mp_cap, &mt_local);
-        t->mt_local.reset(mt_local);
-        if (rc != SGS_OK) return rc;
-        HandleResources& R = t->res;
-        // 16 bytes of slack past the end of every array, as in sgs_tracker_create
-        SGS_CUDA_TRY_AT(fn, R.regrow(&t->d_enable, B + 16)); SGS_CUDA_TRY_AT(fn, R.regrow(&t->d_nm2, B * 4 + 16)); SGS_CUDA_TRY_AT(fn, R.regrow(&t->d_obs, B * K + 16));
-        SGS_CUDA_TRY_AT(fn, R.regrow(&t->d_seen, B * M + 16)); SGS_CUDA_TRY_AT(fn, R.regrow(&t->d_ninl, B * 4 + 16)); SGS_CUDA_TRY_AT(fn, R.regrow(&t->d_nml, B * 4 + 16));
-        SGS_CUDA_TRY_AT(fn, R.regrow(&t->d_po_err, B * K * 24 + 16)); SGS_CUDA_TRY_AT(fn, R.regrow(&t->d_po_level, B * K + 16)); SGS_CUDA_TRY_AT(fn, R.regrow(&t->d_inview, B * M + 16));
-        SGS_CUDA_TRY_AT(fn, R.regrow(&t->d_projx, B * M * 4 + 16)); SGS_CUDA_TRY_AT(fn, R.regrow(&t->d_projy, B * M * 4 + 16)); SGS_CUDA_TRY_AT(fn, R.regrow(&t->d_projxr, B * M * 4 + 16));
-        SGS_CUDA_TRY_AT(fn, R.regrow(&t->d_level, B * M * 4 + 16)); SGS_CUDA_TRY_AT(fn, R.regrow(&t->d_viewcos, B * M * 4 + 16)); SGS_CUDA_TRY_AT(fn, R.regrow(&t->d_ncand2, B * 8 + 16));
-        t->chain_mp_cap = a->mp_cap;
+    int rc = ensure_chain_scratch(t, fn, a->mp_cap);
+    if (rc != SGS_OK) return rc;
+    if (t->mdisc_cap < a->mp_cap) {
+        t->mdisc_cap = 0;
+        SGS_CUDA_TRY_AT(fn, t->res.regrow(&t->d_mdisc, (size_t)t->max_batch * a->mp_cap + 16));
+        t->mdisc_cap = a->mp_cap;
     }
     const int F = nframes, cap = t->cap;
     // 1. the wide-window retry of the frames with fewer than 20 matches: the search of the track call with 2 th, on those frames, into its own counts
@@ -769,44 +913,80 @@ SGS_API int sgs_tracker_pose_chain_device(sgs_tracker* t, const sgs_posechain_ba
     lf.nmatches = t->d_nm2; lf.ncand = (uint64_t*)t->d_ncand2; lf.frame_enable = t->d_enable;
     SGS_CUDA_TRY(cudaMemsetAsync(t->d_ncand2, 0, (size_t)F * 8, st));
     SGS_CUDA_TRY(cudaMemsetAsync(t->d_nm2, 0, (size_t)F * 4, st));
-    int rc = sgs_match_project_lastframe_batch_device(t->mt.get(), &lf, F, st);
+    rc = sgs_match_project_lastframe_batch_device(t->mt.get(), &lf, F, st);
     if (rc != SGS_OK) return rc;
     chain_merge_counts_kernel<<<(F + 127) / 128, 128, 0, st>>>(t->d_enable, t->d_nm2, t->d_nm, a->stats, F);
     // 2. PoseOptimization on the last-frame matches
     SGS_CUDA_TRY(cudaMemsetAsync(a->outlier, 0, (size_t)F * cap, st));
-    sgs_poseopt_batch po;
-    std::memset(&po, 0, sizeof po);
-    po.cam = t->cam; po.tcw_in = a->tcw_cur; po.kps = t->keys_un; po.uright = t->d_uright2; po.n = t->d_cnt2; po.cap = cap;
-    po.mp_index = t->d_mp; po.points_xyz = a->last_xyz; po.point_cap = t->point_cap;
-    for (int l = 0; l < 16; ++l) po.inv_level_sigma2[l] = a->inv_level_sigma2[l];
-    po.tcw_out = a->tcw_motion; po.outlier = a->outlier; po.ninliers = t->d_ninl; po.scratch_err = t->d_po_err; po.scratch_level = t->d_po_level;
+    sgs_poseopt_batch po = first_optimization(t, a->tcw_cur, t->d_cnt2, t->d_mp, a->last_xyz, a->inv_level_sigma2, a->tcw_motion, a->outlier);
     rc = sgs_pose_optimization_batch_device(&po, F, st);
     if (rc != SGS_OK) return rc;
-    // 3. discard outliers, mark the map points seen in the frame
-    SGS_CUDA_TRY(cudaMemsetAsync(t->d_seen, 0, (size_t)F * M, st));
-    chain_discard_kernel<<<F, 256, 0, st>>>(t->d_cnt2, cap, t->point_cap, a->last_flags, a->last_local_id, a->mp_cap, t->d_mp, a->outlier, t->d_obs, t->d_seen, t->d_nm, a->stats);
-    // 4. SearchLocalPoints: frustum test with the new pose, scale prediction, projection search
-    sgs_frustum_batch fr;
-    std::memset(&fr, 0, sizeof fr);
-    fr.cam = t->cam; fr.tcw = a->tcw_motion; fr.mp_xyz = a->mp_xyz; fr.mp_normal = a->mp_normal; fr.mp_min_dist = a->mp_min_dist; fr.mp_max_dist = a->mp_max_dist;
-    fr.mp_n = a->mp_n; fr.point_cap = a->mp_cap; fr.viewing_cos_limit = 0.5f;
-    fr.mp_inview = t->d_inview; fr.proj_x = t->d_projx; fr.proj_y = t->d_projy; fr.proj_xr = t->d_projxr; fr.level = t->d_level; fr.view_cos = t->d_viewcos;
-    rc = sgs_frustum_batch_device(&fr, F, st);
+    // 3-5. discard, SearchLocalPoints, PoseOptimization, inlier count; the discarded outliers' local-map ids are kept for sgs_tracker_motion_discards_device
+    SGS_CUDA_TRY(cudaMemsetAsync(t->d_mdisc, 0, (size_t)F * a->mp_cap, st));
+    FirstHalf h;
+    h.n = t->d_cnt2; h.nm = t->d_nm; h.flags = a->last_flags; h.local_id = a->last_local_id; h.discards = t->d_mdisc; h.mp = t->d_mp;
+    h.tcw_first = a->tcw_motion; h.tcw_final = a->tcw_final; h.f_mp = a->f_mp; h.stats = a->stats;
+    return enqueue_local_half(t, local_map(a, a->mp_n), h, po, F, st);
+}
+
+SGS_API int sgs_tracker_motion_discards_device(const sgs_tracker* t, const uint8_t** d_mask) {
+    if (!t || !d_mask) return bad("sgs_tracker_motion_discards_device", "NULL");
+    if (!t->d_mdisc) return bad("sgs_tracker_motion_discards_device", "no pose chain has run on this handle");
+    *d_mask = t->d_mdisc;
+    return SGS_OK;
+}
+
+SGS_API int sgs_tracker_refkf_chain_device(sgs_tracker* t, const sgs_vocabulary* voc, const sgs_refkf_batch* a, int nframes, void* stream) {
+    const char* const fn = "sgs_tracker_refkf_chain_device";
+    if (!t || !voc || !a) return bad(fn, "NULL");
+    if (!a->kf_node || !a->kf_weight || !a->kf_desc || !a->kf_angle || !a->kf_xyz || !a->kf_flags || !a->kf_n || !a->tcw_last || !a->mp_xyz || !a->mp_normal ||
+        !a->mp_min_dist || !a->mp_max_dist || !a->mp_desc || !a->mp_valid || !a->mp_obs || !a->mp_n || !a->tcw_refkf || !a->tcw_final || !a->f_mp || !a->outlier ||
+        !a->stats)
+        return bad(fn, "NULL array");
+    if (!frames_ok(fn, nframes, t->last_nframes)) return SGS_ERR_INVALID;
+    if (a->mp_cap < 1) return bad(fn, "mp_cap < 1");
+    if (t->point_cap > 8192 || t->cap > 8192) { set_error("%s: SearchByBoW takes at most 8192 features per side (point_cap %d, cap %d)", fn, t->point_cap, t->cap); return SGS_ERR_UNSUPPORTED; }
+    SGS_CUDA_TRY(cudaSetDevice(t->device));
+    cudaStream_t st = stream ? (cudaStream_t)stream : t->st;
+    int rc = ensure_chain_scratch(t, fn, a->mp_cap);
     if (rc != SGS_OK) return rc;
-    chain_mask_kernel<<<F, 256, 0, st>>>(a->mp_n, a->mp_cap, a->mp_valid, t->d_seen, t->d_inview, a->stats);
-    sgs_localmap_batch lm;
-    std::memset(&lm, 0, sizeof lm);
-    lm.cam = t->cam; lm.cur_kps = t->keys_un; lm.cur_desc = t->d_desc2; lm.cur_uright = t->d_uright2; lm.cur_n = t->d_cnt2;
-    lm.mp_inview = t->d_inview; lm.proj_x = t->d_projx; lm.proj_y = t->d_projy; lm.proj_xr = t->d_projxr; lm.level = t->d_level; lm.view_cos = t->d_viewcos;
-    lm.mp_desc = a->mp_desc; lm.mp_obs = a->mp_obs; lm.mp_n = a->mp_n; lm.th = a->th_local; lm.nnratio = a->nnratio_local; lm.id_base = t->point_cap;
-    lm.f_mp = t->d_mp; lm.f_mp_obs = t->d_obs; lm.nmatches = t->d_nml; lm.ncand = (uint64_t*)t->d_ncand2;
-    rc = sgs_match_project_localmap_batch_device(t->mt_local.get(), &lm, F, st);
+    if (!t->d_rk_T2) {      // allocated last: a failed first attempt is repeated whole by the next call
+        HandleResources& R = t->res;
+        const size_t B = t->max_batch, K = t->cap, P = t->point_cap;
+        SGS_CUDA_TRY_AT(fn, R.regrow(&t->d_rk_word, B * K * 4 + 16)); SGS_CUDA_TRY_AT(fn, R.regrow(&t->d_rk_weight, B * K * 8 + 16)); SGS_CUDA_TRY_AT(fn, R.regrow(&t->d_rk_node, B * K * 4 + 16));
+        SGS_CUDA_TRY_AT(fn, R.regrow(&t->d_rk_ang, B * K * 4 + 16)); SGS_CUDA_TRY_AT(fn, R.regrow(&t->d_rk_valid, B * P + 16)); SGS_CUDA_TRY_AT(fn, R.regrow(&t->d_rk_mp, B * K * 4 + 16));
+        SGS_CUDA_TRY_AT(fn, R.regrow(&t->d_rk_n, B * 4 + 16)); SGS_CUDA_TRY_AT(fn, R.regrow(&t->d_rk_kfn, B * 4 + 16)); SGS_CUDA_TRY_AT(fn, R.regrow(&t->d_rk_mpn, B * 4 + 16));
+        SGS_CUDA_TRY_AT(fn, R.regrow(&t->d_rk_nm, B * 4 + 16)); SGS_CUDA_TRY_AT(fn, R.regrow(&t->d_rk_run, B + 16)); SGS_CUDA_TRY_AT(fn, R.regrow(&t->d_rk_T1, B * 64 + 16));
+        SGS_CUDA_TRY_AT(fn, R.regrow(&t->d_rk_T2, B * 64 + 16));
+    }
+    const int F = nframes, cap = t->cap, pc = t->point_cap;
+    // 1. Frame::ComputeBoW (:799, levelsup 4) of the running rows
+    refkf_prep_kernel<<<F, 256, 0, st>>>(a->frame_enable, t->d_cnt2, cap, a->kf_n, pc, a->kf_flags, t->keys_un, t->d_rk_n, t->d_rk_kfn, t->d_rk_run, t->d_rk_valid,
+                                         t->d_rk_ang, a->stats);
+    rc = sgs_bow_transform_batch_device(voc, t->d_desc2, t->d_rk_n, cap, F, 4, t->d_rk_word, t->d_rk_weight, t->d_rk_node, st);
     if (rc != SGS_OK) return rc;
-    // 5. PoseOptimization on last-frame + local-map matches, inlier count
-    po.tcw_in = a->tcw_motion; po.tcw_out = a->tcw_final; po.points2_xyz = a->mp_xyz; po.id_base2 = t->point_cap; po.point2_cap = a->mp_cap;
+    // 2. ORBmatcher(0.7, true).SearchByBoW(mpReferenceKF, mCurrentFrame, vpMapPointMatches) (:803-806)
+    sgs_bow_batch bw;
+    std::memset(&bw, 0, sizeof bw);
+    bw.kf_node = a->kf_node; bw.kf_weight = a->kf_weight; bw.kf_valid = t->d_rk_valid; bw.kf_desc = a->kf_desc; bw.kf_angle = a->kf_angle; bw.kf_n = t->d_rk_kfn;
+    bw.kf_cap = pc; bw.f_node = t->d_rk_node; bw.f_weight = t->d_rk_weight; bw.f_desc = t->d_desc2; bw.f_angle = t->d_rk_ang; bw.f_n = t->d_rk_n; bw.f_cap = cap;
+    bw.nnratio = 0.7f; bw.check_orientation = 1; bw.match_f = t->d_rk_mp; bw.nmatches = t->d_rk_nm;
+    rc = sgs_match_bow_batch_device(&bw, F, st);
+    if (rc != SGS_OK) return rc;
+    // 3. below 15 matches the row stops (:808-809)
+    refkf_gate_kernel<<<F, 256, 0, st>>>(t->d_rk_nm, a->mp_n, cap, t->d_rk_n, t->d_rk_mpn, t->d_rk_run, a->outlier, a->stats);
+    // 4. mvpMapPoints = the matches, SetPose(mLastFrame.mTcw), PoseOptimization (:811-814)
+    sgs_poseopt_batch po = first_optimization(t, a->tcw_last, t->d_rk_n, t->d_rk_mp, a->kf_xyz, a->inv_level_sigma2, t->d_rk_T1, a->outlier);
     rc = sgs_pose_optimization_batch_device(&po, F, st);
     if (rc != SGS_OK) return rc;
-    chain_final_kernel<<<F, 256, 0, st>>>(t->d_cnt2, cap, t->d_mp, a->outlier, t->d_obs, t->d_nml, a->f_mp, a->stats);
+    // 5-6. discard the outliers (:816-835), then TrackLocalMap as in the pose chain, with the seen_in points left out as well
+    SGS_CUDA_TRY(cudaMemsetAsync(t->d_ncand2, 0, (size_t)F * 8, st));
+    FirstHalf h;
+    h.n = t->d_rk_n; h.run = t->d_rk_run; h.nm = t->d_rk_nm; h.flags = a->kf_flags; h.local_id = a->kf_local_id; h.seen_in = a->seen_in; h.mp = t->d_rk_mp;
+    h.tcw_first = t->d_rk_T1; h.tcw_final = t->d_rk_T2; h.f_mp = a->f_mp; h.stats = a->stats;
+    rc = enqueue_local_half(t, local_map(a, t->d_rk_mpn), h, po, F, st);
+    if (rc != SGS_OK) return rc;
+    refkf_commit_kernel<<<F, 32, 0, st>>>(t->d_rk_run, t->d_rk_T1, t->d_rk_T2, a->tcw_refkf, a->tcw_final);
     SGS_CUDA_TRY(cudaGetLastError());
     return SGS_OK;
 }

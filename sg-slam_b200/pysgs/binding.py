@@ -103,6 +103,16 @@ class PoseChainBatch(C.Structure):          # sgs_posechain_batch
                 ('tcw_motion', C.c_void_p), ('tcw_final', C.c_void_p), ('f_mp', C.c_void_p), ('outlier', C.c_void_p), ('stats', C.c_void_p)]
 
 
+class RefKfBatch(C.Structure):              # sgs_refkf_batch
+    _fields_ = [('kf_node', C.c_void_p), ('kf_weight', C.c_void_p), ('kf_desc', C.c_void_p), ('kf_angle', C.c_void_p), ('kf_xyz', C.c_void_p),
+                ('kf_flags', C.c_void_p), ('kf_n', C.c_void_p), ('kf_local_id', C.c_void_p), ('tcw_last', C.c_void_p), ('frame_enable', C.c_void_p),
+                ('seen_in', C.c_void_p),
+                ('mp_xyz', C.c_void_p), ('mp_normal', C.c_void_p), ('mp_min_dist', C.c_void_p), ('mp_max_dist', C.c_void_p), ('mp_desc', C.c_void_p),
+                ('mp_valid', C.c_void_p), ('mp_obs', C.c_void_p), ('mp_n', C.c_void_p), ('mp_cap', C.c_int32),
+                ('th_local', C.c_float), ('nnratio_local', C.c_float), ('inv_level_sigma2', C.c_float * 16),
+                ('tcw_refkf', C.c_void_p), ('tcw_final', C.c_void_p), ('f_mp', C.c_void_p), ('outlier', C.c_void_p), ('stats', C.c_void_p)]
+
+
 class FuseBatch(C.Structure):
     _fields_ = [('cam', Camera), ('kf_kps', C.c_void_p), ('kf_desc', C.c_void_p), ('kf_uright', C.c_void_p), ('kf_n', C.c_void_p), ('kf_cap', C.c_int32),
                 ('tcw', C.c_void_p), ('ow', C.c_void_p), ('mp_xyz', C.c_void_p), ('mp_normal', C.c_void_p), ('mp_min_dist', C.c_void_p), ('mp_max_dist', C.c_void_p),
