@@ -162,6 +162,20 @@ struct TcGeom {
     int coalesce;                 // contiguous [pixel][channel] output (frame_stride == HW * pitch): a pixel's row address needs no division by HW
 };
 
+#ifdef SGS_GEMM_TRACE
+// Probe build only (tools/gemm_tile_trace.py): clock64() stamps of the first kTraceTiles tiles of CTA (0, 0), by role (consumer warpgroup 0, 1,
+// producer) and CTA-local tile: TR_START tile start, TR_RING clocks spent in ring waits (summed over the tile's k-blocks), TR_ISSUED last wgmma
+// issued, TR_DRAINED its wait_group returned, TR_EPI_END epilogue done, TR_KWAIT clocks in the k-loop's wait_group (summed).
+constexpr int kTraceTiles = 16;
+enum { TR_START, TR_RING, TR_ISSUED, TR_DRAINED, TR_EPI_END, TR_KWAIT, TR_EVENTS };
+__device__ long long g_gemm_trace[3][kTraceTiles][TR_EVENTS];
+#define SGS_STAMP() clock64()
+#define SGS_TRACE(on, role, tile, ev, v) do { if ((on) && blockIdx.x == 0 && blockIdx.y == 0 && (tile) < kTraceTiles) g_gemm_trace[role][tile][ev] = (v); } while (0)
+#else
+#define SGS_STAMP() 0ll
+#define SGS_TRACE(on, role, tile, ev, v) do { } while (0)
+#endif
+
 // Persistent, warp-specialised.  CTA (x, y) owns output-channel tile y and walks the pixel tiles x, x + gridDim.x, ...
 //   warps 0-3, 4-7 : consumer warpgroups (pixels 0-63 / 64-127 of the tile): split the activation fragments, issue the wgmma, run the epilogue
 //   warps 8-11     : producer warpgroup, registers handed to the consumers (setmaxnreg); one thread issues the TMA loads of the activation k-blocks (and of the weight k-blocks unless resident) into a ring of `stages` slots
@@ -219,10 +233,14 @@ __global__ void __launch_bounds__(kThreads, ctas_per_sm<NC>()) conv1x1_tc_kernel
             }
             uint32_t g = 0;
             for (int it = 0; it < my_tiles; ++it) {
+                SGS_TRACE(true, 2, it, TR_START, SGS_STAMP());
+                long long ring_wait = 0;
                 const int m0 = ((int)blockIdx.x + it * (int)gridDim.x) * kBM;
                 for (int kb = 0; kb < G.KB; ++kb, ++g) {
                     const uint32_t s = g % (uint32_t)G.stages, ph = (g / (uint32_t)G.stages) & 1u;
+                    const long long w0 = SGS_STAMP();
                     mbar_wait(smem_addr(&s_empty[s]), ph ^ 1u);
+                    ring_wait += SGS_STAMP() - w0;
                     const uint32_t st = sbase + s * stage_bytes, bar = smem_addr(&s_full[s]);
                     mbar_expect_tx(bar, a_bytes + (G.b_resident ? 0u : 2 * b_bytes));
                     tma_load_2d(st, &mapA, kb * BKT, m0, bar);
@@ -231,6 +249,8 @@ __global__ void __launch_bounds__(kThreads, ctas_per_sm<NC>()) conv1x1_tc_kernel
                         tma_load_2d(st + a_bytes + b_bytes, &mapBl, kb * BKT, n0, bar);
                     }
                 }
+                SGS_TRACE(true, 2, it, TR_RING, ring_wait);
+                SGS_TRACE(true, 2, it, TR_ISSUED, SGS_STAMP());
             }
         }
         return;
@@ -243,17 +263,23 @@ __global__ void __launch_bounds__(kThreads, ctas_per_sm<NC>()) conv1x1_tc_kernel
     const int wg = warp >> 2, g = lane >> 2, t = lane & 3;
     const int r0 = 64 * wg + 16 * (warp & 3) + g;                            // tile row of fragment rows 0 (and r0 + 8)
     const int ncol = min(NT, G.Cout - n0);                                   // real output channels of this tile (uniform)
+    const bool tr = (tid & 127) == 0;                                         // the warpgroup's trace thread (probe build only)
+    (void)tr;
     // bias of channel n0 + 2t + d at bias_t[d]: the epilogue's loads then differ by constant offsets (one base address, not one per channel pair)
     const float* bias_t = bias ? bias + n0 + 2 * t : nullptr;
     if (G.b_resident) mbar_wait(smem_addr(&s_bfull), 0);
     float acc[NT / 2];
     uint32_t g_ring = 0;
     for (int it = 0; it < my_tiles; ++it) {
+        SGS_TRACE(tr, wg, it, TR_START, SGS_STAMP());
+        long long ring_wait = 0, k_wait = 0, issued = 0;
 #pragma unroll
         for (int i = 0; i < NT / 2; ++i) acc[i] = 0.f;
         for (int kb = 0; kb < G.KB; ++kb, ++g_ring) {
             const uint32_t s = g_ring % (uint32_t)G.stages, ph = (g_ring / (uint32_t)G.stages) & 1u;
+            const long long w0 = SGS_STAMP();
             mbar_wait(smem_addr(&s_full[s]), ph);
+            ring_wait += SGS_STAMP() - w0;
             const uint8_t* sa = gbase + (size_t)s * stage_bytes;
             const uint32_t bh0 = G.b_resident ? bres + (uint32_t)kb * 2 * b_bytes : sbase + s * stage_bytes + a_bytes;
             const int ksteps = min(BKT, G.Cin - kb * BKT + 7) >> 3;          // 8-wide k-steps that hold real channels (the rest is zero fill)
@@ -280,12 +306,21 @@ __global__ void __launch_bounds__(kThreads, ctas_per_sm<NC>()) conv1x1_tc_kernel
                 }
             }
             wgmma_commit();
+            issued = SGS_STAMP();
             wgmma_wait_all();
+            k_wait += SGS_STAMP() - issued;
             __syncwarp();
             if (lane == 0) mbar_arrive(smem_addr(&s_empty[s]));              // this warp's MMAs on slot s are complete
         }
+        SGS_TRACE(tr, wg, it, TR_ISSUED, issued);
+        SGS_TRACE(tr, wg, it, TR_DRAINED, SGS_STAMP());
+        SGS_TRACE(tr, wg, it, TR_RING, ring_wait);
+        SGS_TRACE(tr, wg, it, TR_KWAIT, k_wait);
 
         // ------------------------------------------------------------------------------------------------ epilogue
+        // Wide tiles load the bias of a chunk's 8 channels of this thread before the chunk's first store, so the 8 loads are in flight together.
+        // (Loaded at each use, behind the branches on the column, every load's latency stood between two stores: the epilogue of a 128 x 256
+        // tile took 7 x its MMAs, DESIGN.md section 6.)  Narrow tiles load at each use: their 80 registers leave no room for the 8 values.
         const int pt = ((int)blockIdx.x + it * (int)gridDim.x) * kBM + r0;
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
@@ -298,19 +333,30 @@ __global__ void __launch_bounds__(kThreads, ctas_per_sm<NC>()) conv1x1_tc_kernel
 #pragma unroll
             for (int c = 0; c < NC; ++c) {
                 if (c * kWN >= ncol) break;
+                float bc[8];                                                 // bias of channels 8j + 2t + q, j = 4c .. 4c + 3, at bc[2(j - 4c) + q]
+                if constexpr (kSplitRegs) {
+#pragma unroll
+                    for (int i = 0; i < 8; ++i) {
+                        const int j = 4 * c + i / 2, q = i & 1;
+                        bc[i] = bias_t && 8 * j + 2 * t + q < ncol ? __ldg(bias_t + 8 * j + q) : 0.f;
+                    }
+                }
+                auto bias_of = [&](int j, int q) {
+                    if constexpr (kSplitRegs) return bc[2 * (j - 4 * c) + q];
+                    else return bias_t ? __ldg(bias_t + 8 * j + q) : 0.f;
+                };
 #pragma unroll
                 for (int j = 4 * c; j < 4 * c + 4; ++j) {                      // 8-channel groups of the 32-channel chunk c
                     const int col = 8 * j + 2 * t;
                     if (col + 1 < ncol && G.vec_ok) {
-                        float v[2] = {__fadd_rn(acc[4 * j + 2 * h], bias_t ? __ldg(bias_t + 8 * j) : 0.f),
-                                      __fadd_rn(acc[4 * j + 2 * h + 1], bias_t ? __ldg(bias_t + 8 * j + 1) : 0.f)};
+                        float v[2] = {__fadd_rn(acc[4 * j + 2 * h], bias_of(j, 0)), __fadd_rn(acc[4 * j + 2 * h + 1], bias_of(j, 1))};
                         epi.template run<2>(v, idx + col);
                         *reinterpret_cast<float2*>(o + col) = make_float2(v[0], v[1]);
                     } else {
 #pragma unroll
                         for (int q = 0; q < 2; ++q) {
                             if (col + q < ncol) {
-                                float one[1] = {__fadd_rn(acc[4 * j + 2 * h + q], bias_t ? __ldg(bias_t + 8 * j + q) : 0.f)};
+                                float one[1] = {__fadd_rn(acc[4 * j + 2 * h + q], bias_of(j, q))};
                                 epi.template run<1>(one, idx + col + q);
                                 o[col + q] = one[0];
                             }
@@ -319,8 +365,11 @@ __global__ void __launch_bounds__(kThreads, ctas_per_sm<NC>()) conv1x1_tc_kernel
                 }
             }
         }
+        SGS_TRACE(tr, wg, it, TR_EPI_END, SGS_STAMP());
     }
 }
+#undef SGS_TRACE
+#undef SGS_STAMP
 
 // ---------------------------------------------------------------------------------------------------------------- host side
 typedef CUresult (*PFN_tmap_encode)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*, const cuuint32_t*, const cuuint32_t*,
