@@ -713,7 +713,10 @@ typedef struct sgs_object2d {   /* Object2D, include/Detector2D.h:29-37 (name = 
 /* Detector2D::Detector2D(detection_confidence_threshold, dynamic_detection_confidence_threshold) + load_param/load_model.
  * max_frames = largest batch one sgs_detector_detect_device call may carry.  flags: bit 0 = diagnostic mode (every layer its own kernel,
  * every intermediate blob kept, readable with sgs_detector_blob); bit 1 = plan only (parse, shapes, kernel list and activation pool are
- * built, no device is touched; the handle serves sgs_detector_info / sgs_detector_describe only).
+ * built, no device is touched; the handle serves sgs_detector_info / sgs_detector_describe only); bit 2 = test hook: the fused schedule of
+ * flags 0 (same kernels, tails and concatenation-direct heads) with every materialised blob in a buffer of its own, readable with
+ * sgs_detector_blob -- it holds every blob at once, so it is not a mode to run a detector in (blobs absorbed into a tail and head outputs written
+ * straight into a concatenation have no buffer and stay unreadable).
  * The 1x1 convolutions (90 % of the MACs) run as a TMA-fed wgmma GEMM on [frame][h][w][c] activations with error-compensated TF32 operands
  * (three wgmma per 8-wide k-step, FP32 accumulate: ~1e-6 relative); there is no other GEMM path. */
 SGS_API int sgs_detector_create(const char* param_path, const char* bin_path, int max_frames, float detection_confidence_threshold,
@@ -846,7 +849,7 @@ SGS_API int sgs_detector_describe(const sgs_detector* d, char* out, int64_t cap,
  * over ncalls completed calls.  Costs one event per kernel: leave it off in production. */
 SGS_API int sgs_detector_set_profiling(sgs_detector* d, int enable);
 SGS_API int sgs_detector_kernel_times(sgs_detector* d, double* ms_total, int cap, int* nkernels, int* ncalls);
-/* Diagnostics: copies blob `name` of frame `frame` of the last batch to host floats (ncnn memory order c,h,w).  Needs flags bit 0. */
+/* Diagnostics: copies blob `name` of frame `frame` of the last batch to host floats (ncnn memory order c,h,w).  Needs flags bit 0 or 2. */
 SGS_API int sgs_detector_blob(sgs_detector* d, const char* name, int frame, float* out, int64_t cap, int64_t* n);
 
 #ifdef __cplusplus

@@ -858,6 +858,7 @@ int build_graph(sgs_detector* D) {
     };
     auto set3 = [](Blob& b, int c, int h, int w) { b.dims = 3; b.c = c; b.h = h; b.w = w; b.n = (int64_t)c * h * w; };
     const bool diag = D->flags & 1;
+    const bool keep = D->flags & 5;            // every materialised blob keeps its own buffer (diagnostic mode, or the fused schedule with bit 2)
     // consumers per blob (by layer index)
     std::vector<std::vector<int>> cons;
     std::vector<std::vector<int>> lin(Ls.size()), lout(Ls.size());
@@ -1104,7 +1105,7 @@ int build_graph(sgs_detector* D) {
         for (size_t q = 0; q < free_list.size(); ++q)
             if (D->pool_size[free_list[q]] >= n && (best < 0 || D->pool_size[free_list[q]] < D->pool_size[free_list[best]])) best = (int)q;
         if (best >= 0) { const int b = free_list[best]; free_list.erase(free_list.begin() + best); return b; }
-        if (!free_list.empty() && !diag) {        // grow the largest free buffer instead of adding one
+        if (!free_list.empty() && !keep) {        // grow the largest free buffer instead of adding one
             int big = 0;
             for (size_t q = 1; q < free_list.size(); ++q) if (D->pool_size[free_list[q]] > D->pool_size[free_list[big]]) big = (int)q;
             const int b = free_list[big]; free_list.erase(free_list.begin() + big); D->pool_size[b] = n; return b;
@@ -1116,7 +1117,7 @@ int build_graph(sgs_detector* D) {
     for (size_t q = 0; q < D->ops.size(); ++q) {
         const int r = root_of(*D, D->ops[q].out);
         if (B[r].buf < 0) B[r].buf = acquire(B[r].n);
-        if (diag) continue;
+        if (keep) continue;
         // buffers whose last reader is this kernel go back to the pool (after it: in/out never alias)
         for (size_t b = 0; b < B.size(); ++b)
             if (B[b].root == (int)b && B[b].buf >= 0 && last[b] == (int)q) free_list.push_back(B[b].buf);
@@ -1370,7 +1371,7 @@ int sgs_detector_describe(const sgs_detector* D, char* out, int64_t cap, int64_t
 
 int sgs_detector_blob(sgs_detector* D, const char* name, int frame, float* out, int64_t cap, int64_t* n) {
     if (!D || !name || !n) { set_error("sgs_detector_blob: bad argument"); return SGS_ERR_INVALID; }
-    if (!(D->flags & 1)) { set_error("sgs_detector_blob: the handle was not created in diagnostic mode (flags bit 0)"); return SGS_ERR_UNSUPPORTED; }
+    if (!(D->flags & 5)) { set_error("sgs_detector_blob: the handle keeps no blobs (flags bit 0 or 2)"); return SGS_ERR_UNSUPPORTED; }
     auto it = D->blob_id.find(name);
     if (it == D->blob_id.end()) { set_error("sgs_detector_blob: no blob named %s", name); return SGS_ERR_INVALID; }
     const Blob& b = D->blobs[it->second];

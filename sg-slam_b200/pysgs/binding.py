@@ -530,7 +530,7 @@ def memcpy_d2h(dst_array, d_ptr):
 
 
 OBJ_DTYPE = np.dtype([('id', '<i4'), ('prob', '<f4'), ('x', '<f4'), ('y', '<f4'), ('w', '<f4'), ('h', '<f4')])   # sgs_object2d
-DET_DIAGNOSTIC, DET_PLAN_ONLY = 1, 2
+DET_DIAGNOSTIC, DET_PLAN_ONLY, DET_KEEP_BLOBS = 1, 2, 4       # DET_KEEP_BLOBS: fused schedule, every materialised blob kept (a test hook)
 
 
 class Detector(_Handle):

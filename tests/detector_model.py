@@ -258,6 +258,149 @@ def write_tail_model(dirpath, seed=0, name='tails'):
     return pp, bp
 
 
+TAIL_KINDS = ('relu', 'clip', 'hswish', 'add', 'se_gate', 'se_tail', 'generic')      # the tails make_epi recognises, and its generic chain
+TENSOR_TAILS = ('add', 'se_gate', 'se_tail')                                        # the kinds that read same-shape operand tensors
+
+
+def _wide_tail_cases():
+    """Cases (kind, cin, cout, hw) of write_wide_tail_model, planned at PROBE_FRAMES frames per batch (plan_tiling's cost model, one H100 of 132 SMs):
+      grid    every kind at every tile width NT = 32 ... 256 with Cin 40 (two 32-float k-blocks, the second partial): Cout <= 128 on the 19x19 map (one
+              N-tile of roundup32(Cout), 23 pixel tiles), Cout 129-256 on 38x38 (91 pixel tiles: one N-tile of roundup32(Cout) is cheaper than two);
+              Cout = NT or NT - 4 (a partial last 8-channel group) in a checkerboard over (kind, NT);
+      Cin 16  (16-float k-blocks) ReLU at NT 32 and 64 and +tensor at NT 32 (the reference model has these), clip at 128, hard-swish at 256, the
+              generic chain at 192, and three of the cases below;
+      extras  streamed weights (Cin 96: 3 k-blocks of 2 x NT x 32 floats > 128 KB) under hard-swish (NT 256) and the SE tail (NT 224); each tensor kind
+              on Cout 400 at 38x38 (two N-tiles of 224, 176 real channels in the second: its chunk 6 is cut off) and on the odd Cout 161 (NT 192,
+              scalar stores); hard-swish on Cout 1000 at 10x10 (eight N-tiles of 128, the last with 104 channels); the SE tail on 75x75 (352 pixel
+              tiles: several per persistent CTA).  Every map leaves a partial last pixel tile (8 * hw^2 is not a multiple of 128)."""
+    cases = []
+    for i, kind in enumerate(TAIL_KINDS):
+        for j in range(8):
+            nt = 32 * (j + 1)
+            cases.append((kind, 40, nt - 4 if (i + j) % 2 else nt, 19 if nt <= 128 else 38))
+    cases += [('relu', 16, 30, 19), ('relu', 16, 64, 19), ('add', 16, 32, 19), ('clip', 16, 124, 19), ('hswish', 16, 252, 38), ('generic', 16, 190, 38),
+              ('hswish', 96, 256, 38), ('se_tail', 96, 224, 38), ('add', 40, 400, 38), ('se_gate', 16, 400, 38), ('se_tail', 40, 400, 38),
+              ('add', 16, 161, 38), ('se_gate', 40, 161, 38), ('se_tail', 16, 161, 38), ('hswish', 40, 1000, 10), ('se_tail', 40, 96, 75)]
+    return cases
+
+
+WIDE_TAIL_CASES = _wide_tail_cases()
+
+
+def write_wide_tail_model(dirpath, seed=0, cases=WIDE_TAIL_CASES, name='wide_tails'):
+    """Fused element-wise tails on 1x1 GEMMs of chosen shapes, for the fused == per-layer and float32 restatement checks of
+    tests/test_gpu_detector_fused_tails.py.  The trunk is write_probe_model's (3x3/s2 stem 3 -> 16 with per-channel gains, depth-wise 3x3/s2 chain);
+    a feed of `cin` channels at map `hw` is the chain map itself (cin 16) or one dense 1x1 expansion 16 -> cin, shared by every case on it.  Each
+    case (kind, cin, cout, hw) hangs a dense 1x1 GEMM y = W x + b (cin -> cout) off its feed and puts the tail after it, as ncnn exports it:
+      relu     ReLU(y)                      clip     Clip(y, 0, 6)                  hswish   y * Clip(y + 3, 0, 6) / 6
+      add      y + t1                       se_gate  t1 * (Clip(y + 3, 0, 6) / 6)   se_tail  t1 * (Clip(y + 3, 0, 6) / 6) + t2
+      generic  ReLU(y * 0.5)
+    t1, t2: further dense 1x1 convolutions cin -> cout of the same feed, written before y so that they exist when y's GEMM runs.  Each tail output
+    is a dead end; write_probe_model's minimal SSD head on the 19x19 map closes the graph.
+    Returns (param path, bin path, info, head): info[i] = dict(kind, cin, cout, hw, x (feed blob), y (the GEMM's output blob), ops (operand blobs
+    t1, t2), out (the tail's final blob), w ([cout][cin] float32), b) of cases[i]; head = the output blobs of the head convolutions."""
+    g = Graph(seed)
+    data = g.add('Input', [], name='input')
+    ws = (g.rng.standard_normal((16, 3, 3, 3)) * np.sqrt(2.0 / 27) * np.exp2(g.rng.uniform(-3, 3, (16, 1, 1, 1))) / 64).astype(np.float32)
+    chain = {150: g.conv(data, 3, 16, 3, 2, 1, w=ws)}
+    smallest = min([19] + [c[3] for c in cases])
+    for a, bsz in zip(CHAIN, CHAIN[1:]):
+        if bsz < smallest:
+            break
+        chain[bsz] = g.conv(chain[a], 16, 16, 3, 2, 1, dw=True, gain=1.5)
+    feeds = {}
+
+    def feed(cin, hw):
+        if (cin, hw) not in feeds:
+            feeds[(cin, hw)] = chain[hw] if cin == 16 else g.conv(chain[hw], 16, cin)
+        return feeds[(cin, hw)]
+
+    def hsig(y):
+        return g.binop(g.clip(g.binop(y, g.const(3.0), 0)), g.const(6.0), 3)
+
+    info = []
+    for kind, cin, cout, hw in cases:
+        x = feed(cin, hw)
+        ops = [g.conv(x, cin, cout) for _ in range({'add': 1, 'se_gate': 1, 'se_tail': 2}.get(kind, 0))]
+        y = g.conv(x, cin, cout, name=g.name('wide_%s_' % kind))
+        w, b = g.layers[-1][5][1].reshape(cout, cin), g.layers[-1][5][2]
+        if kind == 'relu':
+            out = g.relu(y)
+        elif kind == 'clip':
+            out = g.clip(y)
+        elif kind == 'hswish':
+            out = g.hswish(y)
+        elif kind == 'add':
+            out = g.binop(y, ops[0], 0)
+        elif kind == 'se_gate':
+            out = g.binop(ops[0], hsig(y), 2)
+        elif kind == 'se_tail':
+            out = g.binop(g.binop(ops[0], hsig(y), 2), ops[1], 0)
+        elif kind == 'generic':
+            out = g.relu(g.binop(y, g.const(0.5), 2))
+        else:
+            raise ValueError(kind)
+        info.append(dict(kind=kind, cin=cin, cout=cout, hw=hw, x=x, y=y, ops=ops, out=out, w=w, b=b))
+    n0 = len(g.layers)
+    _head(g, data, [(chain[19], 16)], 4, '-23300=1,60.000000 -23301=1,105.0 -23302=1,2.000000 7=1')
+    head = [L[3][0] for L in g.layers[n0:] if L[0] == 'Convolution']
+    os.makedirs(dirpath, exist_ok=True)
+    pp, bp = os.path.join(dirpath, name + '.param'), os.path.join(dirpath, name + '.bin')
+    g.write(pp, bp)
+    return pp, bp, info, head
+
+
+def plan_tails(describe_text):
+    """parse_plan of describe_text, each line with 'steps' (the fused element-wise steps after ' | ': (op, rev, src, value) with src 'scalar' /
+    'start' / 'tensor', value the scalar, the clip bounds or the operand blob) and 'kind': make_epi's classification of the steps (detector.cu) --
+    'none', one of TAIL_KINDS.  Like make_epi it ignores (rev) on add and mul, and takes the hard-swish / hard-sigmoid forms only with the divisor 6
+    and an un-reversed division."""
+    out = []
+    for p in parse_plan(describe_text):
+        steps = []
+        for s in p['line'].split(' | ')[1:]:
+            t = s.split()
+            op, rev = t[0].replace('(rev)', ''), t[0].endswith('(rev)')
+            if op in ('relu', 'clip'):
+                steps.append((op, rev, None, tuple(float(v) for v in t[1:])))
+            elif t[1] == 'start':
+                steps.append((op, rev, 'start', None))
+            elif len(t) == 4 and t[2] == 'buf':                  # '<blob> buf <n>' (blob names may be numbers)
+                steps.append((op, rev, 'tensor', t[1]))
+            else:
+                steps.append((op, rev, 'scalar', float(t[1])))
+        p['steps'] = steps
+        p['kind'] = epi_kind(steps)
+        out.append(p)
+    return out
+
+
+def epi_kind(steps):
+    """make_epi's tail kind of the (op, rev, src, value) steps of plan_tails"""
+    def is_(i, op, src=None):
+        return steps[i][0] == op and (src is None or steps[i][2] == src)
+
+    def div6(i):
+        return is_(i, 'div', 'scalar') and not steps[i][1] and steps[i][3] == 6.0
+
+    n = len(steps)
+    if n == 0:
+        return 'none'
+    if n == 1 and is_(0, 'relu'):
+        return 'relu'
+    if n == 1 and is_(0, 'clip'):
+        return 'clip'
+    if n == 1 and is_(0, 'add', 'tensor'):
+        return 'add'
+    if n == 4 and is_(0, 'add', 'scalar') and is_(1, 'clip') and is_(2, 'mul', 'start') and div6(3):
+        return 'hswish'
+    if n == 5 and is_(0, 'add', 'scalar') and is_(1, 'clip') and div6(2) and is_(3, 'mul', 'tensor') and is_(4, 'add', 'tensor'):
+        return 'se_tail'
+    if n == 4 and is_(0, 'add', 'scalar') and is_(1, 'clip') and div6(2) and is_(3, 'mul', 'tensor'):
+        return 'se_gate'
+    return 'generic'
+
+
 # GEMM shapes (cin, cout, map) for the parity tests, at PROBE_FRAMES frames per batch: BK = 16 (cin <= 16) and 32 with a partial last k-step /
 # k-block (20, 36, 100, 964), streamed weights with more k-blocks than ring stages (960, 964), cout < 32 and odd (1, 21, 63: scalar stores),
 # an exact tile (32, 256), one channel past a tile (257), several output-channel tiles (600, 1000), 1 / 4 / 25 / 9 pixels per frame, and
