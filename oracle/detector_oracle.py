@@ -20,25 +20,38 @@ MEAN = (123.675, 116.28, 103.53)               # Detector2D.h:71 (norm_vals are 
 PERSON = 15                                    # Detector2D.cc:74
 
 
-def resize_bilinear_u8c3(img, dw, dh):
+def round_half_even(v):
+    """saturate_cast<short>(float) as cv2 computes it (cvRound: round half to even)"""
+    return int(np.rint(v))
+
+
+def round_half_away(v):
+    """round half away from zero: the convention a +-0.5-and-truncate cast gives (the one ncnn's rounding would follow if it works that way; unverified)"""
+    return int(math.copysign(math.floor(abs(v) + 0.5), v))
+
+
+def resize_coeffs(dn, sn, rnd=round_half_even):
+    """The resize's coefficients along one axis of sn source and dn destination pixels: (source index [dn], 11-bit weights [dn][2]) as int64.
+    rnd rounds the float32 products weight * 2048 to an integer."""
+    scale = sn / dn
+    idx = np.zeros(dn, np.int64); a = np.zeros((dn, 2), np.int64)
+    for d in range(dn):
+        f = np.float32((d + 0.5) * scale - 0.5)
+        s = int(math.floor(f)); f = np.float32(f - s)
+        if s < 0: s, f = 0, np.float32(0)
+        if s >= sn - 1: s, f = sn - 2, np.float32(1)
+        idx[d] = s
+        sat = lambda v: max(-32768, min(32767, rnd(float(v))))     # noqa: E731
+        a[d, 0] = sat((np.float32(1) - f) * np.float32(2048)); a[d, 1] = sat(f * np.float32(2048))
+    return idx, a
+
+
+def resize_bilinear_u8c3(img, dw, dh, rnd=round_half_even):
     """Mat::from_pixels_resize (Detector2D.cc:39): fixed-point bilinear, 11-bit coefficients, the same arithmetic as cv::resize INTER_LINEAR
-    on 8-bit data: horizontal pass keeps value*2048, vertical pass is ((b0*(r0>>4))>>16) + ((b1*(r1>>4))>>16) + 2) >> 2."""
+    on 8-bit data: horizontal pass keeps value*2048, vertical pass is ((b0*(r0>>4))>>16) + ((b1*(r1>>4))>>16) + 2) >> 2.
+    rnd: the rounding of the coefficients (resize_coeffs); the default is cv2's."""
     sh, sw, ch = img.shape
-    def coeffs(dn, sn):
-        scale = sn / dn
-        idx = np.zeros(dn, np.int64); a = np.zeros((dn, 2), np.int64)
-        for d in range(dn):
-            f = np.float32((d + 0.5) * scale - 0.5)
-            s = int(math.floor(f)); f = np.float32(f - s)
-            if s < 0: s, f = 0, np.float32(0)
-            if s >= sn - 1: s, f = sn - 2, np.float32(1)
-            idx[d] = s
-            def sat(v):
-                v = float(v); r = int(np.rint(v))        # saturate_cast<short>(float): round half to even
-                return max(-32768, min(32767, r))
-            a[d, 0] = sat((np.float32(1) - f) * np.float32(2048)); a[d, 1] = sat(f * np.float32(2048))
-        return idx, a
-    xi, xa = coeffs(dw, sw); yi, ya = coeffs(dh, sh)
+    xi, xa = resize_coeffs(dw, sw, rnd); yi, ya = resize_coeffs(dh, sh, rnd)
     src = img.astype(np.int64)
     rows = src[:, xi, :] * xa[None, :, 0, None] + src[:, xi + 1, :] * xa[None, :, 1, None]      # sh x dw x ch, scaled by 2048
     r0 = rows[yi] >> 4; r1 = rows[yi + 1] >> 4
@@ -46,9 +59,9 @@ def resize_bilinear_u8c3(img, dw, dh):
     return np.clip(out, 0, 255).astype(np.uint8)
 
 
-def preprocess(rgb):
+def preprocess(rgb, rnd=round_half_even):
     """u8 HxWx3 -> float32 3x300x300, mean-subtracted (Detector2D.cc:39-40).  Channel order is kept as given (PIXEL_RGB = no swap)."""
-    small = resize_bilinear_u8c3(rgb, TARGET, TARGET)
+    small = resize_bilinear_u8c3(rgb, TARGET, TARGET, rnd)
     x = small.astype(np.float32).transpose(2, 0, 1).copy()
     for c in range(3):
         x[c] = (x[c] - np.float32(MEAN[c])) * np.float32(1.0)

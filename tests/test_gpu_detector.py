@@ -27,13 +27,19 @@ def _run(det, frames, max_boxes=32):
     import torch
     F, H, W, _ = frames.shape
     d = torch.from_numpy(np.ascontiguousarray(frames)).cuda()
+    return _run_ptr(det, d.data_ptr(), H * W * 3, W * 3, W, H, F, max_boxes)
+
+
+def _run_ptr(det, d_rgb, frame_stride, pitch, W, H, F, max_boxes=32):
+    """F frames of W x H at device address d_rgb, frame_stride / pitch bytes apart -> dict of host arrays."""
+    import torch
     R = det.rows_cap
     o = dict(rows=torch.zeros((F, R, 6), device='cuda'), nrows=torch.zeros(F, dtype=torch.int32, device='cuda'),
              objects=torch.zeros((F, R, 6), device='cuda'), nobjects=torch.zeros(F, dtype=torch.int32, device='cuda'),
              dyn_map=torch.zeros((F, max_boxes, 4), device='cuda'), ndyn_map=torch.zeros(F, dtype=torch.int32, device='cuda'),
              dyn_rm=torch.zeros((F, max_boxes, 4), device='cuda'), ndyn_rm=torch.zeros(F, dtype=torch.int32, device='cuda'),
              have=torch.zeros(F, dtype=torch.uint8, device='cuda'), status=torch.zeros(F, dtype=torch.int32, device='cuda'))
-    det.detect_device(d.data_ptr(), H * W * 3, W * 3, W, H, F, *[o[k].data_ptr() for k in
+    det.detect_device(d_rgb, frame_stride, pitch, W, H, F, *[o[k].data_ptr() for k in
                       ('rows', 'nrows', 'objects', 'nobjects', 'dyn_map', 'ndyn_map', 'dyn_rm', 'ndyn_rm', 'have')], max_boxes, o['status'].data_ptr())
     torch.cuda.synchronize()
     out = {k: v.cpu().numpy() for k, v in o.items()}
