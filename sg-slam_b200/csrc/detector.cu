@@ -79,24 +79,11 @@ __device__ __forceinline__ float apply_epi(const Epi& e, float v, int64_t idx) {
     }
 }
 
-// Runs `body` with the tail kind as a compile-time constant: the (block-uniform) switch is taken once per thread, not once per output.
+// Runs `body` with the tail kind as a compile-time constant.  In a kernel the (block-uniform) switch is taken once per thread, not once per output;
+// on the host it picks the GEMM instantiation of the kind.
 template <int KIND> struct EpiKind { static constexpr int value = KIND; };
 template <class F>
-__device__ __forceinline__ void epi_dispatch(int kind, F&& body) {
-    switch (kind) {
-    case EK_NONE: body(EpiKind<EK_NONE>{}); break;
-    case EK_RELU: body(EpiKind<EK_RELU>{}); break;
-    case EK_CLIP: body(EpiKind<EK_CLIP>{}); break;
-    case EK_HSWISH: body(EpiKind<EK_HSWISH>{}); break;
-    case EK_ADD_T: body(EpiKind<EK_ADD_T>{}); break;
-    case EK_SE_TAIL: body(EpiKind<EK_SE_TAIL>{}); break;
-    case EK_SE_MUL: body(EpiKind<EK_SE_MUL>{}); break;
-    default: body(EpiKind<EK_GENERIC>{}); break;
-    }
-}
-
-template <class F>
-inline void epi_dispatch_host(int kind, F&& body) {
+__host__ __device__ __forceinline__ void epi_dispatch(int kind, F&& body) {
     switch (kind) {
     case EK_NONE: body(EpiKind<EK_NONE>{}); break;
     case EK_RELU: body(EpiKind<EK_RELU>{}); break;
@@ -131,6 +118,37 @@ __device__ __forceinline__ void apply_epi4(const Epi& e, float (&v)[4], int64_t 
         for (int q = 0; q < 4; ++q) v[q] = apply_epi<KIND>(e, v[q], idx + q);
     }
 }
+
+// The tail on N consecutive channels v of one pixel, the first at flat index idx0: as float4 groups when N % 4 == 0 and idx0 % 4 == 0, else one
+// channel at a time.  ALIGNED: the caller knows that idx0 % 4 == 0, and the test is not made at run time.
+template <int KIND, bool ALIGNED = false, int N>
+__device__ __forceinline__ void apply_epi_n(const Epi& e, float (&v)[N], int64_t idx0) {
+    static_assert(!ALIGNED || N % 4 == 0, "ALIGNED takes whole float4 groups");
+    if constexpr (N % 4 == 0) {
+        if (ALIGNED || (idx0 & 3) == 0) {
+#pragma unroll
+            for (int q = 0; q < N; q += 4) {
+                float w[4] = {v[q], v[q + 1], v[q + 2], v[q + 3]};
+                apply_epi4<KIND>(e, w, idx0 + q);
+                v[q] = w[0]; v[q + 1] = w[1]; v[q + 2] = w[2]; v[q + 3] = w[3];
+            }
+            return;
+        }
+    }
+    if constexpr (!ALIGNED)
+#pragma unroll
+        for (int q = 0; q < N; ++q) v[q] = apply_epi<KIND>(e, v[q], idx0 + q);
+}
+
+// The tail as the functor conv1x1_tc_kernel takes, with the kind fixed at compile time: one instantiation of the GEMM per kind, so that the epilogue
+// carries the code of one tail only (with a run-time switch every tail is inlined at every call site of the epilogue, and the kernel's code outgrows
+// the instruction cache).
+template <int KIND>
+struct EpiFnK {
+    Epi e;
+    template <int N>
+    __device__ __forceinline__ void run(float (&v)[N], int64_t idx0) const { apply_epi_n<KIND>(e, v, idx0); }
+};
 
 // ---------------------------------------------------------------------------------------------------------------- kernels
 // Mat::from_pixels_resize(..., PIXEL_RGB, w, h, 300, 300) + substract_mean_normalize (norm = 1).  11-bit fixed-point bilinear, the arithmetic
@@ -179,55 +197,6 @@ __global__ void __launch_bounds__(256) preprocess_kernel(const uint8_t* __restri
 
 struct ConvGeom {
     int Cin, Cout, H, W, OH, OW, k, stride, pad, dil;
-};
-
-// The tail of a kernel's epilogue as the functor conv1x1_tc_kernel takes: the (block-uniform) switch on the tail kind is taken once per group of
-// N consecutive channels, the recognised kinds run as straight-line code.
-struct EpiFn {
-    Epi e;
-    template <int N>
-    __device__ __forceinline__ void run(float (&v)[N], int64_t idx0) const {
-        epi_dispatch(e.kind, [&](auto kind) {
-            constexpr int EK = decltype(kind)::value;
-            if constexpr (N % 4 == 0) {
-                if ((idx0 & 3) == 0) {
-#pragma unroll
-                    for (int q = 0; q < N; q += 4) {
-                        float w[4] = {v[q], v[q + 1], v[q + 2], v[q + 3]};
-                        apply_epi4<EK>(e, w, idx0 + q);
-                        v[q] = w[0]; v[q + 1] = w[1]; v[q + 2] = w[2]; v[q + 3] = w[3];
-                    }
-                    return;
-                }
-            }
-#pragma unroll
-            for (int q = 0; q < N; ++q) v[q] = apply_epi<EK>(e, v[q], idx0 + q);
-        });
-    }
-    __host__ __device__ bool reads_tensors() const { return e.kind == EK_ADD_T || e.kind == EK_SE_TAIL || e.kind == EK_SE_MUL || e.kind == EK_GENERIC; }
-};
-
-// The same with the tail kind fixed at compile time: one instantiation of the GEMM per kind, so that the epilogue carries the code of one
-// tail only (with a run-time switch every tail is inlined at every call site of the epilogue, and the kernel's code outgrows the instruction cache).
-template <int KIND>
-struct EpiFnK {
-    Epi e;
-    template <int N>
-    __device__ __forceinline__ void run(float (&v)[N], int64_t idx0) const {
-        if constexpr (N % 4 == 0) {
-            if ((idx0 & 3) == 0) {
-#pragma unroll
-                for (int q = 0; q < N; q += 4) {
-                    float w[4] = {v[q], v[q + 1], v[q + 2], v[q + 3]};
-                    apply_epi4<KIND>(e, w, idx0 + q);
-                    v[q] = w[0]; v[q + 1] = w[1]; v[q + 2] = w[2]; v[q + 3] = w[3];
-                }
-                return;
-            }
-        }
-#pragma unroll
-        for (int q = 0; q < N; ++q) v[q] = apply_epi<KIND>(e, v[q], idx0 + q);
-    }
 };
 
 // depth-wise K x K, stride S on [frame][h][w][c]: V channels (float4 when C % 4 == 0) x XT consecutive outputs of one row per thread; the
@@ -307,11 +276,12 @@ __global__ void __launch_bounds__(256) dwconv_kernel(const float* __restrict__ i
             for (int o = 0; o < XT; ++o) {
                 if (ox0 + o >= g.OW) break;
                 const int64_t oi = o0 + (int64_t)o * g.Cout;
-                if constexpr (V == 4) {
-                    float rr[4] = {__fadd_rn(acc[y][o][0], b[0]), __fadd_rn(acc[y][o][1], b[1]), __fadd_rn(acc[y][o][2], b[2]), __fadd_rn(acc[y][o][3], b[3])};
-                    apply_epi4<EK>(epi, rr, oi);
-                    *reinterpret_cast<float4*>(out + oi) = make_float4(rr[0], rr[1], rr[2], rr[3]);
-                } else out[oi] = apply_epi<EK>(epi, __fadd_rn(acc[y][o][0], b[0]), oi);
+                float r[V];
+#pragma unroll
+                for (int q = 0; q < V; ++q) r[q] = __fadd_rn(acc[y][o][q], b[q]);
+                apply_epi_n<EK, V == 4>(epi, r, oi);                   // V == 4: Cout % 4 == 0 and c % 4 == 0
+                if constexpr (V == 4) *reinterpret_cast<float4*>(out + oi) = make_float4(r[0], r[1], r[2], r[3]);
+                else out[oi] = r[0];
             }
         }
     });
@@ -366,14 +336,16 @@ __global__ void __launch_bounds__(256) conv_small_kernel(const float* __restrict
                 float w[4];
 #pragma unroll
                 for (int q = 0; q < 4; ++q) w[q] = __fadd_rn(acc[o + q], bias ? __ldg(bias + co0 + o + q) : 0.f);
-                apply_epi4<EK>(epi, w, idx0 + co0 + o);
+                apply_epi_n<EK, true>(epi, w, idx0 + co0 + o);         // vec: Cout % 4 == 0 and co0 % 8 == 0
                 *reinterpret_cast<float4*>(orow + co0 + o) = make_float4(w[0], w[1], w[2], w[3]);
             }
         } else {
 #pragma unroll
             for (int o = 0; o < kCot; ++o) {
                 const int co = co0 + o;
-                r[o] = co < g.Cout ? apply_epi<EK>(epi, __fadd_rn(acc[o], bias ? __ldg(bias + co) : 0.f), idx0 + co) : 0.f;
+                float w[1] = {0.f};
+                if (co < g.Cout) { w[0] = __fadd_rn(acc[o], bias ? __ldg(bias + co) : 0.f); apply_epi_n<EK>(epi, w, idx0 + co); }
+                r[o] = w[0];
             }
 #pragma unroll
             for (int o = 0; o < kCot; ++o) if (co0 + o < g.Cout) orow[co0 + o] = r[o];
@@ -431,7 +403,7 @@ __global__ void __launch_bounds__(256) conv_first_kernel(const float* __restrict
             float w[4];
 #pragma unroll
             for (int q = 0; q < 4; ++q) w[q] = __fadd_rn(acc[o + q], bias ? __ldg(bias + o + q) : 0.f);
-            apply_epi4<EK>(epi, w, idx0 + o);
+            apply_epi_n<EK, true>(epi, w, idx0 + o);
             *reinterpret_cast<float4*>(out + idx0 + o) = make_float4(w[0], w[1], w[2], w[3]);
         }
     });
@@ -440,7 +412,11 @@ __global__ void __launch_bounds__(256) conv_first_kernel(const float* __restrict
 __global__ void __launch_bounds__(256) eltwise_kernel(const float* __restrict__ in, float* __restrict__ out, int64_t total, Epi epi) {
     const int64_t idx = (int64_t)blockIdx.x * 256 + threadIdx.x;
     if (idx >= total) return;
-    epi_dispatch(epi.kind, [&](auto kind) { out[idx] = apply_epi<decltype(kind)::value>(epi, __ldg(in + idx), idx); });
+    epi_dispatch(epi.kind, [&](auto kind) {
+        float v[1] = {__ldg(in + idx)};
+        apply_epi_n<decltype(kind)::value>(epi, v, idx);
+        out[idx] = v[0];
+    });
 }
 
 // Concat piece: per frame n floats from src (frame stride n) to dst + off (frame stride dst_n)
@@ -845,8 +821,16 @@ int upload(sgs_detector* D, const std::vector<float>& h, float** d) {
     return SGS_OK;
 }
 
-// Shapes, constant folding, kernel list with fused element-wise tails, liveness-planned activation pool.
-int build_graph(sgs_detector* D) {
+// ---- graph builder.  sgs_detector_create runs wire_graph, infer_shapes, schedule and plan_pool in this order, then allocate unless the handle is
+// plan-only.
+
+// Which blobs each layer reads and writes, and which layers read each blob: set up once from the layer list, read by every later step.
+struct Wiring {
+    std::vector<std::vector<int>> in, out;     // blob ids, per layer
+    std::vector<std::vector<int>> readers;     // layer indices, per blob
+};
+
+int wire_graph(sgs_detector* D, Wiring& w) {
     auto& Ls = D->layers;
     auto& B = D->blobs;
     auto blob = [&](const std::string& n) -> int {
@@ -856,177 +840,274 @@ int build_graph(sgs_detector* D) {
         B.push_back(b); D->blob_id[n] = (int)B.size() - 1;
         return (int)B.size() - 1;
     };
-    auto set3 = [](Blob& b, int c, int h, int w) { b.dims = 3; b.c = c; b.h = h; b.w = w; b.n = (int64_t)c * h * w; };
-    const bool diag = D->flags & 1;
-    const bool keep = D->flags & 5;            // every materialised blob keeps its own buffer (diagnostic mode, or the fused schedule with bit 2)
-    // consumers per blob (by layer index)
-    std::vector<std::vector<int>> cons;
-    std::vector<std::vector<int>> lin(Ls.size()), lout(Ls.size());
+    w.in.assign(Ls.size(), {});
+    w.out.assign(Ls.size(), {});
     for (size_t i = 0; i < Ls.size(); ++i) {
         for (auto& n : Ls[i].in) {
             if (!D->blob_id.count(n)) { set_error("sgs_detector_create: layer %s reads undefined blob %s", Ls[i].name.c_str(), n.c_str()); return SGS_ERR_INVALID; }
-            lin[i].push_back(blob(n));
+            w.in[i].push_back(blob(n));
         }
-        for (auto& n : Ls[i].out) { const int b = blob(n); B[b].producer = (int)i; lout[i].push_back(b); }
+        for (auto& n : Ls[i].out) { const int b = blob(n); B[b].producer = (int)i; w.out[i].push_back(b); }
     }
-    cons.assign(B.size(), {});
-    for (size_t i = 0; i < Ls.size(); ++i) for (int b : lin[i]) cons[b].push_back((int)i);
+    w.readers.assign(B.size(), {});
+    for (size_t i = 0; i < Ls.size(); ++i) for (int b : w.in[i]) w.readers[b].push_back((int)i);
+    return SGS_OK;
+}
 
-    // ---- pass 1: shapes, aliases, constants
-    for (size_t i = 0; i < Ls.size(); ++i) {
-        const Layer& L = Ls[i];
-        auto in0 = [&]() -> Blob& { return B[lin[i][0]]; };
-        if (L.type == "Input") { set3(B[lout[i][0]], 3, D->T, D->T); B[lout[i][0]].hwc = true; D->input_blob = lout[i][0]; }
+// ---- shapes, aliases and constants
+void set3(Blob& b, int c, int h, int w) { b.dims = 3; b.c = c; b.h = h; b.w = w; b.n = (int64_t)c * h * w; }
+
+int infer_conv(sgs_detector* D, const Wiring& w, int i) {
+    const Layer& L = D->layers[i];
+    const Blob& s = D->blobs[w.in[i][0]];
+    const int k = L.pi(1, 1), dil = L.pi(2, 1), st = L.pi(3, 1), pad = L.pi(4, 0), cout = L.pi(0, 0);
+    if (s.dims != 3 || L.pi(11, k) != k || L.pi(12, dil) != dil || L.pi(13, st) != st || L.pi(14, pad) != pad || pad < 0) {
+        set_error("sgs_detector_create: layer %s: only square kernels with symmetric explicit padding are supported", L.name.c_str()); return SGS_ERR_UNSUPPORTED; }
+    const int oh = (s.h + 2 * pad - dil * (k - 1) - 1) / st + 1, ow = (s.w + 2 * pad - dil * (k - 1) - 1) / st + 1;
+    Blob& o = D->blobs[w.out[i][0]];
+    set3(o, cout, oh, ow);
+    o.hwc = true;
+    if (!s.hwc) { set_error("sgs_detector_create: layer %s convolves a blob that is not an activation map", L.name.c_str()); return SGS_ERR_UNSUPPORTED; }
+    const bool dw = L.type == "ConvolutionDepthWise";
+    const int group = dw ? L.pi(7, 1) : 1;
+    if (dw && !(group == s.c && cout == s.c && cout <= 65535 && dil == 1 && (k == 3 || k == 5) && (st == 1 || st == 2))) { set_error("sgs_detector_create: layer %s: grouped convolution other than depth-wise 3x3/5x5 with stride 1/2 is not supported", L.name.c_str()); return SGS_ERR_UNSUPPORTED; }
+    const int64_t expect = dw ? (int64_t)cout * k * k : (int64_t)cout * s.c * k * k;
+    if ((int64_t)L.weight.size() != expect) { set_error("sgs_detector_create: layer %s: weight size %zu, expected %lld", L.name.c_str(), L.weight.size(), (long long)expect); return SGS_ERR_INVALID; }
+    return SGS_OK;
+}
+
+int infer_detection_output(sgs_detector* D, const Wiring& w, int i) {
+    const Layer& L = D->layers[i];
+    auto& B = D->blobs;
+    if (w.in[i].size() != 3 || !B[w.in[i][2]].is_const) { set_error("sgs_detector_create: DetectionOutput %s: expects location, confidence and constant prior boxes", L.name.c_str()); return SGS_ERR_UNSUPPORTED; }
+    const Blob& pr = B[w.in[i][2]];
+    DetOutParams& P = D->dp;
+    P.ncls = L.pi(0, 0); P.nms_thr = (float)L.p(1, 0.05); P.nms_topk = L.pi(2, 300); P.keep_topk = L.pi(3, 100); P.conf_thr = (float)L.p(4, 0.5);
+    P.nprior = pr.w / 4;
+    D->loc_blob = w.in[i][0]; D->conf_blob = w.in[i][1];
+    if (B[D->loc_blob].n != (int64_t)P.nprior * 4 || B[D->conf_blob].n != (int64_t)P.nprior * P.ncls || P.ncls < 2 || P.ncls > 256 || P.nprior > kDetSortCap ||
+        P.nms_topk < 1 || P.nms_topk > 1024 || P.keep_topk < 1 || P.keep_topk > 1024 || (int64_t)(P.ncls - 1) * P.nms_topk > kMergeCap) {
+        set_error("sgs_detector_create: DetectionOutput %s: sizes outside what the kernels take (priors %d of at most %d, classes %d)", L.name.c_str(), P.nprior, kDetSortCap, P.ncls); return SGS_ERR_UNSUPPORTED; }
+    std::vector<float> pb(pr.cval.begin(), pr.cval.begin() + pr.w), vr(pr.cval.begin() + pr.w, pr.cval.end());
+    int rc = upload(D, pb, &D->d_prior); if (rc) return rc;
+    rc = upload(D, vr, &D->d_var); if (rc) return rc;
+    Blob& o = B[w.out[i][0]]; o.dims = 2; o.h = P.keep_topk; o.w = 6; o.n = 0;
+    return SGS_OK;
+}
+
+// Every blob's shape for the fixed input; Split / Permute(3) / Flatten / Reshape outputs become aliases (root), constant sub-graphs are folded.
+int infer_shapes(sgs_detector* D, const Wiring& w) {
+    auto& B = D->blobs;
+    for (size_t i = 0; i < D->layers.size(); ++i) {
+        const Layer& L = D->layers[i];
+        auto in0 = [&]() -> Blob& { return B[w.in[i][0]]; };
+        int rc = SGS_OK;
+        if (L.type == "Input") { set3(B[w.out[i][0]], 3, D->T, D->T); B[w.out[i][0]].hwc = true; D->input_blob = w.out[i][0]; }
         else if (L.type == "MemoryData") {
-            Blob& o = B[lout[i][0]];
+            Blob& o = B[w.out[i][0]];
             o.dims = 1; o.w = (int)L.data.size(); o.n = o.w; o.is_const = true; o.cval = L.data;
             if (L.pi(1, 0) > 0 || L.pi(2, 0) > 0 || o.n != 1) { set_error("sgs_detector_create: MemoryData %s: only scalar constants are supported", L.name.c_str()); return SGS_ERR_UNSUPPORTED; }
         } else if (L.type == "Split") {
-            for (int o : lout[i]) { Blob& ob = B[o]; const Blob& s = in0(); ob.dims = s.dims; ob.c = s.c; ob.h = s.h; ob.w = s.w; ob.n = s.n; ob.root = lin[i][0]; ob.is_const = s.is_const; ob.cval = s.cval; ob.hwc = s.hwc; }
-        } else if (L.type == "Convolution" || L.type == "ConvolutionDepthWise") {
-            const Blob& s = in0();
-            const int k = L.pi(1, 1), dil = L.pi(2, 1), st = L.pi(3, 1), pad = L.pi(4, 0), cout = L.pi(0, 0);
-            if (s.dims != 3 || L.pi(11, k) != k || L.pi(12, dil) != dil || L.pi(13, st) != st || L.pi(14, pad) != pad || pad < 0) {
-                set_error("sgs_detector_create: layer %s: only square kernels with symmetric explicit padding are supported", L.name.c_str()); return SGS_ERR_UNSUPPORTED; }
-            const int oh = (s.h + 2 * pad - dil * (k - 1) - 1) / st + 1, ow = (s.w + 2 * pad - dil * (k - 1) - 1) / st + 1;
-            set3(B[lout[i][0]], cout, oh, ow);
-            B[lout[i][0]].hwc = true;
-            if (!s.hwc) { set_error("sgs_detector_create: layer %s convolves a blob that is not an activation map", L.name.c_str()); return SGS_ERR_UNSUPPORTED; }
-            const bool dw = L.type == "ConvolutionDepthWise";
-            const int group = dw ? L.pi(7, 1) : 1;
-            if (dw && !(group == s.c && cout == s.c && cout <= 65535 && dil == 1 && (k == 3 || k == 5) && (st == 1 || st == 2))) { set_error("sgs_detector_create: layer %s: grouped convolution other than depth-wise 3x3/5x5 with stride 1/2 is not supported", L.name.c_str()); return SGS_ERR_UNSUPPORTED; }
-            const int64_t expect = dw ? (int64_t)cout * k * k : (int64_t)cout * s.c * k * k;
-            if ((int64_t)L.weight.size() != expect) { set_error("sgs_detector_create: layer %s: weight size %zu, expected %lld", L.name.c_str(), L.weight.size(), (long long)expect); return SGS_ERR_INVALID; }
-        } else if (is_eltwise(L)) {
-            const Blob& s = in0(); Blob& o = B[lout[i][0]];
+            for (int o : w.out[i]) { Blob& ob = B[o]; const Blob& s = in0(); ob.dims = s.dims; ob.c = s.c; ob.h = s.h; ob.w = s.w; ob.n = s.n; ob.root = w.in[i][0]; ob.is_const = s.is_const; ob.cval = s.cval; ob.hwc = s.hwc; }
+        } else if (L.type == "Convolution" || L.type == "ConvolutionDepthWise") rc = infer_conv(D, w, (int)i);
+        else if (is_eltwise(L)) {
+            const Blob& s = in0(); Blob& o = B[w.out[i][0]];
             o.dims = s.dims; o.c = s.c; o.h = s.h; o.w = s.w; o.n = s.n; o.hwc = s.hwc;
             if (L.type == "BinaryOp") {
-                const Blob& t = B[lin[i][1]];
+                const Blob& t = B[w.in[i][1]];
                 if (s.is_const || !(t.is_const ? t.n == 1 : t.n == s.n)) { set_error("sgs_detector_create: BinaryOp %s: unsupported operand shapes", L.name.c_str()); return SGS_ERR_UNSUPPORTED; }
                 if (L.pi(0, 0) < 0 || L.pi(0, 0) > 3) { set_error("sgs_detector_create: BinaryOp %s: op_type %d not supported", L.name.c_str(), L.pi(0, 0)); return SGS_ERR_UNSUPPORTED; }
             }
-        } else if (L.type == "Permute") {
+        }
+        else if (L.type == "Permute") {
             const Blob& s = in0();
             if (s.dims != 3 || L.pi(0, 0) != 3 || !s.hwc) { set_error("sgs_detector_create: Permute %s: only order_type 3 on 3-D activation maps is supported", L.name.c_str()); return SGS_ERR_UNSUPPORTED; }
-            set3(B[lout[i][0]], s.h, s.w, s.c);
-            B[lout[i][0]].root = lin[i][0];                   // (c,h,w) -> (h,w,c) is how the activation is stored already: an alias, in ncnn's "native" order from here on
+            set3(B[w.out[i][0]], s.h, s.w, s.c);
+            B[w.out[i][0]].root = w.in[i][0];                 // (c,h,w) -> (h,w,c) is how the activation is stored already: an alias, in ncnn's "native" order from here on
         } else if (L.type == "Flatten") {
-            const Blob& s = in0(); Blob& o = B[lout[i][0]];
+            const Blob& s = in0(); Blob& o = B[w.out[i][0]];
             if (s.hwc && s.c > 1 && s.h * s.w > 1) { set_error("sgs_detector_create: Flatten %s of an un-permuted activation map is not supported", L.name.c_str()); return SGS_ERR_UNSUPPORTED; }
-            o.dims = 1; o.w = (int)s.n; o.n = s.n; o.root = lin[i][0]; o.is_const = s.is_const; o.cval = s.cval;
+            o.dims = 1; o.w = (int)s.n; o.n = s.n; o.root = w.in[i][0]; o.is_const = s.is_const; o.cval = s.cval;
         } else if (L.type == "Reshape") {
-            const Blob& s = in0(); Blob& o = B[lout[i][0]];
-            const int w = L.pi(0, -233), h = L.pi(1, -233);
-            if (w <= 0 || L.pi(2, -233) != -233 || (s.hwc && s.c > 1 && s.h * s.w > 1)) { set_error("sgs_detector_create: Reshape %s: unsupported target", L.name.c_str()); return SGS_ERR_UNSUPPORTED; }
-            if (h == -233) { o.dims = 1; o.w = w; } else { o.dims = 2; o.w = w; o.h = h == -1 ? (int)(s.n / w) : h; }
-            o.n = s.n; o.root = lin[i][0];
+            const Blob& s = in0(); Blob& o = B[w.out[i][0]];
+            const int rw = L.pi(0, -233), rh = L.pi(1, -233);
+            if (rw <= 0 || L.pi(2, -233) != -233 || (s.hwc && s.c > 1 && s.h * s.w > 1)) { set_error("sgs_detector_create: Reshape %s: unsupported target", L.name.c_str()); return SGS_ERR_UNSUPPORTED; }
+            if (rh == -233) { o.dims = 1; o.w = rw; } else { o.dims = 2; o.w = rw; o.h = rh == -1 ? (int)(s.n / rw) : rh; }
+            o.n = s.n; o.root = w.in[i][0];
             if ((int64_t)o.w * o.h != s.n) { set_error("sgs_detector_create: Reshape %s: element count mismatch", L.name.c_str()); return SGS_ERR_INVALID; }
         } else if (L.type == "Concat") {
-            Blob& o = B[lout[i][0]];
+            Blob& o = B[w.out[i][0]];
             const Blob& f = in0();
             const int axis = L.pi(0, 0);
             bool all_const = true; int64_t total = 0;
-            for (int b : lin[i]) { all_const = all_const && B[b].is_const; total += B[b].n; }
+            for (int b : w.in[i]) { all_const = all_const && B[b].is_const; total += B[b].n; }
             if (f.dims == 1 && axis == 0) { o.dims = 1; o.w = (int)total; o.n = total; }
             else if (f.dims == 2 && axis == 1 && all_const) {       // rows concatenated along w (prior boxes)
-                o.dims = 2; o.h = f.h; int w = 0; for (int b : lin[i]) w += B[b].w; o.w = w; o.n = (int64_t)o.h * w;
+                o.dims = 2; o.h = f.h; int ow = 0; for (int b : w.in[i]) ow += B[b].w; o.w = ow; o.n = (int64_t)o.h * ow;
             } else { set_error("sgs_detector_create: Concat %s: unsupported axis / rank", L.name.c_str()); return SGS_ERR_UNSUPPORTED; }
             if (all_const) {
                 o.is_const = true; o.cval.resize(o.n);
-                if (o.dims == 1) { int64_t off = 0; for (int b : lin[i]) { std::copy(B[b].cval.begin(), B[b].cval.end(), o.cval.begin() + off); off += B[b].n; } }
-                else for (int r = 0; r < o.h; ++r) { int64_t off = 0; for (int b : lin[i]) { std::copy(B[b].cval.begin() + (int64_t)r * B[b].w, B[b].cval.begin() + (int64_t)(r + 1) * B[b].w, o.cval.begin() + (int64_t)r * o.w + off); off += B[b].w; } }
+                if (o.dims == 1) { int64_t off = 0; for (int b : w.in[i]) { std::copy(B[b].cval.begin(), B[b].cval.end(), o.cval.begin() + off); off += B[b].n; } }
+                else for (int r = 0; r < o.h; ++r) { int64_t off = 0; for (int b : w.in[i]) { std::copy(B[b].cval.begin() + (int64_t)r * B[b].w, B[b].cval.begin() + (int64_t)(r + 1) * B[b].w, o.cval.begin() + (int64_t)r * o.w + off); off += B[b].w; } }
             }
         } else if (L.type == "Softmax") {
-            const Blob& s = in0(); Blob& o = B[lout[i][0]];
+            const Blob& s = in0(); Blob& o = B[w.out[i][0]];
             if (s.dims != 2 || L.pi(0, 0) != 1) { set_error("sgs_detector_create: Softmax %s: only the inner axis of a 2-D blob is supported", L.name.c_str()); return SGS_ERR_UNSUPPORTED; }
             o.dims = 2; o.h = s.h; o.w = s.w; o.n = s.n;
         } else if (L.type == "PriorBox") {
-            const Blob& fm = B[lin[i][0]]; const Blob& im = B[lin[i][1]];
-            Blob& o = B[lout[i][0]];
+            const Blob& fm = B[w.in[i][0]]; const Blob& im = B[w.in[i][1]];
+            Blob& o = B[w.out[i][0]];
             prior_box(L, fm.w, fm.h, im.w, im.h, o.cval);
             o.is_const = true; o.dims = 2; o.h = 2; o.w = (int)(o.cval.size() / 2); o.n = (int64_t)o.cval.size();
-        } else if (L.type == "DetectionOutput") {
-            if (lin[i].size() != 3 || !B[lin[i][2]].is_const) { set_error("sgs_detector_create: DetectionOutput %s: expects location, confidence and constant prior boxes", L.name.c_str()); return SGS_ERR_UNSUPPORTED; }
-            const Blob& pr = B[lin[i][2]];
-            D->dp.ncls = L.pi(0, 0); D->dp.nms_thr = (float)L.p(1, 0.05); D->dp.nms_topk = L.pi(2, 300); D->dp.keep_topk = L.pi(3, 100); D->dp.conf_thr = (float)L.p(4, 0.5);
-            D->dp.nprior = pr.w / 4;
-            D->loc_blob = lin[i][0]; D->conf_blob = lin[i][1];
-            if (B[D->loc_blob].n != (int64_t)D->dp.nprior * 4 || B[D->conf_blob].n != (int64_t)D->dp.nprior * D->dp.ncls || D->dp.ncls < 2 || D->dp.ncls > 256 ||
-                D->dp.nprior > kDetSortCap || D->dp.nms_topk < 1 || D->dp.nms_topk > 1024 || D->dp.keep_topk < 1 || D->dp.keep_topk > 1024 ||
-                (int64_t)(D->dp.ncls - 1) * D->dp.nms_topk > kMergeCap) {
-                set_error("sgs_detector_create: DetectionOutput %s: sizes outside what the kernels take (priors %d of at most %d, classes %d)", L.name.c_str(), D->dp.nprior, kDetSortCap, D->dp.ncls); return SGS_ERR_UNSUPPORTED; }
-            std::vector<float> pb(pr.cval.begin(), pr.cval.begin() + pr.w), vr(pr.cval.begin() + pr.w, pr.cval.end());
-            int rc = upload(D, pb, &D->d_prior); if (rc) return rc;
-            rc = upload(D, vr, &D->d_var); if (rc) return rc;
-            Blob& o = B[lout[i][0]]; o.dims = 2; o.h = D->dp.keep_topk; o.w = 6; o.n = 0;
-        } else { set_error("sgs_detector_create: layer type %s (%s) is not supported", L.type.c_str(), L.name.c_str()); return SGS_ERR_UNSUPPORTED; }
+        } else if (L.type == "DetectionOutput") rc = infer_detection_output(D, w, (int)i);
+        else { set_error("sgs_detector_create: layer type %s (%s) is not supported", L.type.c_str(), L.name.c_str()); return SGS_ERR_UNSUPPORTED; }
+        if (rc) return rc;
     }
     if (D->input_blob < 0 || D->loc_blob < 0) { set_error("sgs_detector_create: the graph has no Input / DetectionOutput layer"); return SGS_ERR_INVALID; }
+    return SGS_OK;
+}
 
-    // ---- pass 2: kernel list.  absorbed[i] = layer i was folded into an earlier kernel's element-wise tail.
-    auto consumers_of_root = [&](int b) {      // layers reading b or any alias of it (aliases never chain through compute layers)
-        std::vector<int> r; const int rb = root_of(*D, b);
-        for (size_t q = 0; q < B.size(); ++q) if (!B[q].is_const && root_of(*D, (int)q) == rb) for (int l : cons[q]) if (Ls[l].type != "Split" && Ls[l].type != "Flatten" && Ls[l].type != "Reshape" && Ls[l].type != "Permute") r.push_back(l);
-        std::sort(r.begin(), r.end());
-        return r;
-    };
-    std::vector<char> absorbed(Ls.size(), 0);
-    auto step_of = [&](int li, int vblob, int start_blob, int owner_layer, EpiStepH& st) -> bool {
-        const Layer& L = Ls[li];
-        st = EpiStepH{0, SRC_SCALAR, 0, 0.f, 0.f, -1};
-        if (L.type == "ReLU") { if (L.p(0, 0.0) != 0.0) return false; st.op = E_RELU; return root_of(*D, lin[li][0]) == root_of(*D, vblob); }
-        if (L.type == "Clip") { st.op = E_CLIP; st.a = (float)L.p(0, -3.4e38); st.b = (float)L.p(1, 3.4e38); return root_of(*D, lin[li][0]) == root_of(*D, vblob); }
-        if (L.type != "BinaryOp") return false;
-        const int a = lin[li][0], b = lin[li][1];
-        const bool va = root_of(*D, a) == root_of(*D, vblob), vb = !B[b].is_const && root_of(*D, b) == root_of(*D, vblob);
-        if (!va && !vb) return false;
-        st.op = L.pi(0, 0);
-        st.rev = va ? 0 : 1;
-        const int o = va ? b : a;
-        if (B[o].is_const) { st.src = SRC_SCALAR; st.a = B[o].cval[0]; return true; }
-        if (start_blob >= 0 && root_of(*D, o) == root_of(*D, start_blob) && root_of(*D, o) != root_of(*D, vblob)) { st.src = SRC_START; return true; }
-        if (va && vb) return false;                                             // x op x: leave to the generic path
-        if (B[root_of(*D, o)].producer < owner_layer) { st.src = SRC_TENSOR; st.tblob = o; return true; }   // already computed when the owner runs
-        return false;
-    };
-    auto build_tail = [&](int owner_layer, int out_blob, std::vector<EpiStepH>& tail, int& final_blob) {
-        // greedy chain, then the longest prefix whose intermediate blobs are read only inside the prefix
-        std::vector<int> chain_layers; std::vector<int> chain_blobs{out_blob};
-        std::vector<EpiStepH> steps;
-        int cur = out_blob;
-        while ((int)steps.size() < kMaxEpi) {
-            int next = -1; EpiStepH st{};
-            for (int l : consumers_of_root(cur)) {
-                if (std::find(chain_layers.begin(), chain_layers.end(), l) != chain_layers.end() || !is_eltwise(Ls[l]) || absorbed[l]) continue;
-                if (step_of(l, cur, out_blob, owner_layer, st)) { next = l; break; }
-            }
-            if (next < 0) break;
-            chain_layers.push_back(next); steps.push_back(st); cur = lout[next][0]; chain_blobs.push_back(cur);
+// ---- scheduling: the kernel list, and which element-wise layers each kernel applies in its epilogue.  absorbed[l]: layer l is a step of an
+// earlier kernel's tail and gets no kernel of its own.
+
+// Layers reading blob b or any alias of it, in graph order (aliases never chain through compute layers).
+std::vector<int> readers_of_root(const sgs_detector& D, const Wiring& w, int b) {
+    std::vector<int> r; const int rb = root_of(D, b);
+    for (size_t q = 0; q < D.blobs.size(); ++q)
+        if (!D.blobs[q].is_const && root_of(D, (int)q) == rb)
+            for (int l : w.readers[q]) { const std::string& t = D.layers[l].type; if (t != "Split" && t != "Flatten" && t != "Reshape" && t != "Permute") r.push_back(l); }
+    std::sort(r.begin(), r.end());
+    return r;
+}
+
+// Layer li as one step of a tail whose running value is vblob, in the kernel of layer owner_layer; false when it cannot be one.  ReLU (slope 0) and
+// Clip of the value are steps.  A BinaryOp is a step when the value is one operand (rev: the second) and the other is a scalar constant
+// (SRC_SCALAR), the tail's start value start_blob when that is not the value itself (SRC_START; -1: no start value), or a tensor whose producer
+// runs before the owner (SRC_TENSOR).  The value combined with itself is not a step.
+bool step_of(const sgs_detector& D, const Wiring& w, int li, int vblob, int start_blob, int owner_layer, EpiStepH& st) {
+    const Layer& L = D.layers[li];
+    const auto& B = D.blobs;
+    st = EpiStepH{0, SRC_SCALAR, 0, 0.f, 0.f, -1};
+    if (L.type == "ReLU") { if (L.p(0, 0.0) != 0.0) return false; st.op = E_RELU; return root_of(D, w.in[li][0]) == root_of(D, vblob); }
+    if (L.type == "Clip") { st.op = E_CLIP; st.a = (float)L.p(0, -3.4e38); st.b = (float)L.p(1, 3.4e38); return root_of(D, w.in[li][0]) == root_of(D, vblob); }
+    if (L.type != "BinaryOp") return false;
+    const int a = w.in[li][0], b = w.in[li][1];
+    const bool va = root_of(D, a) == root_of(D, vblob), vb = !B[b].is_const && root_of(D, b) == root_of(D, vblob);
+    if (!va && !vb) return false;
+    st.op = L.pi(0, 0);
+    st.rev = va ? 0 : 1;
+    const int o = va ? b : a;
+    if (B[o].is_const) { st.src = SRC_SCALAR; st.a = B[o].cval[0]; return true; }
+    if (start_blob >= 0 && root_of(D, o) == root_of(D, start_blob) && root_of(D, o) != root_of(D, vblob)) { st.src = SRC_START; return true; }
+    if (va && vb) return false;                                                 // x op x: leave to the generic path
+    if (B[root_of(D, o)].producer < owner_layer) { st.src = SRC_TENSOR; st.tblob = o; return true; }
+    return false;
+}
+
+// The tail of the convolution owner_layer, whose output is out_blob.  The chain grows greedily: the next step is the first not yet absorbed
+// element-wise reader (in graph order) of the running value that step_of takes, with out_blob as the start value, up to kMaxEpi steps.  The tail
+// is the longest prefix of the chain whose intermediate blobs are read only inside the prefix, so that nothing needs a value the fused kernel does
+// not store.  Marks its layers absorbed; returns the blob the tail's last step writes (out_blob for an empty tail).
+int build_tail(const sgs_detector& D, const Wiring& w, std::vector<char>& absorbed, int owner_layer, int out_blob, std::vector<EpiStepH>& tail) {
+    std::vector<int> chain_layers; std::vector<int> chain_blobs{out_blob};
+    std::vector<EpiStepH> steps;
+    int cur = out_blob;
+    while ((int)steps.size() < kMaxEpi) {
+        int next = -1; EpiStepH st{};
+        for (int l : readers_of_root(D, w, cur)) {
+            if (std::find(chain_layers.begin(), chain_layers.end(), l) != chain_layers.end() || !is_eltwise(D.layers[l]) || absorbed[l]) continue;
+            if (step_of(D, w, l, cur, out_blob, owner_layer, st)) { next = l; break; }
         }
-        int best = 0;
-        for (int m = 1; m <= (int)steps.size(); ++m) {
-            bool ok = true;
-            for (int j = 0; j < m && ok; ++j)
-                for (int l : consumers_of_root(chain_blobs[j]))
-                    if (std::find(chain_layers.begin(), chain_layers.begin() + m, l) == chain_layers.begin() + m) { ok = false; break; }
-            if (ok) best = m;
-        }
-        tail.assign(steps.begin(), steps.begin() + best);
-        for (int j = 0; j < best; ++j) absorbed[chain_layers[j]] = 1;
-        final_blob = chain_blobs[best];
-    };
-    for (size_t i = 0; i < Ls.size(); ++i) {
-        const Layer& L = Ls[i];
-        if (absorbed[i]) continue;
-        if (L.type == "Convolution" || L.type == "ConvolutionDepthWise") {
-            Op op; op.layer = (int)i; op.in = lin[i][0];
-            const Blob& s = B[lin[i][0]]; const Blob& o = B[lout[i][0]];
+        if (next < 0) break;
+        chain_layers.push_back(next); steps.push_back(st); cur = w.out[next][0]; chain_blobs.push_back(cur);
+    }
+    int best = 0;
+    for (int m = 1; m <= (int)steps.size(); ++m) {
+        bool ok = true;
+        for (int j = 0; j < m && ok; ++j)
+            for (int l : readers_of_root(D, w, chain_blobs[j]))
+                if (std::find(chain_layers.begin(), chain_layers.begin() + m, l) == chain_layers.begin() + m) { ok = false; break; }
+        if (ok) best = m;
+    }
+    tail.assign(steps.begin(), steps.begin() + best);
+    for (int j = 0; j < best; ++j) absorbed[chain_layers[j]] = 1;
+    return chain_blobs[best];
+}
+
+// Extends a stand-alone element-wise kernel (layer owner_layer, its output out_blob) by the layers that follow it: while the running value has one
+// reader, and that reader is a not yet absorbed element-wise layer that step_of takes, it becomes the next step, up to kMaxEpi steps in all.  With
+// one reader per value no step ever needs to be cut off again, unlike build_tail.  No step is SRC_START: the start value of a stand-alone chain
+// is its input, which SRC_START does not mean.  Returns the blob the last step writes.
+int eltwise_chain(const sgs_detector& D, const Wiring& w, std::vector<char>& absorbed, int owner_layer, int out_blob, std::vector<EpiStepH>& steps) {
+    int cur = out_blob;
+    EpiStepH st{};
+    while ((int)steps.size() < kMaxEpi) {
+        auto cs = readers_of_root(D, w, cur);
+        if (cs.size() != 1 || !is_eltwise(D.layers[cs[0]]) || absorbed[cs[0]] || !step_of(D, w, cs[0], cur, -1, owner_layer, st)) break;
+        absorbed[cs[0]] = 1; steps.push_back(st); cur = w.out[cs[0]][0];
+    }
+    return cur;
+}
+
+// The tail kinds the kernels run as straight-line code (Epi::kind); each reproduces the generic loop operation for operation (same operand
+// order, one rounding each).
+int epi_kind(const std::vector<EpiStepH>& h) {
+    const int n = (int)h.size();
+    auto is = [&](int i, int op, int src) { return h[i].op == op && (op >= E_CLIP || h[i].src == src); };
+    if (n == 0) return EK_NONE;
+    if (n == 1 && h[0].op == E_RELU) return EK_RELU;
+    if (n == 1 && h[0].op == E_CLIP) return EK_CLIP;
+    if (n == 1 && is(0, E_ADD, SRC_TENSOR)) return EK_ADD_T;                  // addition commutes: rev is irrelevant
+    if (n == 4 && is(0, E_ADD, SRC_SCALAR) && h[1].op == E_CLIP && is(2, E_MUL, SRC_START) && is(3, E_DIV, SRC_SCALAR) && !h[3].rev && h[3].a == 6.0f) return EK_HSWISH;
+    if (n == 5 && is(0, E_ADD, SRC_SCALAR) && h[1].op == E_CLIP && is(2, E_DIV, SRC_SCALAR) && !h[2].rev && h[2].a == 6.0f && is(3, E_MUL, SRC_TENSOR) && is(4, E_ADD, SRC_TENSOR))
+        return EK_SE_TAIL;
+    if (n == 4 && is(0, E_ADD, SRC_SCALAR) && h[1].op == E_CLIP && is(2, E_DIV, SRC_SCALAR) && !h[2].rev && h[2].a == 6.0f && is(3, E_MUL, SRC_TENSOR)) return EK_SE_MUL;
+    return EK_GENERIC;
+}
+
+// The SSD head outputs.  When every piece is the (permuted, flattened) [h][w][c] output of a convolution that nothing else reads, and none of those
+// convolutions' tails reads a tensor, the convolutions write their rows straight into the concatenated buffer; otherwise, and in diagnostic mode,
+// each piece is copied by a kernel of its own.
+void schedule_concat(sgs_detector* D, const Wiring& w, int i) {
+    std::vector<int> prod;
+    bool direct = !(D->flags & 1);
+    for (int b : w.in[i]) {
+        const int r = root_of(*D, b);
+        int q = -1;
+        for (size_t o = 0; o < D->ops.size(); ++o) if (root_of(*D, D->ops[o].out) == r && !D->ops[o].cat) q = (int)o;
+        const auto cs = readers_of_root(*D, w, r);
+        bool ok = q >= 0 && (D->ops[q].kind == OP_CONV1X1 || D->ops[q].kind == OP_CONV_DIRECT) && cs.size() == 1 && cs[0] == i && D->blobs[r].hwc;
+        if (ok) for (auto& st : D->ops[q].epi) if (st.src == SRC_TENSOR) ok = false;
+        direct = direct && ok;
+        prod.push_back(q);
+    }
+    int64_t off = 0;
+    for (size_t j = 0; j < w.in[i].size(); ++j) {
+        const int b = w.in[i][j];
+        if (direct) { Op& po = D->ops[prod[j]]; po.out = w.out[i][0]; po.cat = true; po.off = off; }
+        else { Op op; op.kind = OP_CONCAT_COPY; op.layer = i; op.in = b; op.out = w.out[i][0]; op.off = off; D->ops.push_back(op); }
+        off += D->blobs[b].n;
+    }
+}
+
+// The kernel list in graph order.  A convolution takes the tail build_tail finds; an element-wise layer no tail took gets a kernel of its own on
+// whichever operand step_of takes as the running value (the first, else a tensor second), extended by eltwise_chain.  Diagnostic mode (flags
+// bit 0) fuses nothing: one kernel per computing layer.
+int schedule(sgs_detector* D, const Wiring& w) {
+    const bool diag = D->flags & 1;
+    std::vector<char> absorbed(D->layers.size(), 0);
+    for (int i = 0; i < (int)D->layers.size(); ++i) {
+        const Layer& L = D->layers[i];
+        const bool conv = L.type == "Convolution" || L.type == "ConvolutionDepthWise";
+        if (absorbed[i] || !(conv || is_eltwise(L) || L.type == "Concat" || L.type == "Softmax")) continue;
+        Op op; op.layer = i; op.in = w.in[i][0]; op.out = w.out[i][0];
+        if (conv) {
+            const Blob& s = D->blobs[op.in]; const Blob& o = D->blobs[op.out];
             op.g = ConvGeom{s.c, o.c, s.h, s.w, o.h, o.w, L.pi(1, 1), L.pi(3, 1), L.pi(4, 0), L.pi(2, 1)};
             if (L.type == "ConvolutionDepthWise") op.kind = OP_DWCONV;
             else op.kind = (op.g.k == 1 && op.g.stride == 1 && op.g.pad == 0 && s.c % 4 == 0) ? OP_CONV1X1 : OP_CONV_DIRECT;
+            if (!diag) op.out = build_tail(*D, w, absorbed, i, op.out, op.epi);
             int rc = SGS_OK;
-            int fin = lout[i][0];
-            if (!diag) build_tail((int)i, lout[i][0], op.epi, fin);
             if (op.kind == OP_CONV1X1) {
                 const int m_tiles = (int)std::min<int64_t>(((int64_t)D->max_frames * op.g.OH * op.g.OW + tc::kBM - 1) / tc::kBM, 1 << 30);      // pixel tiles of a full batch
                 if (D->flags & 2) tc::plan_tiling(op.g.Cin, op.g.Cout, &op.gp, 0, m_tiles);
@@ -1039,59 +1120,29 @@ int build_graph(sgs_detector* D) {
             } else rc = upload(D, L.weight, &op.d_w);
             if (rc) return rc;
             rc = upload(D, L.bias, &op.d_b); if (rc) return rc;
-            op.out = fin;
-            D->ops.push_back(op);
         } else if (is_eltwise(L)) {
-            Op op; op.kind = OP_ELTWISE; op.layer = (int)i;
+            op.kind = OP_ELTWISE;
             EpiStepH st{};
-            int v = lin[i][0];
-            if (!step_of((int)i, v, -1, (int)i, st)) {
-                if (L.type == "BinaryOp" && !B[lin[i][1]].is_const) { v = lin[i][1]; }
-                if (!step_of((int)i, v, -1, (int)i, st)) { set_error("sgs_detector_create: layer %s cannot be scheduled", L.name.c_str()); return SGS_ERR_UNSUPPORTED; }
+            if (!step_of(*D, w, i, op.in, -1, i, st)) {
+                if (L.type == "BinaryOp" && !D->blobs[w.in[i][1]].is_const) op.in = w.in[i][1];
+                if (!step_of(*D, w, i, op.in, -1, i, st)) { set_error("sgs_detector_create: layer %s cannot be scheduled", L.name.c_str()); return SGS_ERR_UNSUPPORTED; }
             }
-            op.in = v; op.epi.push_back(st);
-            int fin = lout[i][0];
-            if (!diag) {
-                // extend with followers; the chain-start value of a stand-alone chain is its input, which SRC_START would not mean: pass -1
-                std::vector<EpiStepH> more; int cur = fin;
-                while ((int)op.epi.size() < kMaxEpi) {
-                    auto cs = consumers_of_root(cur);
-                    if (cs.size() != 1 || !is_eltwise(Ls[cs[0]]) || absorbed[cs[0]] || !step_of(cs[0], cur, -1, (int)i, st)) break;
-                    absorbed[cs[0]] = 1; op.epi.push_back(st); cur = lout[cs[0]][0];
-                }
-                fin = cur;
-            }
-            op.out = fin;
-            D->ops.push_back(op);
-        } else if (L.type == "Concat" && !B[lout[i][0]].is_const) {
-            // SSD head outputs: when every piece is the (permuted, flattened) output of a convolution that nothing else reads, those convolutions
-            // write their [h][w][c] rows straight into the concatenated buffer; otherwise (and in diagnostic mode) the pieces are copied
-            std::vector<int> prod;
-            bool direct = !diag;
-            for (int b : lin[i]) {
-                const int r = root_of(*D, b);
-                int q = -1;
-                for (size_t o = 0; o < D->ops.size(); ++o) if (root_of(*D, D->ops[o].out) == r && !D->ops[o].cat) q = (int)o;
-                const auto cs = consumers_of_root(r);
-                bool ok = q >= 0 && (D->ops[q].kind == OP_CONV1X1 || D->ops[q].kind == OP_CONV_DIRECT) && cs.size() == 1 && cs[0] == (int)i && B[r].hwc;
-                if (ok) for (auto& st : D->ops[q].epi) if (st.src == SRC_TENSOR) ok = false;
-                direct = direct && ok;
-                prod.push_back(q);
-            }
-            int64_t off = 0;
-            for (size_t j = 0; j < lin[i].size(); ++j) {
-                const int b = lin[i][j];
-                if (direct) { Op& po = D->ops[prod[j]]; po.out = lout[i][0]; po.cat = true; po.off = off; }
-                else { Op op; op.kind = OP_CONCAT_COPY; op.layer = (int)i; op.in = b; op.out = lout[i][0]; op.off = off; D->ops.push_back(op); }
-                off += B[b].n;
-            }
-        } else if (L.type == "Softmax") {
-            Op op; op.kind = OP_SOFTMAX; op.layer = (int)i; op.in = lin[i][0]; op.out = lout[i][0];
-            D->ops.push_back(op);
-        }
+            op.epi.push_back(st);
+            if (!diag) op.out = eltwise_chain(*D, w, absorbed, i, op.out, op.epi);
+        } else if (L.type == "Concat") {
+            if (!D->blobs[op.out].is_const) schedule_concat(D, w, i);
+            continue;
+        } else op.kind = OP_SOFTMAX;
+        D->ops.push_back(op);
     }
+    return SGS_OK;
+}
 
-    // ---- pass 3: activation pool.  A root's buffer is free again after the last kernel that reads it (or any alias).
+// ---- activation pool.  A root's buffer is free again after the last kernel that reads it (or any alias); a free buffer is reused best-fit, or the
+// largest one grows.  With every blob kept (flags bit 0 or 2) no buffer is ever reused.
+void plan_pool(sgs_detector* D) {
+    auto& B = D->blobs;
+    const bool keep = D->flags & 5;
     std::vector<int> last(B.size(), -1);
     auto touch = [&](int b, int opi) { const int r = root_of(*D, b); last[r] = std::max(last[r], opi); };
     for (size_t q = 0; q < D->ops.size(); ++q) {
@@ -1113,7 +1164,6 @@ int build_graph(sgs_detector* D) {
         D->pool_size.push_back(n); return (int)D->pool_size.size() - 1;
     };
     B[root_of(*D, D->input_blob)].buf = acquire(B[D->input_blob].n);
-    std::vector<std::vector<int>> release_at(D->ops.size());
     for (size_t q = 0; q < D->ops.size(); ++q) {
         const int r = root_of(*D, D->ops[q].out);
         if (B[r].buf < 0) B[r].buf = acquire(B[r].n);
@@ -1125,8 +1175,12 @@ int build_graph(sgs_detector* D) {
         if (q == 0 && last[ri] <= 0 && std::find(free_list.begin(), free_list.end(), B[ri].buf) == free_list.end()) free_list.push_back(B[ri].buf);
         if (last[r] < 0 && r != root_of(*D, D->loc_blob) && r != root_of(*D, D->conf_blob)) free_list.push_back(B[r].buf);   // never read: dead output
     }
+}
+
+// ---- device memory: the pool buffers (max_frames x size), every blob's address in them, the GEMMs' activation tensor maps, the DetectionOutput scratch.
+int allocate(sgs_detector* D) {
+    auto& B = D->blobs;
     D->pool.assign(D->pool_size.size(), nullptr);
-    if (D->flags & 2) return SGS_OK;                     // plan only
     for (size_t q = 0; q < D->pool_size.size(); ++q) SGS_CUDA_TRY(D->res.alloc(&D->pool[q], (size_t)D->pool_size[q] * D->max_frames * sizeof(float)));
     for (auto& b : B) { const int r = root_of(*D, (int)(&b - &B[0])); if (B[r].buf >= 0) b.dev = D->pool[B[r].buf]; }
     for (auto& op : D->ops)                                   // the GEMMs' activation operand: [max_frames * H * W][Cin], rows past the batch are never stored
@@ -1140,25 +1194,28 @@ int build_graph(sgs_detector* D) {
 }
 
 Epi make_epi(const sgs_detector* D, const std::vector<EpiStepH>& h) {
-    Epi e; e.n = (int)h.size(); e.kind = EK_GENERIC;
+    Epi e; e.n = (int)h.size(); e.kind = epi_kind(h);
     for (int i = 0; i < e.n; ++i) {
         e.s[i].op = h[i].op; e.s[i].src = h[i].src; e.s[i].rev = h[i].rev; e.s[i].a = h[i].a; e.s[i].b = h[i].b;
         e.s[i].t = h[i].src == SRC_TENSOR ? D->blobs[h[i].tblob].dev : nullptr;
     }
-    auto is = [&](int i, int op, int src) { return h[i].op == op && (op >= E_CLIP || h[i].src == src); };
-    // the fast paths reproduce the generic loop operation for operation (same operand order, one rounding each)
-    if (e.n == 0) e.kind = EK_NONE;
-    else if (e.n == 1 && h[0].op == E_RELU) e.kind = EK_RELU;
-    else if (e.n == 1 && h[0].op == E_CLIP) e.kind = EK_CLIP;
-    else if (e.n == 1 && is(0, E_ADD, SRC_TENSOR)) e.kind = EK_ADD_T;          // addition commutes: rev is irrelevant
-    else if (e.n == 4 && is(0, E_ADD, SRC_SCALAR) && h[1].op == E_CLIP && is(2, E_MUL, SRC_START) && is(3, E_DIV, SRC_SCALAR) && !h[3].rev && h[3].a == 6.0f) e.kind = EK_HSWISH;
-    else if (e.n == 5 && is(0, E_ADD, SRC_SCALAR) && h[1].op == E_CLIP && is(2, E_DIV, SRC_SCALAR) && !h[2].rev && h[2].a == 6.0f && is(3, E_MUL, SRC_TENSOR) && is(4, E_ADD, SRC_TENSOR))
-        e.kind = EK_SE_TAIL;
-    else if (e.n == 4 && is(0, E_ADD, SRC_SCALAR) && h[1].op == E_CLIP && is(2, E_DIV, SRC_SCALAR) && !h[2].rev && h[2].a == 6.0f && is(3, E_MUL, SRC_TENSOR)) e.kind = EK_SE_MUL;
     return e;
 }
 
 inline unsigned nblk(int64_t total) { return (unsigned)((total + 255) / 256); }
+
+// Depth-wise convolutions: V = 4 channels per thread (float4) when Cout % 4 == 0, and then two output rows per thread on maps of 4 rows or more
+// (the K + S input rows serve both: 1.5x / 1.67x fewer row loads for 3x3 / 5x5 at stride 1).
+template <int K, int S>
+void launch_dwconv(const float* in, const Op& op, float* out, int F, const Epi& epi, cudaStream_t st) {
+    auto go = [&](auto kernel, int V, int YT) {
+        const int64_t total = (int64_t)F * ((op.g.OH + YT - 1) / YT) * ((op.g.OW + 3) / 4) * (op.g.Cout / V);
+        kernel<<<nblk(total), 256, 0, st>>>(in, op.d_w, op.d_b, out, op.g, total, epi);
+    };
+    if (op.g.Cout % 4) go(dwconv_kernel<K, S, 1, 1>, 1, 1);
+    else if (op.g.OH >= 4) go(dwconv_kernel<K, S, 4, 2>, 4, 2);
+    else go(dwconv_kernel<K, S, 4, 1>, 4, 1);
+}
 
 }  // namespace
 
@@ -1175,7 +1232,12 @@ int sgs_detector_create(const char* param_path, const char* bin_path, int max_fr
     try {                                              // malformed files must come back as a status, never as an exception through the C ABI
         rc = parse_param(param_path, D->layers);
         if (rc == SGS_OK) rc = load_bin(bin_path, D->layers);
-        if (rc == SGS_OK) rc = build_graph(D.get());
+        Wiring w;
+        if (rc == SGS_OK) rc = wire_graph(D.get(), w);
+        if (rc == SGS_OK) rc = infer_shapes(D.get(), w);
+        if (rc == SGS_OK) rc = schedule(D.get(), w);
+        if (rc == SGS_OK) plan_pool(D.get());
+        if (rc == SGS_OK && !(flags & 2)) rc = allocate(D.get());
     } catch (const std::exception& ex) {
         set_error("sgs_detector_create: %s while reading %s / %s", ex.what(), param_path, bin_path);
         rc = SGS_ERR_INVALID;
@@ -1256,7 +1318,7 @@ int sgs_detector_detect_device(sgs_detector* D, const uint8_t* d_rgb, int64_t fr
             if (npix >= (1ll << 31) - 256) { set_error("sgs_detector_detect_device: batch too large for 32-bit pixel indices"); return SGS_ERR_UNSUPPORTED; }
             const int64_t fstride = op.cat ? bo.n : (int64_t)HW * op.g.Cout;
             bool launched = false;
-            epi_dispatch_host(epi.kind, [&](auto kind) {
+            epi_dispatch(epi.kind, [&](auto kind) {
                 launched = tc::launch_conv1x1_tc_map(op.gp, op.map_in, (int)npix, op.d_b, bo.dev, HW, fstride, op.cat ? op.off : 0, op.g.Cout, EpiFnK<decltype(kind)::value>{epi}, st);
             });
             if (!launched) {
@@ -1276,18 +1338,8 @@ int sgs_detector_detect_device(sgs_detector* D, const uint8_t* d_rgb, int64_t fr
             break;
         }
         case OP_DWCONV: {
-            const int V = op.g.Cout % 4 == 0 ? 4 : 1;
-            // two output rows per thread on the vectorised layers (the K + S input rows serve both: 1.5x / 1.67x fewer row loads for 3x3 / 5x5 at stride 1)
-            const int YT = (V == 4 && op.g.OH >= 4) ? 2 : 1;
-            const int64_t total = (int64_t)F * ((op.g.OH + YT - 1) / YT) * ((op.g.OW + 3) / 4) * (op.g.Cout / V);
-#define SGS_DW(K, S) do { if (V == 4 && YT == 2) dwconv_kernel<K, S, 4, 2><<<nblk(total), 256, 0, st>>>(bi.dev, op.d_w, op.d_b, bo.dev, op.g, total, epi); \
-                          else if (V == 4) dwconv_kernel<K, S, 4, 1><<<nblk(total), 256, 0, st>>>(bi.dev, op.d_w, op.d_b, bo.dev, op.g, total, epi); \
-                          else dwconv_kernel<K, S, 1, 1><<<nblk(total), 256, 0, st>>>(bi.dev, op.d_w, op.d_b, bo.dev, op.g, total, epi); } while (0)
-            if (op.g.k == 3 && op.g.stride == 1) SGS_DW(3, 1);
-            else if (op.g.k == 3) SGS_DW(3, 2);
-            else if (op.g.stride == 1) SGS_DW(5, 1);
-            else SGS_DW(5, 2);
-#undef SGS_DW
+            if (op.g.k == 3) (op.g.stride == 1 ? launch_dwconv<3, 1> : launch_dwconv<3, 2>)(bi.dev, op, bo.dev, F, epi, st);
+            else (op.g.stride == 1 ? launch_dwconv<5, 1> : launch_dwconv<5, 2>)(bi.dev, op, bo.dev, F, epi, st);
             break;
         }
         case OP_ELTWISE: {

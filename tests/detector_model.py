@@ -258,7 +258,7 @@ def write_tail_model(dirpath, seed=0, name='tails'):
     return pp, bp
 
 
-TAIL_KINDS = ('relu', 'clip', 'hswish', 'add', 'se_gate', 'se_tail', 'generic')      # the tails make_epi recognises, and its generic chain
+TAIL_KINDS = ('relu', 'clip', 'hswish', 'add', 'se_gate', 'se_tail', 'generic')      # the tails epi_kind (detector.cu) recognises, and its generic chain
 TENSOR_TAILS = ('add', 'se_gate', 'se_tail')                                        # the kinds that read same-shape operand tensors
 
 
@@ -352,8 +352,8 @@ def write_wide_tail_model(dirpath, seed=0, cases=WIDE_TAIL_CASES, name='wide_tai
 
 def plan_tails(describe_text):
     """parse_plan of describe_text, each line with 'steps' (the fused element-wise steps after ' | ': (op, rev, src, value) with src 'scalar' /
-    'start' / 'tensor', value the scalar, the clip bounds or the operand blob) and 'kind': make_epi's classification of the steps (detector.cu) --
-    'none', one of TAIL_KINDS.  Like make_epi it ignores (rev) on add and mul, and takes the hard-swish / hard-sigmoid forms only with the divisor 6
+    'start' / 'tensor', value the scalar, the clip bounds or the operand blob) and 'kind': epi_kind's classification of the steps (detector.cu) --
+    'none', one of TAIL_KINDS.  Like epi_kind it ignores (rev) on add and mul, and takes the hard-swish / hard-sigmoid forms only with the divisor 6
     and an un-reversed division."""
     out = []
     for p in parse_plan(describe_text):
@@ -376,7 +376,7 @@ def plan_tails(describe_text):
 
 
 def epi_kind(steps):
-    """make_epi's tail kind of the (op, rev, src, value) steps of plan_tails"""
+    """epi_kind's tail kind of the (op, rev, src, value) steps of plan_tails"""
     def is_(i, op, src=None):
         return steps[i][0] == op and (src is None or steps[i][2] == src)
 

@@ -27,7 +27,7 @@ MAC_PER_S = 132 * 1024 * 1.98e9
 
 
 def tail_kind(tail):
-    """the planner's classification (make_epi in detector.cu), from the describe text of the tail"""
+    """the planner's classification (epi_kind in detector.cu), from the describe text of the tail"""
     steps = [s.strip() for s in tail.split('|') if s.strip()]
     ops = [s.split()[0] for s in steps]
     tensor = [bool(re.match(r'(?:add|mul|sub|div)(?:\(rev\))? [0-9A-Za-z_]+ buf', s)) for s in steps]
