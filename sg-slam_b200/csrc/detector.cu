@@ -914,8 +914,13 @@ int infer_shapes(sgs_detector* D, const Wiring& w) {
             const Blob& s = in0(); Blob& o = B[w.out[i][0]];
             o.dims = s.dims; o.c = s.c; o.h = s.h; o.w = s.w; o.n = s.n; o.hwc = s.hwc;
             if (L.type == "BinaryOp") {
+                // the kernels read a tensor operand at the value's flat [h][w][c] index: only an operand of the value's own shape and layout is that
+                // element (ncnn would broadcast other shapes; a flattened or permuted view orders the elements differently)
                 const Blob& t = B[w.in[i][1]];
-                if (s.is_const || !(t.is_const ? t.n == 1 : t.n == s.n)) { set_error("sgs_detector_create: BinaryOp %s: unsupported operand shapes", L.name.c_str()); return SGS_ERR_UNSUPPORTED; }
+                const bool same = t.dims == s.dims && t.c == s.c && t.h == s.h && t.w == s.w && t.hwc == s.hwc;
+                if (s.is_const || !(t.is_const ? t.n == 1 : same)) { set_error("sgs_detector_create: BinaryOp %s: unsupported operand shapes", L.name.c_str()); return SGS_ERR_UNSUPPORTED; }
+                if (!t.is_const && root_of(*D, w.in[i][0]) == root_of(*D, w.in[i][1])) {
+                    set_error("sgs_detector_create: BinaryOp %s: both operands are the same blob (x op x is not supported)", L.name.c_str()); return SGS_ERR_UNSUPPORTED; }
                 if (L.pi(0, 0) < 0 || L.pi(0, 0) > 3) { set_error("sgs_detector_create: BinaryOp %s: op_type %d not supported", L.name.c_str(), L.pi(0, 0)); return SGS_ERR_UNSUPPORTED; }
             }
         }
@@ -999,7 +1004,7 @@ bool step_of(const sgs_detector& D, const Wiring& w, int li, int vblob, int star
     const int o = va ? b : a;
     if (B[o].is_const) { st.src = SRC_SCALAR; st.a = B[o].cval[0]; return true; }
     if (start_blob >= 0 && root_of(D, o) == root_of(D, start_blob) && root_of(D, o) != root_of(D, vblob)) { st.src = SRC_START; return true; }
-    if (va && vb) return false;                                                 // x op x: leave to the generic path
+    if (va && vb) return false;                                                 // x op x: infer_shapes refuses it, no kernel computes it
     if (B[root_of(D, o)].producer < owner_layer) { st.src = SRC_TENSOR; st.tblob = o; return true; }
     return false;
 }
@@ -1404,6 +1409,7 @@ int sgs_detector_describe(const sgs_detector* D, char* out, int64_t cap, int64_t
         ss << kind[op.kind] << ' ' << D->layers[op.layer].name << " in " << bi.name << " buf " << D->blobs[root_of(*D, op.in)].buf << " out " << bo.name << " buf "
            << D->blobs[root_of(*D, op.out)].buf << " n " << bo.n;
         if (op.kind <= OP_DWCONV) ss << " geom " << op.g.Cin << 'x' << op.g.H << 'x' << op.g.W << "->" << op.g.Cout << 'x' << op.g.OH << 'x' << op.g.OW << " k" << op.g.k << " s" << op.g.stride << " p" << op.g.pad;
+        if (op.kind <= OP_DWCONV && op.g.dil != 1) ss << " d" << op.g.dil;
         if (op.kind == OP_CONCAT_COPY || op.cat) ss << " off " << op.off;
         if (op.kind == OP_CONV1X1) ss << " tile " << op.gp.NT << "x" << op.gp.n_tiles << " kb " << op.gp.KB << "x" << op.gp.BK << " stages " << op.gp.stages << (op.gp.b_resident ? " wres" : "")
                                     << " smem " << op.gp.smem_bytes << " wgmma m64n" << op.gp.NT << "k8";

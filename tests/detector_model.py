@@ -29,19 +29,20 @@ class Graph:
         self.layers.insert(1, ['MemoryData', n, [], [n], '0=1', [np.array([v], np.float32)]])
         return n
 
-    def conv(self, x, cin, cout, k=1, s=1, p=0, gain=1.0, dw=False, w=None, b=None, name=None):
+    def conv(self, x, cin, cout, k=1, s=1, p=0, gain=1.0, dw=False, w=None, b=None, name=None, bias=True, dil=1):
+        """bias=False: bias_term 0 (5=0) and no bias floats in the weight file; dil: dilation (2= / 12=)"""
         fan = k * k * (1 if dw else cin)
         if w is None:
             w = (self.rng.standard_normal((cout, 1 if dw else cin, k, k)) * gain * np.sqrt(2.0 / fan)).astype(np.float32)
-        if b is None:
+        if b is None and bias:
             b = (self.rng.standard_normal(cout) * 0.1).astype(np.float32)
-        prm = '0=%d 1=%d 11=%d 2=1 12=1 3=%d 13=%d 4=%d 14=%d 5=1 6=%d' % (cout, k, k, s, s, p, p, w.size)
+        prm = '0=%d 1=%d 11=%d 2=%d 12=%d 3=%d 13=%d 4=%d 14=%d 5=%d 6=%d' % (cout, k, k, dil, dil, s, s, p, p, int(bias), w.size)
         if dw:
             prm += ' 7=%d' % cout
-        return self.add('ConvolutionDepthWise' if dw else 'Convolution', [x], prm, [np.zeros(1, np.uint32), w, b], name=name)
+        return self.add('ConvolutionDepthWise' if dw else 'Convolution', [x], prm, [np.zeros(1, np.uint32), w] + ([b] if bias else []), name=name)
 
     def relu(self, x): return self.add('ReLU', [x])
-    def clip(self, x): return self.add('Clip', [x], '0=0.000000 1=6.000000')
+    def clip(self, x, lo=0.0, hi=6.0): return self.add('Clip', [x], '0=%f 1=%f' % (lo, hi))
     def binop(self, a, b, op): return self.add('BinaryOp', [a, b], '0=%d' % op)
 
     def hswish(self, x):
@@ -260,6 +261,29 @@ def write_tail_model(dirpath, seed=0, name='tails'):
 
 TAIL_KINDS = ('relu', 'clip', 'hswish', 'add', 'se_gate', 'se_tail', 'generic')      # the tails epi_kind (detector.cu) recognises, and its generic chain
 TENSOR_TAILS = ('add', 'se_gate', 'se_tail')                                        # the kinds that read same-shape operand tensors
+TAIL_OPERANDS = {'add': 1, 'se_gate': 1, 'se_tail': 2}                              # operand tensors t1, t2 each kind reads
+
+
+def _tail(g, kind, y, ops):
+    """The tail `kind` after y, as ncnn exports it (ops: the operand blobs t1, t2); returns its last blob:
+      relu     ReLU(y)                      clip     Clip(y, 0, 6)                  hswish   y * Clip(y + 3, 0, 6) / 6
+      add      y + t1                       se_gate  t1 * (Clip(y + 3, 0, 6) / 6)   se_tail  t1 * (Clip(y + 3, 0, 6) / 6) + t2
+      generic  ReLU(y * 0.5)"""
+    if kind == 'relu':
+        return g.relu(y)
+    if kind == 'clip':
+        return g.clip(y)
+    if kind == 'hswish':
+        return g.hswish(y)
+    if kind == 'add':
+        return g.binop(y, ops[0], 0)
+    if kind == 'se_gate':
+        return g.binop(ops[0], g.hsigmoid(y), 2)
+    if kind == 'se_tail':
+        return g.binop(g.binop(ops[0], g.hsigmoid(y), 2), ops[1], 0)
+    if kind == 'generic':
+        return g.relu(g.binop(y, g.const(0.5), 2))
+    raise ValueError(kind)
 
 
 def _wide_tail_cases():
@@ -315,32 +339,13 @@ def write_wide_tail_model(dirpath, seed=0, cases=WIDE_TAIL_CASES, name='wide_tai
             feeds[(cin, hw)] = chain[hw] if cin == 16 else g.conv(chain[hw], 16, cin)
         return feeds[(cin, hw)]
 
-    def hsig(y):
-        return g.binop(g.clip(g.binop(y, g.const(3.0), 0)), g.const(6.0), 3)
-
     info = []
     for kind, cin, cout, hw in cases:
         x = feed(cin, hw)
-        ops = [g.conv(x, cin, cout) for _ in range({'add': 1, 'se_gate': 1, 'se_tail': 2}.get(kind, 0))]
+        ops = [g.conv(x, cin, cout) for _ in range(TAIL_OPERANDS.get(kind, 0))]
         y = g.conv(x, cin, cout, name=g.name('wide_%s_' % kind))
         w, b = g.layers[-1][5][1].reshape(cout, cin), g.layers[-1][5][2]
-        if kind == 'relu':
-            out = g.relu(y)
-        elif kind == 'clip':
-            out = g.clip(y)
-        elif kind == 'hswish':
-            out = g.hswish(y)
-        elif kind == 'add':
-            out = g.binop(y, ops[0], 0)
-        elif kind == 'se_gate':
-            out = g.binop(ops[0], hsig(y), 2)
-        elif kind == 'se_tail':
-            out = g.binop(g.binop(ops[0], hsig(y), 2), ops[1], 0)
-        elif kind == 'generic':
-            out = g.relu(g.binop(y, g.const(0.5), 2))
-        else:
-            raise ValueError(kind)
-        info.append(dict(kind=kind, cin=cin, cout=cout, hw=hw, x=x, y=y, ops=ops, out=out, w=w, b=b))
+        info.append(dict(kind=kind, cin=cin, cout=cout, hw=hw, x=x, y=y, ops=ops, out=_tail(g, kind, y, ops), w=w, b=b))
     n0 = len(g.layers)
     _head(g, data, [(chain[19], 16)], 4, '-23300=1,60.000000 -23301=1,105.0 -23302=1,2.000000 7=1')
     head = [L[3][0] for L in g.layers[n0:] if L[0] == 'Convolution']
@@ -350,6 +355,167 @@ def write_wide_tail_model(dirpath, seed=0, cases=WIDE_TAIL_CASES, name='wide_tai
     return pp, bp, info, head
 
 
+DW_KS = ((3, 1), (3, 2), (5, 1), (5, 2))
+# depth-wise variant -> (channels, {stride: input map}): V1 (odd C: one channel per thread), V4Y2 (float4, two output rows per thread: output map
+# 19x19, odd and not a multiple of 4 wide), V4Y1 (float4, one row: output maps of 2 and 3 rows)
+DW_VARIANTS = {'V1': (7, {1: 5, 2: 10}), 'V4Y2': (16, {1: 19, 2: 38}), 'V4Y1': (24, {1: 2, 2: 5})}
+# dense direct shapes (cin, k, s, dil, input map), rotated over the conv_small_kernel cases
+CONV_SHAPES = ((6, 3, 1, 1, 19), (10, 3, 2, 1, 19), (16, 1, 2, 1, 19), (6, 1, 1, 1, 10), (6, 3, 1, 2, 10))
+
+
+def _direct_tail_cases():
+    """Cases of write_direct_tail_model, each ('dw', kind, variant, k, s, bias) / ('conv', kind, cout, shape index, bias) / ('stem', kind, bias) /
+    ('gemm', kind, cout, bias) / ('cat',) / ('chain', name):
+      dw     every TAIL_KINDS entry in each depth-wise variant of DW_VARIANTS (dwconv_kernel<K, S, V, YT>), (K, S) rotating over DW_KS with the kind
+             and the variant, so that each of 3/1, 3/2, 5/1, 5/2 meets every variant and at least one tensor-reading kind; one bias-free case
+             (relu) per variant;
+      conv   every kind on Cout 16 (float4 path), Cout 12 (second 8-channel block partial: scalar path) and Cout 5 (scalar), CONV_SHAPES rotating
+             (3x3 s1 Cin 6, 3x3 s2 Cin 10, 1x1 s2, 1x1 Cin 6, 3x3 dilation 2), all through conv_small_kernel; bias-free cases on the float4 path
+             (hswish, Cout 16) and the scalar path (relu, Cout 5);
+      stem   one 3 -> 16 3x3/s2 stem per kind off the input (conv_first_kernel), its tensor operands further stems; one bias-free stem (clip);
+      gemm   bias-free 1x1 GEMMs 16 -> Cout on the 19x19 chain map (the null bias of conv1x1_tc_kernel): Cout 24 on a narrow tile (NT 32, two CTAs
+             per SM, bias loaded at each use) under hard-swish, Cout 100 on a wide tile (NT 128, bias loaded per chunk) under the SE tail;
+      cat    the SSD head: 3x3 conv_small_kernel pieces with non-tensor tails written straight into mbox_conf / mbox_loc, on the 5x5 (4 priors),
+             3x3 (3 priors) and 2x2 (4 priors) maps: mbox_conf is 2100 + 567 + 336 = 3003 floats per frame, so its 84-channel first piece sits at
+             offset 0 (a multiple of 4) with a frame stride that is not, and its third piece at the odd offset 2667;
+      chain  'cut': a depth-wise output whose tail's second value has a second element-wise reader: build_tail keeps the longest valid prefix
+             (add, relu), the rest runs through eltwise_kernel, one of whose values has two readers again (eltwise_chain stops there);
+             'long': ten steps after a 3x3 conv: eight fused, two in one stand-alone eltwise_kernel;
+             'ops': sub, sub(rev) by a tensor first operand, div 0.75, clip(-1, 2.5), add 2, div(rev) of that tensor, div by a tensor >= 1;
+             'start': y + relu(y) (SRC_START inside a generic tail)."""
+    cases = []
+    for v, var in enumerate(DW_VARIANTS):
+        for i, kind in enumerate(TAIL_KINDS):
+            k, s = DW_KS[(i + v) % 4]
+            cases.append(('dw', kind, var, k, s, True))
+        cases.append(('dw', 'relu', var, *DW_KS[(v + 2) % 4], False))
+    j = 0
+    for cout in (16, 12, 5):
+        for kind in TAIL_KINDS:
+            cases.append(('conv', kind, cout, j % len(CONV_SHAPES), True))
+            j += 1
+    cases += [('conv', 'hswish', 16, 0, False), ('conv', 'relu', 5, 1, False)]
+    cases += [('stem', kind, True) for kind in TAIL_KINDS] + [('stem', 'clip', False)]
+    cases += [('gemm', 'hswish', 24, False), ('gemm', 'se_tail', 100, False)]
+    cases += [('cat',)] + [('chain', n) for n in ('cut', 'long', 'ops', 'start')]
+    return cases
+
+
+DIRECT_TAIL_CASES = _direct_tail_cases()
+CAT_PIECES = ((5, 4, 'hswish', 'clip'), (3, 3, 'relu', 'generic'), (2, 4, 'generic', 'hswish'))      # (map, priors, conf tail, loc tail)
+
+
+def write_direct_tail_model(dirpath, seed=0, cases=DIRECT_TAIL_CASES, name='direct_tails'):
+    """Fused element-wise tails on the direct kernels (depth-wise, conv_small_kernel, conv_first_kernel) and stand-alone element-wise chains, for
+    tests/test_gpu_detector_direct_tails.py; 8-frame batches (PROBE_FRAMES).  The trunk is write_probe_model's (3x3/s2 stem 3 -> 16 with
+    per-channel gains, depth-wise 3x3/s2 chain down to 2x2, here with a third of the gain); a feed of c channels at map hw is the chain map
+    itself (c 16) or one dense 1x1 expansion 16 -> c.  Tails as _tail writes them; tensor operands are convolutions of the tailed layer's own geometry on the same feed, written
+    before it.  The SSD head is the 'cat' case (every case list needs it: it closes the graph).
+    Returns (param path, bin path, info, head): info[i] = dict(case, family ('dw' / 'conv' / 'stem' / 'gemm' / 'cat' / 'chain'), kind, variant (dw),
+    conv (the tailed convolution: in, out, dw, cin, cout, k, s, p, dil, hw, w, b or None), ops (operand blobs), out (the tail's last blob)) for each
+    tailed convolution of cases[i] (the 'cat' case: one entry per head piece; 'chain' entries carry outs, every blob of the chain);
+    head = the head convolutions' outputs."""
+    g = Graph(seed)
+    data = g.add('Input', [], name='input')
+    ws = (g.rng.standard_normal((16, 3, 3, 3)) * np.sqrt(2.0 / 27) * np.exp2(g.rng.uniform(-3, 3, (16, 1, 1, 1))) / 64).astype(np.float32)
+    chain = {150: g.conv(data, 3, 16, 3, 2, 1, w=ws)}
+    for a, bsz in zip(CHAIN, CHAIN[1:]):
+        if bsz < 2:
+            break
+        chain[bsz] = g.conv(chain[a], 16, 16, 3, 2, 1, dw=True, gain=0.5)          # activations stay of order one down the chain
+    feeds = {}
+
+    def feed(c, hw):
+        if (c, hw) not in feeds:
+            feeds[(c, hw)] = chain[hw] if c == 16 else g.conv(chain[hw], 16, c)
+        return feeds[(c, hw)]
+
+    def conv(x, cin, cout, k, s, hw, dw=False, dil=1, bias=True, gain=1.0, tag='d'):
+        p = dil * (k // 2)
+        y = g.conv(x, cin, cout, k, s, p, gain=gain, dw=dw, bias=bias, dil=dil, name=g.name(tag))
+        L = g.layers[-1]
+        return y, dict(dw=dw, cin=cin, cout=cout, k=k, s=s, p=p, dil=dil, hw=hw, w=L[5][1], b=L[5][2] if bias else None, out=y, **{'in': x})
+
+    info, head = [], []
+    for case in cases:
+        fam = case[0]
+        if fam in ('dw', 'conv', 'stem', 'gemm'):
+            kind, bias = case[1], case[-1]
+            if fam == 'dw':
+                _, _, var, k, s, _ = case
+                c, maps = DW_VARIANTS[var]
+                x, geo = feed(c, maps[s]), dict(cin=c, cout=c, k=k, s=s, hw=maps[s], dw=True)
+            elif fam == 'conv':
+                cin, k, s, dil, hw = CONV_SHAPES[case[3]]
+                x, geo = feed(cin, hw), dict(cin=cin, cout=case[2], k=k, s=s, hw=hw, dil=dil)
+            elif fam == 'gemm':
+                x, geo = chain[19], dict(cin=16, cout=case[2], k=1, s=1, hw=19)
+            else:
+                x, geo = data, dict(cin=3, cout=16, k=3, s=2, hw=300, gain=1 / 16)
+            ops = [conv(x, **geo)[0] for _ in range(TAIL_OPERANDS.get(kind, 0))]
+            y, cv = conv(x, bias=bias, tag='%s_%s_' % (fam, kind), **geo)
+            info.append(dict(case=case, family=fam, kind=kind, variant=case[2] if fam == 'dw' else None, conv=cv, ops=ops, out=_tail(g, kind, y, ops)))
+        elif fam == 'chain':
+            info.append(_chain_case(g, case, feed, conv))
+        elif fam != 'cat':
+            raise ValueError(case)
+    ncls = 21
+    locs, confs, priors = [], [], []
+    for hw, npr, ck, lk in CAT_PIECES:
+        f = chain[hw]
+        for what, cout, kind, dst in (('conf', npr * ncls, ck, confs), ('loc', npr * 4, lk, locs)):
+            y, cv = conv(f, 16, cout, 3, 1, hw, gain=2.5 if kind == 'hswish' else 1.0, tag='cat_%s_' % what)     # hard-swish inputs past +-3
+            if what == 'conf':
+                cv['b'][15::ncls] += np.float32(2.0)                              # the person class (15) shows up among the detections
+            head.append(y)
+            out = _tail(g, kind, y, [])
+            info.append(dict(case=('cat',), family='cat', kind=kind, variant=what, conv=cv, ops=[], out=out))
+            dst.append(g.add('Flatten', [g.add('Permute', [out], '0=3')]))
+        priors.append(g.add('PriorBox', [f, data], '-23300=1,60.000000 -23301=1,105.0 -23302=1,2.000000 7=%d 3=0.100000 4=0.100000 5=0.200000 '
+                                                   '6=0.200000 8=0 9=-233 10=-233 11=-233.000000 12=-233.000000 13=0.500000 14=1 15=1' % (npr == 4)))
+    loc = g.add('Concat', locs, '0=0', name='mbox_loc')
+    conf = g.add('Concat', confs, '0=0', name='mbox_conf')
+    pri = g.add('Concat', priors, '0=1', name='mbox_priorbox')
+    sm = g.add('Softmax', [g.add('Reshape', [conf], '0=%d 1=-1' % ncls)], '0=1 1=1')
+    g.add('DetectionOutput', [loc, g.add('Flatten', [sm]), pri], '0=%d 1=0.450000 2=300 3=100 4=0.010000' % ncls, name='detection_out')
+    os.makedirs(dirpath, exist_ok=True)
+    pp, bp = os.path.join(dirpath, name + '.param'), os.path.join(dirpath, name + '.bin')
+    g.write(pp, bp)
+    return pp, bp, info, head
+
+
+def _chain_case(g, case, feed, conv):
+    """The element-wise chains of _direct_tail_cases ('chain', name): info entry with outs = every blob the chain writes, in graph order"""
+    nm = case[1]
+    sc = g.const
+    if nm == 'cut':                                   # depth-wise 3x3/s1 on 16 channels at 19x19 (V4Y2)
+        y, cv = conv(feed(16, 19), 16, 16, 3, 1, 19, dw=True, tag='chain_cut_')
+        a = g.binop(y, sc(1.0), 0); r = g.relu(a); m = g.binop(r, sc(2.0), 2); c = g.clip(m, -1.0, 2.5); s = g.binop(r, sc(0.25), 1); q = g.relu(m)
+        outs, ops = [a, r, m, c, s, q], []
+    elif nm == 'long':                                # 3x3/s1 conv_small_kernel 6 -> 12 at 19x19
+        y, cv = conv(feed(6, 19), 6, 12, 3, 1, 19, tag='chain_long_')
+        v, outs = y, []
+        for op, val in ((0, 0.5), (2, 1.5), ('relu', None), (1, 0.25), ('clip', (-2.0, 3.0)), (2, 0.75), (0, -0.125), (3, 1.25), (2, 2.0), ('relu', None)):
+            v = g.relu(v) if op == 'relu' else g.clip(v, *val) if op == 'clip' else g.binop(v, sc(val), op)
+            outs.append(v)
+        ops = []
+    elif nm == 'ops':                                 # depth-wise 5x5/s1 on 16 channels at 19x19 (V4Y2)
+        x = feed(16, 19)
+        t1 = conv(x, 16, 16, 5, 1, 19, dw=True)[0]
+        tpos = g.binop(g.relu(conv(x, 16, 16, 5, 1, 19, dw=True)[0]), sc(1.0), 0)          # >= 1: a divisor bounded away from zero
+        y, cv = conv(x, 16, 16, 5, 1, 19, dw=True, tag='chain_ops_')
+        a1 = g.binop(y, sc(0.5), 1); a2 = g.binop(t1, a1, 1); a3 = g.binop(a2, sc(0.75), 3); a4 = g.clip(a3, -1.0, 2.5)
+        a5 = g.binop(a4, sc(2.0), 0); a6 = g.binop(t1, a5, 3); a7 = g.binop(a6, tpos, 3)
+        outs, ops = [a1, a2, a3, a4, a5, a6, a7], [t1, tpos]
+    elif nm == 'start':                               # 1x1 conv_small_kernel 6 -> 5 at 10x10
+        y, cv = conv(feed(6, 10), 6, 5, 1, 1, 10, tag='chain_start_')
+        r = g.relu(y)
+        outs, ops = [r, g.binop(y, r, 0)], []
+    else:
+        raise ValueError(nm)
+    return dict(case=case, family='chain', kind=nm, variant=None, conv=cv, ops=ops, out=outs[-1], outs=outs)
+
+
 def plan_tails(describe_text):
     """parse_plan of describe_text, each line with 'steps' (the fused element-wise steps after ' | ': (op, rev, src, value) with src 'scalar' /
     'start' / 'tensor', value the scalar, the clip bounds or the operand blob) and 'kind': epi_kind's classification of the steps (detector.cu) --
@@ -357,22 +523,27 @@ def plan_tails(describe_text):
     and an un-reversed division."""
     out = []
     for p in parse_plan(describe_text):
-        steps = []
-        for s in p['line'].split(' | ')[1:]:
-            t = s.split()
-            op, rev = t[0].replace('(rev)', ''), t[0].endswith('(rev)')
-            if op in ('relu', 'clip'):
-                steps.append((op, rev, None, tuple(float(v) for v in t[1:])))
-            elif t[1] == 'start':
-                steps.append((op, rev, 'start', None))
-            elif len(t) == 4 and t[2] == 'buf':                  # '<blob> buf <n>' (blob names may be numbers)
-                steps.append((op, rev, 'tensor', t[1]))
-            else:
-                steps.append((op, rev, 'scalar', float(t[1])))
-        p['steps'] = steps
-        p['kind'] = epi_kind(steps)
+        p['steps'] = tail_steps(p['line'])
+        p['kind'] = epi_kind(p['steps'])
         out.append(p)
     return out
+
+
+def tail_steps(line):
+    """the element-wise steps of a describe() line (after ' | ') as plan_tails gives them"""
+    steps = []
+    for s in line.split(' | ')[1:]:
+        t = s.split()
+        op, rev = t[0].replace('(rev)', ''), t[0].endswith('(rev)')
+        if op in ('relu', 'clip'):
+            steps.append((op, rev, None, tuple(float(v) for v in t[1:])))
+        elif t[1] == 'start':
+            steps.append((op, rev, 'start', None))
+        elif len(t) == 4 and t[2] == 'buf':                  # '<blob> buf <n>' (blob names may be numbers)
+            steps.append((op, rev, 'tensor', t[1]))
+        else:
+            steps.append((op, rev, 'scalar', float(t[1])))
+    return steps
 
 
 def epi_kind(steps):

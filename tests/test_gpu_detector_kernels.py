@@ -52,7 +52,7 @@ def _pc(a):
 
 
 def _out_hw(c):
-    return (c['hw'] + 2 * c['p'] - c['k']) // c['s'] + 1
+    return (c['hw'] + 2 * c['p'] - c.get('dil', 1) * (c['k'] - 1) - 1) // c['s'] + 1
 
 
 def _probe_run(pp, bp, convs, runs, names=None, max_frames=F):
@@ -194,20 +194,21 @@ def test_short_batch_and_batch_position(tmp_path):
 
 
 def _direct_ref(c, X):
-    """float64 convolution of X [frame][cin][h][w] with ncnn weights [cout][cin or 1][k][k], symmetric zero padding: (R, S) as [frame][cout][oh][ow]"""
-    k, s, p, oh = c['k'], c['s'], c['p'], _out_hw(c)
+    """float64 convolution of X [frame][cin][h][w] with ncnn weights [cout][cin or 1][k][k], symmetric zero padding, dilation c['dil'] (default 1),
+    bias c['b'] (None: none): (R, S) as [frame][cout][oh][ow]"""
+    k, s, p, d, oh = c['k'], c['s'], c['p'], c.get('dil', 1), _out_hw(c)
     Xp = np.pad(X.astype(np.float64), ((0, 0), (0, 0), (p, p), (p, p)))
     W = c['w'].astype(np.float64)
     R = np.zeros((X.shape[0], c['cout'], oh, oh)); S = np.zeros_like(R)
     for ky in range(k):
         for kx in range(k):
-            patch = Xp[:, :, ky:ky + s * (oh - 1) + 1:s, kx:kx + s * (oh - 1) + 1:s]
+            patch = Xp[:, :, ky * d:ky * d + s * (oh - 1) + 1:s, kx * d:kx * d + s * (oh - 1) + 1:s]
             if c['dw']:
                 wk = W[:, 0, ky, kx][None, :, None, None]
                 R += patch * wk; S += np.abs(patch) * np.abs(wk)
             else:
                 R += np.einsum('fchw,oc->fohw', patch, W[:, :, ky, kx]); S += np.einsum('fchw,oc->fohw', np.abs(patch), np.abs(W[:, :, ky, kx]))
-    return R + c['b'][None, :, None, None], S
+    return (R if c['b'] is None else R + c['b'][None, :, None, None]), S
 
 
 def _direct_check(n, c, X, Y):
