@@ -395,6 +395,14 @@ typedef struct sgs_bow_batch {
     int32_t* nmatches;                                   /* out [F] */
 } sgs_bow_batch;
 SGS_API int sgs_match_bow_batch_device(const sgs_bow_batch* args, int nframes, void* stream);
+/* Frame::ComputeBoW's mBowVec (TemplatedVocabulary.h:1158-1175 with BowVector::addWeight, BowVector.cpp:34-46, and BowVector::normalize(L1),
+ * :62-84) from the per-feature output of sgs_bow_transform_batch_device: for each of `nframes` frames, the features i < d_counts[f] (clamped to
+ * [0, cap]) of weight > 0; each word's value is the sum of its features' weights in feature order, then divided by the L1 norm -- the serial sum of
+ * the values in ascending word order -- when that norm is > 0.  Outputs [F][cap]: word ids ascending in d_bow_word, their values in d_bow_value,
+ * d_bow_n [F] words.  Only TF-IDF weighting with L1 scoring, the configuration of the reference's ORBvoc.  cap at most 8192 (SGS_ERR_UNSUPPORTED).
+ * One block per frame on `stream`. */
+SGS_API int sgs_bow_vector_batch_device(const int32_t* d_word, const double* d_weight, const int32_t* d_counts, int cap, int nframes,
+                                        int32_t* d_bow_word, double* d_bow_value, int32_t* d_bow_n, void* stream);
 /* host-pointer variants: one descriptor set / one (key frame, frame) pair */
 SGS_API int sgs_bow_transform(const sgs_vocabulary* v, const uint8_t* desc, int n, int levelsup, int32_t* word, double* weight, int32_t* node);
 SGS_API int sgs_match_bow(int nkf, const int32_t* kf_node, const double* kf_weight, const uint8_t* kf_valid, const uint8_t* kf_desc,
@@ -695,6 +703,66 @@ typedef struct sgs_refkf_batch {
     int32_t* stats;                                    /* [F][8] */
 } sgs_refkf_batch;
 SGS_API int sgs_tracker_refkf_chain_device(sgs_tracker* t, const sgs_vocabulary* voc, const sgs_refkf_batch* args, int nframes, void* stream);
+
+/* ------------------------------------------------------------------------------------
+ * Relocalisation candidates: the first two lines of Tracking::Relocalization (src/Tracking.cc:1460-1467), Frame::ComputeBoW and
+ * KeyFrameDatabase::DetectRelocalizationCandidates (src/KeyFrameDatabase.cc:199-311), against a key-frame database on the device.
+ * sgs_kfdb is KeyFrameDatabase (:33-74) for max_maps independent maps (one per stream) in one handle, with max_keyframes slots shared by all maps;
+ * a slot holds one key frame's BowVector (at most max_words words) and its mRelocScore (include/KeyFrame.h:151).  Which key frames exist, their
+ * covisibility and what to do with the candidates stay with the caller.
+ *   sgs_kfdb_add     KeyFrameDatabase::add: key frame i (slot[i], map[i]: HOST arrays) with the BowVector of row i of d_bow_word / d_bow_value
+ *                    [n][bow_cap] and d_bow_n [n] (device, e.g. from sgs_bow_vector_batch_device) copied into the slot.  Each key frame takes the
+ *                    next value of a handle-wide add counter, in array order: it fixes the key frame's place in every inverted list (add pushes to
+ *                    the back).  mRelocScore is 0 after an add (the reference leaves it uninitialised, DESIGN.md Q16).  Reads d_bow_n to the host
+ *                    (synchronises `stream`).
+ *   sgs_kfdb_erase   KeyFrameDatabase::erase (KeyFrame::SetBadFlag): the slots leave their maps.
+ *   sgs_kfdb_clear   KeyFrameDatabase::clear for one map (Tracking::Reset, src/Tracking.cc:1646).
+ *   These refuse with SGS_ERR_INVALID, and change nothing: a slot out of range or already live (add; a slot given twice), a slot that is not live
+ *   (erase), an unknown map, a BowVector with more than max_words (or bow_cap) words.  SGS_ERR_CAPACITY after 2^40 adds.
+ *   sgs_kfdb_reloc_scores  every slot's mRelocScore [max_keyframes] to the host, after the caller has synchronised the queries' stream.
+ *   sgs_kfdb_reloc_candidates_device  DetectRelocalizationCandidates for `nframes` rows: row f (map[f], a HOST array; -1 skips the row, none of its
+ *       outputs is written) with the frame's BowVector in row f of d_bow_word / d_bow_value [F][bow_cap], d_bow_n [F].  The rows of one call name
+ *       distinct maps: the reference's state flows from one query to the next (Q16), and one frame per stream per call is how the stream step feeds
+ *       the tracker (SGS_ERR_INVALID otherwise).  d_covis [max_keyframes][10] (device, the caller's): each slot's GetBestCovisibilityKeyFrames(10)
+ *       (src/KeyFrame.cc:175-183) in that order, -1 padded.  Exactly as the reference:
+ *         the key frames of the map sharing at least one word with the frame, in lKFsSharingWords order (the frame's words ascending, then
+ *         inverted-list order = add order); minCommonWords = int(maxCommonWords * 0.8f); those above it are scored,
+ *         si = float(L1Scoring::score(F, KF)) (the float64 sum in ascending word order), and si becomes the slot's mRelocScore; the accumulation adds
+ *         mRelocScore of every neighbour that shares a word in this query -- a neighbour that was not scored contributes its stale score (Q16) --,
+ *         pBestKF by strict > from si; entries with accScore > 0.75f * bestAccScore (from 0) are kept and pBestKF deduplicated, first kept.
+ *       Outputs (device): d_cand [F][cand_cap] slot ids in the reference's order (-1 after the last), d_ncand [F], d_stats [F][4] = key frames
+ *       sharing a word, maxCommonWords, nscores, candidates before the cap (above cand_cap: truncated).  Every query counts as a new frame: the
+ *       reference's F->mnId == 0 corner (the initialisation frame, never relocalised) is not reproduced.
+ *   Limits: a queried map holds at most 16384 key frames (SGS_ERR_UNSUPPORTED, nothing enqueued); refused calls enqueue nothing.  Work is
+ *   enqueued on `stream`; the calls on one handle share its device state and scratch, so the caller orders them (one stream, or events).
+ * Out of scope: the per-candidate SearchByBoW / PnPsolver loop and the rest of Relocalization, DetectLoopCandidates, other weighting / scoring
+ * types of DBoW2 (only TF-IDF with L1, the reference's ORBvoc).
+ * ------------------------------------------------------------------------------------ */
+typedef struct sgs_kfdb sgs_kfdb;
+SGS_API int sgs_kfdb_create(int device, int max_maps, int max_keyframes, int max_words, sgs_kfdb** out);
+SGS_API void sgs_kfdb_destroy(sgs_kfdb* db);
+SGS_API int sgs_kfdb_add(sgs_kfdb* db, int n, const int32_t* slot, const int32_t* map, const int32_t* d_bow_word, const double* d_bow_value,
+                         const int32_t* d_bow_n, int bow_cap, void* stream);
+SGS_API int sgs_kfdb_erase(sgs_kfdb* db, int n, const int32_t* slot, void* stream);
+SGS_API int sgs_kfdb_clear(sgs_kfdb* db, int map, void* stream);
+SGS_API int sgs_kfdb_reloc_scores(const sgs_kfdb* db, float* out);
+SGS_API int sgs_kfdb_reloc_candidates_device(sgs_kfdb* db, int nframes, const int32_t* map, const int32_t* d_bow_word, const double* d_bow_value,
+                                             const int32_t* d_bow_n, int bow_cap, const int32_t* d_covis, int32_t* d_cand, int cand_cap,
+                                             int32_t* d_ncand, int32_t* d_stats, void* stream);
+/* Tracking::Relocalization's first two lines (src/Tracking.cc:1460-1467) on the device-resident frame of the last track or step call, for the rows
+ * frame_enable selects: Frame::ComputeBoW (sgs_bow_transform_batch_device with levelsup 4, then sgs_bow_vector_batch_device) and
+ * sgs_kfdb_reloc_candidates_device (KeyFrameDatabase.cc:199-311) against map[f].  Disabled rows are not written.  Limits as those calls; the
+ * tracker's keypoint cap at most 8192.  Enqueued on `stream` (NULL: the tracker's stream). */
+typedef struct sgs_reloc_batch {
+    const int32_t* map;                                /* HOST [F]: the map row f queries (enabled rows: distinct) */
+    const uint8_t* frame_enable;                       /* HOST [F] may be NULL = all; 0 = row untouched */
+    const int32_t* covis;                              /* DEVICE [max_keyframes][10], as sgs_kfdb_reloc_candidates_device */
+    int32_t* cand; int32_t cand_cap;                   /* outputs (device): [F][cand_cap] */
+    int32_t* ncand;                                    /* [F] */
+    int32_t* stats;                                    /* [F][4] */
+} sgs_reloc_batch;
+SGS_API int sgs_tracker_reloc_candidates_device(sgs_tracker* t, const sgs_vocabulary* voc, sgs_kfdb* db, const sgs_reloc_batch* args, int nframes,
+                                                void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------------------------
  * Object detector: Detector2D (src/Detector2D.cc:16-89, include/Detector2D.h:29-80) -- ncnn forward of the MobileNetV3-SSDLite graph

@@ -2,6 +2,7 @@
 //   DBoW2::TemplatedVocabulary::transform(features, BowVector&, FeatureVector&, levelsup)   Thirdparty/DBoW2/DBoW2/TemplatedVocabulary.h:1140-1272
 //       (Frame::ComputeBoW, src/Frame.cc:421-428, levelsup = 4): greedy descent of the k-ary tree by Hamming distance, first child wins ties;
 //   ORBmatcher::SearchByBoW(KeyFrame*, Frame&, vector<MapPoint*>&)                           src/ORBmatcher.cc:159-290.
+//   Frame::ComputeBoW's BowVector (TF-IDF weighting, L1 scoring): bow_vector_kernel, one block per frame, from the transform's per-feature output.
 // The vocabulary lives on the device as flat arrays (the table the multi-GPU bench broadcasts once at start-up).
 //   transform : one warp per descriptor, one lane per child, the arg-min over (distance, child order) by redux.sync.
 //   SearchByBoW: one block per (key frame, frame) pair.  Both feature sets are sorted by (node id, feature index) -- the order of
@@ -20,6 +21,7 @@
 #include <memory>
 #include <vector>
 
+#include "block_compact.cuh"
 #include "host_stage.cuh"
 #include "match_rules.cuh"
 #include "sgs_common.h"
@@ -234,6 +236,59 @@ __global__ void __launch_bounds__(kBowThreads) bow_search_kernel(const BowArgs A
 
 static int pow2_ge(int n) { int p = 1; while (p < n) p <<= 1; return p; }
 
+// Frame::ComputeBoW's BowVector, TF-IDF weighting with L1 scoring (TemplatedVocabulary.h:1158-1175, BowVector.cpp:34-46 and :62-84): one block per
+// frame.  The features of weight > 0 are sorted by (word, feature index); one thread per word run sums its weights in feature order (v = w_a; v += w_b);
+// one thread sums the L1 norm in ascending word order; every value is then divided by the norm when it is > 0.
+__global__ void __launch_bounds__(kBowThreads) bow_vector_kernel(const int32_t* __restrict__ word, const double* __restrict__ weight, const int32_t* __restrict__ counts,
+                                                                 int cap, int pow2, int32_t* __restrict__ out_word, double* __restrict__ out_value,
+                                                                 int32_t* __restrict__ out_n) {
+    extern __shared__ __align__(16) uint8_t smem[];
+    uint64_t* key = reinterpret_cast<uint64_t*>(smem);             // [pow2] (word << 32 | feature index), padding = all ones
+    double* val = reinterpret_cast<double*>(key + pow2);           // [cap] the per-word sums, in word order
+    int32_t* run = reinterpret_cast<int32_t*>(val + cap);          // [cap + 1] start of each word run in key, then the number of live keys
+    __shared__ int s_live;
+    __shared__ double s_norm;
+    const int f = blockIdx.x, tid = threadIdx.x;
+    const int n = min(max(counts[f], 0), cap);
+    const int64_t o = (int64_t)f * cap;
+    if (tid == 0) s_live = 0;
+    for (int i = tid; i < pow2; i += blockDim.x) {
+        uint64_t k = ~0ull;
+        if (i < n && weight[o + i] > 0) k = ((uint64_t)(uint32_t)word[o + i] << 32) | (uint32_t)i;      // not stopped (:1165)
+        key[i] = k;
+    }
+    __syncthreads();
+    bow_bitonic(key, pow2);
+    int nruns = 0;
+    for (int i0 = 0; i0 < pow2; i0 += kBowThreads) {
+        const int i = i0 + tid;
+        const bool live = i < pow2 && key[i] != ~0ull;
+        if (live && (i + 1 == pow2 || key[i + 1] == ~0ull)) s_live = i + 1;
+        const int r = block_ordered_slot<kBowThreads>(live && (i == 0 || (key[i - 1] >> 32) != (key[i] >> 32)), nruns);
+        if (r >= 0) run[r] = i;
+    }
+    __syncthreads();
+    if (tid == 0) run[nruns] = s_live;
+    __syncthreads();
+    for (int r = tid; r < nruns; r += blockDim.x) {                // BowVector::addWeight, in feature order
+        const int s = run[r], e = run[r + 1];
+        double v = weight[o + (uint32_t)key[s]];
+        for (int j = s + 1; j < e; ++j) v += weight[o + (uint32_t)key[j]];
+        val[r] = v;
+        out_word[o + r] = (int32_t)(key[s] >> 32);
+    }
+    __syncthreads();
+    if (tid == 0) {                                                 // BowVector::normalize(L1)
+        double norm = 0.0;
+        for (int r = 0; r < nruns; ++r) norm += fabs(val[r]);
+        s_norm = norm;
+        out_n[f] = nruns;
+    }
+    __syncthreads();
+    const double norm = s_norm;
+    for (int r = tid; r < nruns; r += blockDim.x) out_value[o + r] = norm > 0.0 ? val[r] / norm : val[r];
+}
+
 }  // namespace sgs
 
 using namespace sgs;
@@ -392,6 +447,19 @@ SGS_API int sgs_bow_transform_batch_device(const sgs_vocabulary* v, const uint8_
     dim3 grid((cap + 7) / 8, nframes);
     bow_transform_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(V, d_desc, d_counts, cap, levelsup, d_word, d_weight, d_node);
     SGS_CUDA_TRY(cudaGetLastError());
+    return SGS_OK;
+}
+
+SGS_API int sgs_bow_vector_batch_device(const int32_t* d_word, const double* d_weight, const int32_t* d_counts, int cap, int nframes,
+                                        int32_t* d_bow_word, double* d_bow_value, int32_t* d_bow_n, void* stream) {
+    const char* const fn = "sgs_bow_vector_batch_device";
+    if (!d_word || !d_weight || !d_counts || !d_bow_word || !d_bow_value || !d_bow_n || cap < 1 || nframes < 1) { set_error("%s: bad argument", fn); return SGS_ERR_INVALID; }
+    if (cap > 8192) { set_error("%s: at most 8192 features per frame (cap %d)", fn, cap); return SGS_ERR_UNSUPPORTED; }
+    const int p2 = pow2_ge(cap);
+    const size_t smem = 8 * (size_t)p2 + 8 * (size_t)cap + 4 * (size_t)(cap + 1);
+    if (smem > 40 * 1024) SGS_CUDA_TRY_AT(fn, cudaFuncSetAttribute(bow_vector_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    bow_vector_kernel<<<nframes, kBowThreads, smem, (cudaStream_t)stream>>>(d_word, d_weight, d_counts, cap, p2, d_bow_word, d_bow_value, d_bow_n);
+    SGS_CUDA_TRY_AT(fn, cudaGetLastError());
     return SGS_OK;
 }
 

@@ -2,6 +2,8 @@
 #pragma once
 #include <cuda_runtime.h>
 
+#include <vector>
+
 #include "sgs_common.h"
 
 namespace sgs {
@@ -37,5 +39,14 @@ struct FmArgs {
 };
 // sgs_fundamental_batch_device's launch
 int fm_launch(const FmArgs& a, cudaStream_t st);
+
+// ---- kfdb.cu
+// sgs_kfdb_reloc_candidates_device in two halves, so that a caller can refuse the call before it enqueues anything of its own.  The checks on the
+// host: map[f] == -1 skips row f, the other rows name distinct known maps (SGS_ERR_INVALID) of at most 16384 key frames (SGS_ERR_UNSUPPORTED); rows
+// receives (row, group offset, group length, map) of every queried row, *max_len the largest group.
+int kfdb_plan_query(const sgs_kfdb* db, const char* fn, int nframes, const int32_t* map, std::vector<int4>& rows, int* max_len);
+int kfdb_launch_query(sgs_kfdb* db, const char* fn, const std::vector<int4>& rows, int max_len, const int32_t* d_bow_word, const double* d_bow_value,
+                      const int32_t* d_bow_n, int bow_cap, const int32_t* d_covis, int32_t* d_cand, int cand_cap, int32_t* d_ncand, int32_t* d_stats,
+                      cudaStream_t st);
 
 }  // namespace sgs

@@ -84,6 +84,10 @@ struct sgs_tracker {
     int32_t* d_rk_word = nullptr; double* d_rk_weight = nullptr; int32_t* d_rk_node = nullptr; float* d_rk_ang = nullptr; uint8_t* d_rk_valid = nullptr;
     int32_t* d_rk_mp = nullptr; int32_t* d_rk_n = nullptr; int32_t* d_rk_kfn = nullptr; int32_t* d_rk_mpn = nullptr; int32_t* d_rk_nm = nullptr;
     uint8_t* d_rk_run = nullptr; float* d_rk_T1 = nullptr; float* d_rk_T2 = nullptr;
+    // sgs_tracker_reloc_candidates_device, sized on first use: the enabled rows, their keypoint counts (0 = disabled), the per-feature BoW [B][cap] and
+    // the frames' BowVectors [B][cap]
+    uint8_t* d_rl_en = nullptr; int32_t* d_rl_n = nullptr; int32_t* d_rl_word = nullptr; double* d_rl_weight = nullptr; int32_t* d_rl_node = nullptr;
+    int32_t* d_rl_bw = nullptr; double* d_rl_bv = nullptr; int32_t* d_rl_bn = nullptr;
     StreamState ss;                             // the RGB-D stream steps
 };
 
@@ -255,6 +259,11 @@ __global__ void refkf_commit_kernel(const uint8_t* __restrict__ run, const float
     const int f = blockIdx.x, q = threadIdx.x;
     if (!run[f] || q >= 16) return;
     tcw_refkf[16 * f + q] = T1[16 * f + q]; tcw_final[16 * f + q] = T2[16 * f + q];
+}
+// sgs_tracker_reloc_candidates_device: the keypoints of the enabled rows enter ComputeBoW, the disabled rows get none
+__global__ void reloc_counts_kernel(const uint8_t* __restrict__ enable, const int32_t* __restrict__ n_cur, int32_t* __restrict__ n_out, int nframes) {
+    const int f = blockIdx.x * blockDim.x + threadIdx.x;
+    if (f < nframes) n_out[f] = enable[f] ? n_cur[f] : 0;
 }
 // ---- the RGB-D stream steps (StreamState) ----------------------------------------------------------------------------------------------------
 // Per frame of a call, before LK: a first frame (its slot never held a frame, or new_stream[f]) tracks into its own image and has no previous frame;
@@ -989,6 +998,42 @@ SGS_API int sgs_tracker_refkf_chain_device(sgs_tracker* t, const sgs_vocabulary*
     refkf_commit_kernel<<<F, 32, 0, st>>>(t->d_rk_run, t->d_rk_T1, t->d_rk_T2, a->tcw_refkf, a->tcw_final);
     SGS_CUDA_TRY(cudaGetLastError());
     return SGS_OK;
+}
+
+SGS_API int sgs_tracker_reloc_candidates_device(sgs_tracker* t, const sgs_vocabulary* voc, sgs_kfdb* db, const sgs_reloc_batch* a, int nframes, void* stream) {
+    const char* const fn = "sgs_tracker_reloc_candidates_device";
+    if (!t || !voc || !db || !a) return bad(fn, "NULL");
+    if (!a->map || !a->covis || !a->cand || !a->ncand || !a->stats || a->cand_cap < 1) return bad(fn, "NULL array or cand_cap < 1");
+    if (!frames_ok(fn, nframes, t->last_nframes)) return SGS_ERR_INVALID;
+    if (t->cap > 8192) { set_error("%s: the BowVector takes at most 8192 features (cap %d)", fn, t->cap); return SGS_ERR_UNSUPPORTED; }
+    std::vector<int32_t> map(a->map, a->map + nframes);
+    std::vector<uint8_t> en(nframes, 1);
+    for (int f = 0; f < nframes; ++f)
+        if (a->frame_enable && !a->frame_enable[f]) { en[f] = 0; map[f] = -1; }
+        else if (map[f] < 0) return bad(fn, "an enabled row names no map");
+    std::vector<int4> rows;
+    int max_len = 0;
+    int rc = kfdb_plan_query(db, fn, nframes, map.data(), rows, &max_len);
+    if (rc != SGS_OK) return rc;
+    SGS_CUDA_TRY(cudaSetDevice(t->device));
+    cudaStream_t st = stream ? (cudaStream_t)stream : t->st;
+    if (!t->d_rl_bn) {      // allocated last: a failed first attempt is repeated whole by the next call
+        HandleResources& R = t->res;
+        const size_t B = t->max_batch, K = t->cap;
+        SGS_CUDA_TRY_AT(fn, R.regrow(&t->d_rl_en, B + 16)); SGS_CUDA_TRY_AT(fn, R.regrow(&t->d_rl_n, B * 4 + 16)); SGS_CUDA_TRY_AT(fn, R.regrow(&t->d_rl_word, B * K * 4 + 16));
+        SGS_CUDA_TRY_AT(fn, R.regrow(&t->d_rl_weight, B * K * 8 + 16)); SGS_CUDA_TRY_AT(fn, R.regrow(&t->d_rl_node, B * K * 4 + 16));
+        SGS_CUDA_TRY_AT(fn, R.regrow(&t->d_rl_bw, B * K * 4 + 16)); SGS_CUDA_TRY_AT(fn, R.regrow(&t->d_rl_bv, B * K * 8 + 16)); SGS_CUDA_TRY_AT(fn, R.regrow(&t->d_rl_bn, B * 4 + 16));
+    }
+    const int F = nframes, cap = t->cap;
+    // 1. Frame::ComputeBoW (:1463) of the enabled rows
+    SGS_CUDA_TRY_AT(fn, cudaMemcpyAsync(t->d_rl_en, en.data(), (size_t)F, cudaMemcpyHostToDevice, st));
+    reloc_counts_kernel<<<(F + 127) / 128, 128, 0, st>>>(t->d_rl_en, t->d_cnt2, t->d_rl_n, F);
+    rc = sgs_bow_transform_batch_device(voc, t->d_desc2, t->d_rl_n, cap, F, 4, t->d_rl_word, t->d_rl_weight, t->d_rl_node, st);
+    if (rc != SGS_OK) return rc;
+    rc = sgs_bow_vector_batch_device(t->d_rl_word, t->d_rl_weight, t->d_rl_n, cap, F, t->d_rl_bw, t->d_rl_bv, t->d_rl_bn, st);
+    if (rc != SGS_OK) return rc;
+    // 2. mpKeyFrameDB->DetectRelocalizationCandidates(&mCurrentFrame) (:1467)
+    return kfdb_launch_query(db, fn, rows, max_len, t->d_rl_bw, t->d_rl_bv, t->d_rl_bn, cap, a->covis, a->cand, a->cand_cap, a->ncand, a->stats, st);
 }
 
 // Detector2D::detect for the frames of the batch (src/Tracking.cc:288-307 hands the colour image to the detector thread; src/Frame.cc:478-500

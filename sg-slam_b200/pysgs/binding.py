@@ -113,6 +113,11 @@ class RefKfBatch(C.Structure):              # sgs_refkf_batch
                 ('tcw_refkf', C.c_void_p), ('tcw_final', C.c_void_p), ('f_mp', C.c_void_p), ('outlier', C.c_void_p), ('stats', C.c_void_p)]
 
 
+class RelocBatch(C.Structure):              # sgs_reloc_batch
+    _fields_ = [('map', C.c_void_p), ('frame_enable', C.c_void_p), ('covis', C.c_void_p), ('cand', C.c_void_p), ('cand_cap', C.c_int32),
+                ('ncand', C.c_void_p), ('stats', C.c_void_p)]
+
+
 class FuseBatch(C.Structure):
     _fields_ = [('cam', Camera), ('kf_kps', C.c_void_p), ('kf_desc', C.c_void_p), ('kf_uright', C.c_void_p), ('kf_n', C.c_void_p), ('kf_cap', C.c_int32),
                 ('tcw', C.c_void_p), ('ow', C.c_void_p), ('mp_xyz', C.c_void_p), ('mp_normal', C.c_void_p), ('mp_min_dist', C.c_void_p), ('mp_max_dist', C.c_void_p),
