@@ -705,8 +705,9 @@ typedef struct sgs_refkf_batch {
 SGS_API int sgs_tracker_refkf_chain_device(sgs_tracker* t, const sgs_vocabulary* voc, const sgs_refkf_batch* args, int nframes, void* stream);
 
 /* ------------------------------------------------------------------------------------
- * Relocalisation candidates: the first two lines of Tracking::Relocalization (src/Tracking.cc:1460-1467), Frame::ComputeBoW and
- * KeyFrameDatabase::DetectRelocalizationCandidates (src/KeyFrameDatabase.cc:199-311), against a key-frame database on the device.
+ * Relocalisation and loop candidates: the first two lines of Tracking::Relocalization (src/Tracking.cc:1460-1467), Frame::ComputeBoW and
+ * KeyFrameDatabase::DetectRelocalizationCandidates (src/KeyFrameDatabase.cc:199-311), and KeyFrameDatabase::DetectLoopCandidates (:76-197), against
+ * a key-frame database on the device.
  * sgs_kfdb is KeyFrameDatabase (:33-74) for max_maps independent maps (one per stream) in one handle, with max_keyframes slots shared by all maps;
  * a slot holds one key frame's BowVector (at most max_words words) and its mRelocScore (include/KeyFrame.h:151).  Which key frames exist, their
  * covisibility and what to do with the candidates stay with the caller.
@@ -733,10 +734,30 @@ SGS_API int sgs_tracker_refkf_chain_device(sgs_tracker* t, const sgs_vocabulary*
  *       Outputs (device): d_cand [F][cand_cap] slot ids in the reference's order (-1 after the last), d_ncand [F], d_stats [F][4] = key frames
  *       sharing a word, maxCommonWords, nscores, candidates before the cap (above cand_cap: truncated).  Every query counts as a new frame: the
  *       reference's F->mnId == 0 corner (the initialisation frame, never relocalised) is not reproduced.
+ *   sgs_kfdb_loop_candidates_device  KeyFrameDatabase::DetectLoopCandidates(pKF, minScore) (:76-197) for `nframes` rows, with minScore computed
+ *       as LoopClosing::DetectLoop does (src/LoopClosing.cc:124-138).  Row f is a new key frame of map[f] (HOST; -1 skips the row, none of its
+ *       outputs is written; the rows of one call name distinct maps, as for the relocalisation query) with its BowVector in row f of d_bow_word /
+ *       d_bow_value [F][bow_cap], d_bow_n [F].  Its connected key frames (KeyFrame::GetConnectedKeyFrames, src/KeyFrame.cc:160-167: every key
+ *       frame with a covisibility weight) are the slot ids d_conn[conn_off[f] .. conn_off[f+1]) (device ids, HOST offsets [F+1]); ids that are not
+ *       live in map[f] are ignored.  Its covisible key frames (GetVectorCovisibleKeyFrames, :169-173, the isBad() ones left out by the caller) are
+ *       the BowVectors in rows [cov_off[f] .. cov_off[f+1]) of d_cov_word / d_cov_value [C][bow_cap] and d_cov_n [C] (device, HOST offsets [F+1]):
+ *       BowVectors rather than slots, because DetectLoop adds the key frame to the database after the query (:215), so a lagging loop closer
+ *       sees covisible key frames that are not in it yet.  d_covis as for the relocalisation query.  Exactly as the reference:
+ *         minScore = 1, then the least float(L1Scoring::score(pKF, KF)) over the covisible rows in order by strict <;
+ *         lKFsSharingWords: the key frames of the map sharing a word with pKF that are not connected to it, in the relocalisation query's order;
+ *         a connected key frame counts towards neither the list nor maxCommonWords; minCommonWords = int(maxCommonWords * 0.8f); those above it
+ *         are scored (nscores) and enter the list of matches if si >= minScore; the accumulation adds the si of every neighbour listed in this
+ *         query above minCommonWords, pBestKF by strict > from si; bestAccScore starts at minScore; entries with accScore > 0.75f * bestAccScore
+ *         are kept and pBestKF deduplicated, first kept.
+ *       Outputs (device): d_cand [F][cand_cap], d_ncand [F], d_stats [F][4] as for the relocalisation query (stats[0]: the non-connected key frames
+ *       sharing a word), d_min_score [F].  Every query counts as a new key frame; a key frame already added is its own candidate, as in the
+ *       reference (DESIGN.md Q17).  The query keeps no per-slot state: it neither reads nor writes mRelocScore.  SGS_ERR_INVALID also for CSR
+ *       offsets that are negative or decrease, and for connected ids or covisible rows given with a NULL array.
  *   Limits: a queried map holds at most 16384 key frames (SGS_ERR_UNSUPPORTED, nothing enqueued); refused calls enqueue nothing.  Work is
- *   enqueued on `stream`; the calls on one handle share its device state and scratch, so the caller orders them (one stream, or events).
- * Out of scope: the per-candidate SearchByBoW / PnPsolver loop and the rest of Relocalization, DetectLoopCandidates, other weighting / scoring
- * types of DBoW2 (only TF-IDF with L1, the reference's ORBvoc).
+ *   enqueued on `stream`; the calls on one handle (add, erase, clear and both queries) share its device state and per-slot scratch, so the caller
+ *   orders them (one stream, or events).
+ * Out of scope: the per-candidate SearchByBoW / PnPsolver loop and the rest of Relocalization, DetectLoop's consistency groups and what follows it,
+ * other weighting / scoring types of DBoW2 (only TF-IDF with L1, the reference's ORBvoc).
  * ------------------------------------------------------------------------------------ */
 typedef struct sgs_kfdb sgs_kfdb;
 SGS_API int sgs_kfdb_create(int device, int max_maps, int max_keyframes, int max_words, sgs_kfdb** out);
@@ -749,6 +770,10 @@ SGS_API int sgs_kfdb_reloc_scores(const sgs_kfdb* db, float* out);
 SGS_API int sgs_kfdb_reloc_candidates_device(sgs_kfdb* db, int nframes, const int32_t* map, const int32_t* d_bow_word, const double* d_bow_value,
                                              const int32_t* d_bow_n, int bow_cap, const int32_t* d_covis, int32_t* d_cand, int cand_cap,
                                              int32_t* d_ncand, int32_t* d_stats, void* stream);
+SGS_API int sgs_kfdb_loop_candidates_device(sgs_kfdb* db, int nframes, const int32_t* map, const int32_t* d_bow_word, const double* d_bow_value,
+                                            const int32_t* d_bow_n, int bow_cap, const int32_t* conn_off, const int32_t* d_conn, const int32_t* cov_off,
+                                            const int32_t* d_cov_word, const double* d_cov_value, const int32_t* d_cov_n, const int32_t* d_covis,
+                                            int32_t* d_cand, int cand_cap, int32_t* d_ncand, int32_t* d_stats, float* d_min_score, void* stream);
 /* Tracking::Relocalization's first two lines (src/Tracking.cc:1460-1467) on the device-resident frame of the last track or step call, for the rows
  * frame_enable selects: Frame::ComputeBoW (sgs_bow_transform_batch_device with levelsup 4, then sgs_bow_vector_batch_device) and
  * sgs_kfdb_reloc_candidates_device (KeyFrameDatabase.cc:199-311) against map[f].  Disabled rows are not written.  Limits as those calls; the

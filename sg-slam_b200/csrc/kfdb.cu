@@ -9,6 +9,8 @@
 //                        ascending word order;
 //          row kernel    one block per row: maxCommonWords and the 0.8 gate, mRelocScore of the scored key frames, their (first common word, add
 //                        counter) sort, the covisibility accumulation, the 0.75 retention and the pBestKF dedupe in list order.
+// The loop query KeyFrameDatabase::DetectLoopCandidates (:76-197), with LoopClosing::DetectLoop's minScore, runs the same pair kernel, then a prep
+// kernel (the connected key frames leave the sharing set; minScore against the covisible BowVectors), then the row kernel with the loop rules.
 // Floating point: the score is DBoW2's float64 sum in DBoW2's order, rounded to float once; the accumulation is float in the reference's order.
 #include <cuda_runtime.h>
 
@@ -47,6 +49,8 @@ struct sgs_kfdb {
     int32_t* d_cnt = nullptr; int32_t* d_first = nullptr; float* d_si = nullptr; int32_t* d_mark = nullptr;
     // add: the slots, add counters and source rows of one call; query: per row (row, group offset, group length, map)
     int32_t* d_add_slot = nullptr; uint64_t* d_add_seq = nullptr; int4* d_rows = nullptr;
+    // loop query: per row (connected ids begin, end, covisible rows begin, end)
+    int4* d_loop = nullptr;
 };
 
 namespace sgs {
@@ -69,20 +73,12 @@ struct KfdbDev {
     float* score; int32_t* cnt; int32_t* first; float* si; int32_t* mark;
 };
 
-// :207-222 mnRelocWords and the first common word, and :249 L1Scoring::score (ScoringObject.cpp:23-68) for every key frame of the row's map
-__global__ void __launch_bounds__(256) kfdb_pair_kernel(const KfdbDev D, const int4* __restrict__ rows, const int32_t* __restrict__ fw_all,
-                                                        const double* __restrict__ fv_all, const int32_t* __restrict__ fn_all, int bow_cap) {
-    const int4 row = rows[blockIdx.y];
-    const int p = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
-    if (p >= row.z) return;
-    const int slot = D.group[row.y + p];
-    const int nf = min(max(fn_all[row.x], 0), bow_cap);
-    const int32_t* fw = fw_all + (int64_t)row.x * bow_cap;
-    const double* fv = fv_all + (int64_t)row.x * bow_cap;
-    const int nk = D.n[slot];
-    const int32_t* kw = D.word + (int64_t)slot * D.max_words;
-    const double* kv = D.value + (int64_t)slot * D.max_words;
-    int cnt = 0, first = -1;
+// One warp: the words the frame's BowVector (fw, fv: nf words) shares with a key frame's (kw, kv: nk words), the index of the first of them in the
+// frame's BowVector (-1: none), and float(L1Scoring::score(F, KF)) (ScoringObject.cpp:23-68): every frame word binary-searched in the key frame's,
+// the terms per lane, their float64 sum serial in ascending word order.  Every lane returns the same values.
+__device__ __forceinline__ float warp_l1_score(const int32_t* fw, const double* fv, int nf, const int32_t* __restrict__ kw, const double* __restrict__ kv,
+                                               int nk, int lane, int& cnt, int& first) {
+    cnt = 0; first = -1;
     double score = 0.0;
     for (int c0 = 0; c0 < nf && nk > 0; c0 += 32) {
         const int i = c0 + lane;
@@ -107,11 +103,53 @@ __global__ void __launch_bounds__(256) kfdb_pair_kernel(const KfdbDev D, const i
             m &= m - 1;
         }
     }
-    if (lane == 0) {
-        D.cnt[slot] = cnt; D.first[slot] = first;
-        score = -score / 2.0;
-        D.si[slot] = __double2float_rn(score);
+    return __double2float_rn(-score / 2.0);
+}
+
+// :207-222 mnRelocWords and the first common word, and :249 L1Scoring::score for every key frame of the row's map
+__global__ void __launch_bounds__(256) kfdb_pair_kernel(const KfdbDev D, const int4* __restrict__ rows, const int32_t* __restrict__ fw_all,
+                                                        const double* __restrict__ fv_all, const int32_t* __restrict__ fn_all, int bow_cap) {
+    const int4 row = rows[blockIdx.y];
+    const int p = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+    if (p >= row.z) return;
+    const int slot = D.group[row.y + p];
+    const int nf = min(max(fn_all[row.x], 0), bow_cap);
+    int cnt, first;
+    const float si = warp_l1_score(fw_all + (int64_t)row.x * bow_cap, fv_all + (int64_t)row.x * bow_cap, nf, D.word + (int64_t)slot * D.max_words,
+                                   D.value + (int64_t)slot * D.max_words, D.n[slot], lane, cnt, first);
+    if (lane == 0) { D.cnt[slot] = cnt; D.first[slot] = first; D.si[slot] = si; }
+}
+
+// LoopClosing.cc:124-138 and KeyFrameDatabase.cc:78, after the pair pass, one block per row: the connected key frames (KeyFrame.cc:160-167) of the
+// row's map get a common-word count of 0, so that they neither enter lKFsSharingWords nor count as sharing neighbours; minScore, from 1 the least
+// score against the covisible BowVectors, one warp per BowVector.  The least (score, visiting index) is kept, so a zero minimum has the sign of the
+// first zero the reference meets (DESIGN.md Q17).  loop[q] = (connected ids begin, end, covisible rows begin, end).
+__global__ void __launch_bounds__(256) kfdb_loop_prep_kernel(const KfdbDev D, const int4* __restrict__ rows, const int4* __restrict__ loop,
+                                                             const int32_t* __restrict__ fw_all, const double* __restrict__ fv_all,
+                                                             const int32_t* __restrict__ fn_all, int bow_cap, const int32_t* __restrict__ conn,
+                                                             const int32_t* __restrict__ cw, const double* __restrict__ cv, const int32_t* __restrict__ cn,
+                                                             float* __restrict__ min_score) {
+    __shared__ unsigned long long s_min;                                    // |score| bits << 32 | visiting index << 1 | sign
+    const int4 row = rows[blockIdx.x], lr = loop[blockIdx.x];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    if (threadIdx.x == 0) s_min = (unsigned long long)__float_as_uint(1.f) << 32 | 0xfffffffeu;
+    for (int i = lr.x + threadIdx.x; i < lr.y; i += blockDim.x) {
+        const int s = conn[i];
+        if (s >= 0 && s < D.max_keyframes && D.map[s] == row.w) D.cnt[s] = 0;
     }
+    __syncthreads();
+    const int nf = min(max(fn_all[row.x], 0), bow_cap);
+    unsigned long long best = ~0ull;
+    for (int c = lr.z + warp; c < lr.w; c += 8) {
+        int cnt, first;
+        const float sc = warp_l1_score(fw_all + (int64_t)row.x * bow_cap, fv_all + (int64_t)row.x * bow_cap, nf, cw + (int64_t)c * bow_cap,
+                                       cv + (int64_t)c * bow_cap, min(max(cn[c], 0), bow_cap), lane, cnt, first);
+        const unsigned bits = __float_as_uint(sc);
+        best = min(best, (unsigned long long)(bits & 0x7fffffffu) << 32 | (unsigned)(c - lr.z) << 1 | bits >> 31);
+    }
+    if (lane == 0) atomicMin(&s_min, best);
+    __syncthreads();
+    if (threadIdx.x == 0) min_score[row.x] = __uint_as_float((unsigned)(s_min >> 32) | (unsigned)(s_min & 1) << 31);
 }
 
 __device__ void sort_with_slots(uint64_t* key, int32_t* slot, int n_pow2) {         // ascending, padding = all ones
@@ -130,17 +168,22 @@ __device__ void sort_with_slots(uint64_t* key, int32_t* slot, int n_pow2) {     
 
 // :224-308 for one row: the gate, mRelocScore, lKFsSharingWords order of the scored key frames, accumulation over the covisibility table, retention,
 // dedupe.  stats: key frames sharing a word, maxCommonWords, nscores, candidates before the cap.
+// kLoop: DetectLoopCandidates' :107-193 instead, on the counts kfdb_loop_prep_kernel left (connected key frames do not share): only the scored key
+// frames with si >= minScore are listed, a neighbour adds its si of this query if it is above the gate, bestAccScore starts at minScore, and
+// mRelocScore is not touched.
+template <bool kLoop>
 __global__ void __launch_bounds__(kRowThreads) kfdb_row_kernel(const KfdbDev D, const int4* __restrict__ rows, const int32_t* __restrict__ covis,
                                                                int p2, int32_t* __restrict__ cand, int cand_cap, int32_t* __restrict__ ncand,
-                                                               int32_t* __restrict__ stats) {
+                                                               int32_t* __restrict__ stats, const float* __restrict__ min_score) {
     extern __shared__ __align__(16) uint8_t smem[];
     const int4 row = rows[blockIdx.x];
     uint64_t* key = reinterpret_cast<uint64_t*>(smem);             // [p2] sort keys (first common word's index << 40 | add counter), then (acc, pBestKF)
     int32_t* kslot = reinterpret_cast<int32_t*>(key + p2);          // [p2] the slot of each key
-    __shared__ int s_share, s_max, s_nsc, s_best;
+    __shared__ int s_share, s_max, s_nsc, s_best, s_scored;
     const int tid = threadIdx.x, f = row.x, map = row.w, len = row.z;
+    const float min_si = kLoop ? min_score[f] : 0.f;                // lScoreAndMatch's least si and bestAccScore's start
     const int32_t* grp = D.group + row.y;
-    if (tid == 0) { s_share = 0; s_max = 0; s_nsc = 0; s_best = 0; }
+    if (tid == 0) { s_share = 0; s_max = 0; s_nsc = 0; s_best = __float_as_int(min_si); s_scored = 0; }
     __syncthreads();
     int share = 0, mx = 0;
     for (int p = tid; p < len; p += kRowThreads) {
@@ -155,7 +198,9 @@ __global__ void __launch_bounds__(kRowThreads) kfdb_row_kernel(const KfdbDev D, 
     for (int p = tid; p < len; p += kRowThreads) {
         const int s = grp[p];
         if (nshare > 0 && D.cnt[s] > minc) {
-            D.score[s] = D.si[s];
+            if (kLoop) atomicAdd(&s_scored, 1);
+            else D.score[s] = D.si[s];
+            if (kLoop && !(D.si[s] >= min_si)) continue;            // :136
             const int q = atomicAdd(&s_nsc, 1);
             key[q] = ((uint64_t)D.first[s] << 40) | D.seq[s];
             kslot[q] = s;
@@ -168,20 +213,21 @@ __global__ void __launch_bounds__(kRowThreads) kfdb_row_kernel(const KfdbDev D, 
     for (int q = nsc + tid; q < n2; q += kRowThreads) { key[q] = ~0ull; kslot[q] = -1; }
     __syncthreads();
     if (nsc > 1) sort_with_slots(key, kslot, n2);
-    // :262-287 accumulation by covisibility: neighbours that share a word in this query (mnRelocQuery == F->mnId), fresh or stale mRelocScore (Q16)
+    // :262-287 accumulation by covisibility: neighbours that share a word in this query (mnRelocQuery == F->mnId), fresh or stale mRelocScore (Q16).
+    // The loop query's neighbours (:159) are listed in this query and above the gate, so every score it reads is this query's si.
     for (int q = tid; q < nsc; q += kRowThreads) {
         const int s = kslot[q];
         float best = D.si[s], acc = best;
         int pbest = s;
         for (int k = 0; k < 10; ++k) {
             const int nb = covis[(int64_t)s * 10 + k];
-            if (nb < 0 || nb >= D.max_keyframes || D.map[nb] != map || D.cnt[nb] <= 0) continue;
-            const float sc = D.score[nb];
+            if (nb < 0 || nb >= D.max_keyframes || D.map[nb] != map || D.cnt[nb] <= (kLoop ? minc : 0)) continue;
+            const float sc = kLoop ? D.si[nb] : D.score[nb];
             acc = __fadd_rn(acc, sc);
             if (sc > best) { pbest = nb; best = sc; }
         }
         key[q] = ((uint64_t)(uint32_t)__float_as_int(acc) << 32) | (uint32_t)pbest;
-        if (acc > 0.f) atomicMax(&s_best, __float_as_int(acc));     // positive floats order as their bits; bestAccScore starts at 0
+        if (acc > min_si) atomicMax(&s_best, __float_as_int(acc)); // non-negative floats order as their bits (-0 as the least)
     }
     __syncthreads();
     const float keep_above = __fmul_rn(0.75f, __int_as_float(s_best));   // :290
@@ -203,7 +249,7 @@ __global__ void __launch_bounds__(kRowThreads) kfdb_row_kernel(const KfdbDev D, 
     for (int q = total + tid; q < cand_cap; q += kRowThreads) out[q] = -1;
     if (tid == 0) {
         ncand[f] = min(total, cand_cap);
-        stats[4 * f] = nshare; stats[4 * f + 1] = maxc; stats[4 * f + 2] = nsc; stats[4 * f + 3] = total;
+        stats[4 * f] = nshare; stats[4 * f + 1] = maxc; stats[4 * f + 2] = kLoop ? s_scored : nsc; stats[4 * f + 3] = total;
     }
 }
 
@@ -227,9 +273,16 @@ int kfdb_plan_query(const sgs_kfdb* db, const char* fn, int nframes, const int32
     return SGS_OK;
 }
 
-int kfdb_launch_query(sgs_kfdb* db, const char* fn, const std::vector<int4>& rows, int max_len, const int32_t* d_bow_word, const double* d_bow_value,
-                      const int32_t* d_bow_n, int bow_cap, const int32_t* d_covis, int32_t* d_cand, int cand_cap, int32_t* d_ncand, int32_t* d_stats,
-                      cudaStream_t st) {
+// the loop query's inputs beyond the relocalisation query's: per queried row (connected ids begin, end, covisible rows begin, end) and the arrays
+struct KfdbLoop {
+    std::vector<int4> ranges;
+    const int32_t* conn; const int32_t* cov_word; const double* cov_value; const int32_t* cov_n; float* min_score;
+};
+
+// pair kernel, [loop prep kernel,] row kernel: the relocalisation query, or the loop query when loop is not NULL
+int launch_query(sgs_kfdb* db, const char* fn, const std::vector<int4>& rows, int max_len, const int32_t* d_bow_word, const double* d_bow_value,
+                 const int32_t* d_bow_n, int bow_cap, const int32_t* d_covis, int32_t* d_cand, int cand_cap, int32_t* d_ncand, int32_t* d_stats,
+                 const KfdbLoop* loop, cudaStream_t st) {
     if (rows.empty()) return SGS_OK;
     SGS_CUDA_TRY_AT(fn, cudaSetDevice(db->device));
     const int nq = (int)rows.size();
@@ -240,13 +293,26 @@ int kfdb_launch_query(sgs_kfdb* db, const char* fn, const std::vector<int4>& row
         kfdb_pair_kernel<<<dim3((max_len + 7) / 8, nq), 256, 0, st>>>(D, db->d_rows, d_bow_word, d_bow_value, d_bow_n, bow_cap);
         SGS_CUDA_TRY_AT(fn, cudaGetLastError());
     }
+    if (loop) {
+        SGS_CUDA_TRY_AT(fn, cudaMemcpyAsync(db->d_loop, loop->ranges.data(), sizeof(int4) * nq, cudaMemcpyHostToDevice, st));
+        kfdb_loop_prep_kernel<<<nq, 256, 0, st>>>(D, db->d_rows, db->d_loop, d_bow_word, d_bow_value, d_bow_n, bow_cap, loop->conn, loop->cov_word,
+                                                  loop->cov_value, loop->cov_n, loop->min_score);
+        SGS_CUDA_TRY_AT(fn, cudaGetLastError());
+    }
     int p2 = 1;
     while (p2 < max_len) p2 <<= 1;
     const size_t smem = 12 * (size_t)p2 + 16;
-    if (smem > 40 * 1024) SGS_CUDA_TRY_AT(fn, cudaFuncSetAttribute(kfdb_row_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    kfdb_row_kernel<<<nq, kRowThreads, smem, st>>>(D, db->d_rows, d_covis, p2, d_cand, cand_cap, d_ncand, d_stats);
+    auto row_kernel = loop ? kfdb_row_kernel<true> : kfdb_row_kernel<false>;
+    if (smem > 40 * 1024) SGS_CUDA_TRY_AT(fn, cudaFuncSetAttribute(row_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    row_kernel<<<nq, kRowThreads, smem, st>>>(D, db->d_rows, d_covis, p2, d_cand, cand_cap, d_ncand, d_stats, loop ? loop->min_score : nullptr);
     SGS_CUDA_TRY_AT(fn, cudaGetLastError());
     return SGS_OK;
+}
+
+int kfdb_launch_query(sgs_kfdb* db, const char* fn, const std::vector<int4>& rows, int max_len, const int32_t* d_bow_word, const double* d_bow_value,
+                      const int32_t* d_bow_n, int bow_cap, const int32_t* d_covis, int32_t* d_cand, int cand_cap, int32_t* d_ncand, int32_t* d_stats,
+                      cudaStream_t st) {
+    return launch_query(db, fn, rows, max_len, d_bow_word, d_bow_value, d_bow_n, bow_cap, d_covis, d_cand, cand_cap, d_ncand, d_stats, nullptr, st);
 }
 
 }  // namespace sgs
@@ -289,6 +355,7 @@ SGS_API int sgs_kfdb_create(int device, int max_maps, int max_keyframes, int max
     SGS_CUDA_TRY_AT(fn, R.alloc(&db->d_group, K * 4)); SGS_CUDA_TRY_AT(fn, R.alloc(&db->d_cnt, K * 4)); SGS_CUDA_TRY_AT(fn, R.alloc(&db->d_first, K * 4));
     SGS_CUDA_TRY_AT(fn, R.alloc(&db->d_si, K * 4)); SGS_CUDA_TRY_AT(fn, R.alloc(&db->d_mark, K * 4)); SGS_CUDA_TRY_AT(fn, R.alloc(&db->d_add_slot, K * 4));
     SGS_CUDA_TRY_AT(fn, R.alloc(&db->d_add_seq, K * 8)); SGS_CUDA_TRY_AT(fn, R.alloc(&db->d_rows, sizeof(int4) * (size_t)max_maps));
+    SGS_CUDA_TRY_AT(fn, R.alloc(&db->d_loop, sizeof(int4) * (size_t)max_maps));
     SGS_CUDA_TRY_AT(fn, cudaMemset(db->d_score, 0, K * 4)); SGS_CUDA_TRY_AT(fn, cudaMemset(db->d_n, 0, K * 4));
     if (publish_groups(db.get(), fn, nullptr) != SGS_OK) return SGS_ERR_CUDA;
     SGS_CUDA_TRY_AT(fn, cudaDeviceSynchronize());
@@ -371,6 +438,35 @@ SGS_API int sgs_kfdb_reloc_candidates_device(sgs_kfdb* db, int nframes, const in
     const int rc = kfdb_plan_query(db, fn, nframes, map, rows, &max_len);
     if (rc != SGS_OK) return rc;
     return kfdb_launch_query(db, fn, rows, max_len, d_bow_word, d_bow_value, d_bow_n, bow_cap, d_covis, d_cand, cand_cap, d_ncand, d_stats, (cudaStream_t)stream);
+}
+
+// CSR offsets off[0 .. nframes] (host): from 0 or more, not decreasing
+static bool offsets_ok(const int32_t* off, int nframes) {
+    if (off[0] < 0) return false;
+    for (int f = 0; f < nframes; ++f) if (off[f + 1] < off[f]) return false;
+    return true;
+}
+
+SGS_API int sgs_kfdb_loop_candidates_device(sgs_kfdb* db, int nframes, const int32_t* map, const int32_t* d_bow_word, const double* d_bow_value,
+                                            const int32_t* d_bow_n, int bow_cap, const int32_t* conn_off, const int32_t* d_conn, const int32_t* cov_off,
+                                            const int32_t* d_cov_word, const double* d_cov_value, const int32_t* d_cov_n, const int32_t* d_covis,
+                                            int32_t* d_cand, int cand_cap, int32_t* d_ncand, int32_t* d_stats, float* d_min_score, void* stream) {
+    const char* const fn = "sgs_kfdb_loop_candidates_device";
+    if (!db || !map || nframes < 1 || !d_bow_word || !d_bow_value || !d_bow_n || !conn_off || !cov_off || !d_covis || !d_cand || !d_ncand || !d_stats ||
+        !d_min_score || cand_cap < 1 || bow_cap < 1) {
+        set_error("%s: bad argument", fn); return SGS_ERR_INVALID; }
+    if (bow_cap > kMaxBowCap) { set_error("%s: bow_cap %d above %d", fn, bow_cap, kMaxBowCap); return SGS_ERR_UNSUPPORTED; }
+    if (!offsets_ok(conn_off, nframes) || !offsets_ok(cov_off, nframes)) { set_error("%s: CSR offsets negative or decreasing", fn); return SGS_ERR_INVALID; }
+    if ((conn_off[nframes] > conn_off[0] && !d_conn) || (cov_off[nframes] > cov_off[0] && (!d_cov_word || !d_cov_value || !d_cov_n))) {
+        set_error("%s: connected ids or covisible BowVectors given without their arrays", fn); return SGS_ERR_INVALID; }
+    std::vector<int4> rows;
+    int max_len = 0;
+    const int rc = kfdb_plan_query(db, fn, nframes, map, rows, &max_len);
+    if (rc != SGS_OK) return rc;
+    KfdbLoop loop{{}, d_conn, d_cov_word, d_cov_value, d_cov_n, d_min_score};
+    for (const int4& r : rows) loop.ranges.push_back(make_int4(conn_off[r.x], conn_off[r.x + 1], cov_off[r.x], cov_off[r.x + 1]));
+    return launch_query(db, fn, rows, max_len, d_bow_word, d_bow_value, d_bow_n, bow_cap, d_covis, d_cand, cand_cap, d_ncand, d_stats, &loop,
+                        (cudaStream_t)stream);
 }
 
 }  // extern "C"
