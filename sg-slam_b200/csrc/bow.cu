@@ -71,18 +71,6 @@ __global__ void __launch_bounds__(256) bow_transform_kernel(const VocDev V, cons
     if (lane == 0) { word[o] = V.word[cur]; weight[o] = V.weight[cur]; node[o] = nid; }
 }
 
-struct BowArgs {
-    const int32_t* kf_node; const double* kf_weight; const uint8_t* kf_valid; const uint8_t* kf_desc; const float* kf_angle; const int32_t* kf_n; int kf_cap;
-    const int32_t* f_node; const double* f_weight; const uint8_t* f_valid; const uint8_t* f_desc; const float* f_angle; const int32_t* f_n; int f_cap;
-    float nnratio; int check_ori;
-    int pair_mode;              // 1: SearchByBoW(KF1, KF2): strict < TH_LOW, second side needs map points, result indexed by the first side
-                                // 2: SearchForTriangulation: no ratio test, epipole + epipolar-line gates, last of equal distances wins
-    const uint8_t* kf_stereo; const uint8_t* f_stereo; const float* kf_xy; const float* f_xy; const int32_t* f_octave;
-    const float* F12; const float* epipole; float sigma2[16], scale[16]; int only_stereo;
-    int32_t* match_f; int32_t* nmatches;
-    int kf_pow2, f_pow2;
-};
-
 __device__ void bow_bitonic(uint64_t* keys, int n_pow2) {         // ascending, n_pow2 a power of two, padding = all ones
     for (int k = 2; k <= n_pow2; k <<= 1)
         for (int j = k >> 1; j > 0; j >>= 1) {
@@ -98,13 +86,15 @@ __device__ void bow_bitonic(uint64_t* keys, int n_pow2) {         // ascending, 
         }
 }
 
-// keys: (node id << 32 | feature index)
-__global__ void __launch_bounds__(kBowThreads) bow_search_kernel(const BowArgs A) {
+// keys: (node id << 32 | feature index); kf_pow2 / f_pow2: kf_cap / f_cap rounded up to a power of two (the sorted key arrays).  They are
+// __grid_constant__ like A, so the kernel reads them from the parameter bank where it uses them instead of holding them in registers throughout.
+__global__ void __launch_bounds__(kBowThreads) bow_search_kernel(const __grid_constant__ sgs_bow_batch A, const __grid_constant__ int kf_pow2,
+                                                                 const __grid_constant__ int f_pow2) {
     extern __shared__ __align__(16) uint8_t smem[];
     uint64_t* kkey = reinterpret_cast<uint64_t*>(smem);            // [kf_pow2]
-    uint64_t* fkey = kkey + A.kf_pow2;                              // [f_pow2]
-    int32_t* run_start = reinterpret_cast<int32_t*>(fkey + A.f_pow2);   // [kf_pow2 + 1]
-    int32_t* events = run_start + A.kf_pow2 + 1;                    // [max(kf_cap, f_cap)] (bin << 16 | index in the result array)
+    uint64_t* fkey = kkey + kf_pow2;                                // [f_pow2]
+    int32_t* run_start = reinterpret_cast<int32_t*>(fkey + f_pow2);     // [kf_pow2 + 1]
+    int32_t* events = run_start + kf_pow2 + 1;                      // [max(kf_cap, f_cap)] (bin << 16 | index in the result array)
     uint8_t* taken = reinterpret_cast<uint8_t*>(events + max(A.kf_cap, A.f_cap));  // [f_cap]
     __shared__ int hist[kHistoLen];
     __shared__ int s_nk, s_nf, s_nruns, s_nevent, s_nmatch;
@@ -113,32 +103,32 @@ __global__ void __launch_bounds__(kBowThreads) bow_search_kernel(const BowArgs A
     const int64_t ko = (int64_t)f * A.kf_cap, fo = (int64_t)f * A.f_cap;
     if (tid == 0) { s_nk = 0; s_nf = 0; s_nruns = 0; s_nevent = 0; s_nmatch = 0; }
     if (tid < kHistoLen) hist[tid] = 0;
-    for (int i = tid; i < A.kf_pow2; i += blockDim.x) {
+    for (int i = tid; i < kf_pow2; i += blockDim.x) {
         uint64_t key = ~0ull;
-        if (i < nk_all && A.kf_weight[ko + i] > 0 && A.kf_valid[ko + i] && !(A.pair_mode == 2 && A.only_stereo && !A.kf_stereo[ko + i])) key = ((uint64_t)(uint32_t)A.kf_node[ko + i] << 32) | (uint32_t)i;      // invalid map points never act
+        if (i < nk_all && A.kf_weight[ko + i] > 0 && A.kf_valid[ko + i] && !(A.keyframe_pair == 2 && A.only_stereo && !A.kf_stereo[ko + i])) key = ((uint64_t)(uint32_t)A.kf_node[ko + i] << 32) | (uint32_t)i;      // invalid map points never act
         kkey[i] = key;
     }
-    for (int j = tid; j < A.f_pow2; j += blockDim.x) {
+    for (int j = tid; j < f_pow2; j += blockDim.x) {
         uint64_t key = ~0ull;
-        if (j < nf_all && A.f_weight[fo + j] > 0 && (!A.f_valid || A.f_valid[fo + j]) && !(A.pair_mode == 2 && A.only_stereo && !A.f_stereo[fo + j])) key = ((uint64_t)(uint32_t)A.f_node[fo + j] << 32) | (uint32_t)j;
+        if (j < nf_all && A.f_weight[fo + j] > 0 && (!A.f_valid || A.f_valid[fo + j]) && !(A.keyframe_pair == 2 && A.only_stereo && !A.f_stereo[fo + j])) key = ((uint64_t)(uint32_t)A.f_node[fo + j] << 32) | (uint32_t)j;
         fkey[j] = key;
     }
-    const int64_t oo = A.pair_mode ? ko : fo;                      // the result is indexed by the first side in pair mode
+    const int64_t oo = A.keyframe_pair ? ko : fo;                  // the result is indexed by the first side in pair mode
     for (int j = tid; j < A.f_cap; j += blockDim.x) taken[j] = 0;
-    for (int j = tid; j < (A.pair_mode ? A.kf_cap : A.f_cap); j += blockDim.x) A.match_f[oo + j] = -1;
+    for (int j = tid; j < (A.keyframe_pair ? A.kf_cap : A.f_cap); j += blockDim.x) A.match_f[oo + j] = -1;
     if (nk_all == 0 || nf_all == 0) { if (tid == 0) A.nmatches[f] = 0; return; }      // an empty side matches nothing: no sort (rows a caller switched off by a zero count)
     __syncthreads();
-    bow_bitonic(kkey, A.kf_pow2);
-    bow_bitonic(fkey, A.f_pow2);
+    bow_bitonic(kkey, kf_pow2);
+    bow_bitonic(fkey, f_pow2);
     // number of live entries and the starts of the key-frame node runs
-    for (int i = tid; i < A.kf_pow2; i += blockDim.x) {
+    for (int i = tid; i < kf_pow2; i += blockDim.x) {
         if (kkey[i] != ~0ull) {
-            if (i + 1 == A.kf_pow2 || kkey[i + 1] == ~0ull) s_nk = i + 1;
+            if (i + 1 == kf_pow2 || kkey[i + 1] == ~0ull) s_nk = i + 1;
             if (i == 0 || (kkey[i - 1] >> 32) != (kkey[i] >> 32)) run_start[atomicAdd(&s_nruns, 1)] = i;      // order of the runs does not matter
         }
     }
-    for (int j = tid; j < A.f_pow2; j += blockDim.x)
-        if (fkey[j] != ~0ull && (j + 1 == A.f_pow2 || fkey[j + 1] == ~0ull)) s_nf = j + 1;
+    for (int j = tid; j < f_pow2; j += blockDim.x)
+        if (fkey[j] != ~0ull && (j + 1 == f_pow2 || fkey[j + 1] == ~0ull)) s_nf = j + 1;
     __syncthreads();
     const int nk = s_nk, nf = s_nf, nruns = s_nruns;
     const uint4* kdesc = reinterpret_cast<const uint4*>(A.kf_desc + 32 * ko);
@@ -161,7 +151,7 @@ __global__ void __launch_bounds__(kBowThreads) bow_search_kernel(const BowArgs A
             unsigned key1 = 0xffffffffu; int d2 = 256;              // local best (distance << 16 | bucket position), local second-best distance
             bool accept;
             unsigned K1;
-            if (A.pair_mode == 2) {
+            if (A.keyframe_pair == 2) {
                 // SearchForTriangulation (:706-740): the best is the smallest distance <= TH_LOW among the candidates that pass the epipole and
                 // epipolar-line gates; a later candidate replaces an earlier one of equal distance (dist > bestDist is the skip test)
                 const float x1 = A.kf_xy[2 * (ko + realK)], y1 = A.kf_xy[2 * (ko + realK) + 1];
@@ -181,12 +171,12 @@ __global__ void __launch_bounds__(kBowThreads) bow_search_kernel(const BowArgs A
                     const int oc = A.f_octave[fo + realF];
                     if (!st1 && !A.f_stereo[fo + realF]) {
                         const float dx = __fsub_rn(ex, x2), dy = __fsub_rn(ey, y2);
-                        if (__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)) < __fmul_rn(100.f, A.scale[oc])) continue;
+                        if (__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)) < __fmul_rn(100.f, A.scale_factors[oc])) continue;
                     }
                     if (den == 0.f) continue;
                     const float num = __fadd_rn(__fadd_rn(__fmul_rn(la, x2), __fmul_rn(lb, y2)), lc);
                     const float dsqr = __fdiv_rn(__fmul_rn(num, num), den);
-                    if (!((double)dsqr < 3.84 * (double)A.sigma2[oc])) continue;
+                    if (!((double)dsqr < 3.84 * (double)A.level_sigma2[oc])) continue;
                     key1 = min(key1, ((unsigned)dist << 16) | (unsigned)(0xffff - (p - b0)));
                 }
                 K1 = __reduce_min_sync(0xffffffffu, key1);
@@ -205,15 +195,15 @@ __global__ void __launch_bounds__(kBowThreads) bow_search_kernel(const BowArgs A
             const int c2 = key1 == K1 ? d2 : min((int)(key1 >> 16), 256);
             const int best2 = __reduce_min_sync(0xffffffffu, c2 > 256 ? 256 : c2);
             const int best1 = K1 == 0xffffffffu ? 256 : (int)(K1 >> 16);
-            accept = (A.pair_mode ? best1 < kThLow : best1 <= kThLow) && (float)best1 < __fmul_rn(A.nnratio, (float)best2);        // :237-240 / :599-601
+            accept = (A.keyframe_pair ? best1 < kThLow : best1 <= kThLow) && (float)best1 < __fmul_rn(A.nnratio, (float)best2);        // :237-240 / :599-601
             }
             if (accept) {
                 const int realF = (int)(uint32_t)fkey[b0 + (int)(K1 & 0xffffu)];
                 if (lane == 0) {
                     taken[realF] = 1;
-                    const int slot = A.pair_mode ? realK : realF;
-                    A.match_f[oo + slot] = A.pair_mode ? realF : realK;
-                    if (A.check_ori) {
+                    const int slot = A.keyframe_pair ? realK : realF;
+                    A.match_f[oo + slot] = A.keyframe_pair ? realF : realK;
+                    if (A.check_orientation) {
                         const int bin = rotation_bin(A.kf_angle[ko + realK], A.f_angle[fo + realF]);
                         atomicAdd(&hist[bin], 1);
                         events[atomicAdd(&s_nevent, 1)] = (bin << 16) | slot;
@@ -226,7 +216,7 @@ __global__ void __launch_bounds__(kBowThreads) bow_search_kernel(const BowArgs A
     }
     if (lane == 0 && nmatch) atomicAdd(&s_nmatch, nmatch);
     __syncthreads();
-    if (A.check_ori) {                                              // :270-288 / :636-654
+    if (A.check_orientation) {                                      // :270-288 / :636-654
         const int removed = drop_outside_main_bins(hist, events, s_nevent, A.match_f + oo);
         if (removed) atomicSub(&s_nmatch, removed);
         __syncthreads();
@@ -467,22 +457,15 @@ SGS_API int sgs_match_bow_batch_device(const sgs_bow_batch* a, int nframes, void
     if (!a || !a->kf_node || !a->kf_weight || !a->kf_valid || !a->kf_desc || !a->kf_angle || !a->kf_n || !a->f_node || !a->f_weight || !a->f_desc || !a->f_angle ||
         !a->f_n || !a->match_f || !a->nmatches || nframes < 1) { set_error("sgs_match_bow_batch_device: bad argument"); return SGS_ERR_INVALID; }
     if (a->kf_cap < 1 || a->f_cap < 1 || a->kf_cap > 8192 || a->f_cap > 8192) { set_error("sgs_match_bow_batch_device: at most 8192 features per frame"); return SGS_ERR_UNSUPPORTED; }
-    BowArgs A;
-    A.kf_node = a->kf_node; A.kf_weight = a->kf_weight; A.kf_valid = a->kf_valid; A.kf_desc = a->kf_desc; A.kf_angle = a->kf_angle; A.kf_n = a->kf_n; A.kf_cap = a->kf_cap;
-    A.f_node = a->f_node; A.f_weight = a->f_weight; A.f_valid = a->f_valid; A.pair_mode = a->keyframe_pair; A.f_desc = a->f_desc;
-    A.kf_stereo = a->kf_stereo; A.f_stereo = a->f_stereo; A.kf_xy = a->kf_xy; A.f_xy = a->f_xy; A.f_octave = a->f_octave; A.F12 = a->F12; A.epipole = a->epipole;
-    A.only_stereo = a->only_stereo;
-    for (int l = 0; l < 16; ++l) { A.sigma2[l] = a->level_sigma2[l]; A.scale[l] = a->scale_factors[l]; }
     if (a->keyframe_pair < 0 || a->keyframe_pair > 2) { set_error("sgs_match_bow_batch_device: keyframe_pair must be 0, 1 or 2"); return SGS_ERR_INVALID; }
     if (a->keyframe_pair == 2 && (!a->kf_stereo || !a->f_stereo || !a->kf_xy || !a->f_xy || !a->f_octave || !a->F12 || !a->epipole || !a->f_valid)) {
         set_error("sgs_match_bow_batch_device: triangulation mode needs positions, octaves, stereo flags, F12 and the epipole"); return SGS_ERR_INVALID;
-    } A.f_angle = a->f_angle; A.f_n = a->f_n; A.f_cap = a->f_cap;
-    A.nnratio = a->nnratio; A.check_ori = a->check_orientation; A.match_f = a->match_f; A.nmatches = a->nmatches;
-    A.kf_pow2 = pow2_ge(a->kf_cap); A.f_pow2 = pow2_ge(a->f_cap);
-    const size_t smem = 8 * (size_t)A.kf_pow2 + 8 * (size_t)A.f_pow2 + 4 * (size_t)(A.kf_pow2 + 1) + 4 * (size_t)(a->kf_cap > a->f_cap ? a->kf_cap : a->f_cap) + (size_t)A.f_cap + 16;
+    }
+    const int kf_pow2 = pow2_ge(a->kf_cap), f_pow2 = pow2_ge(a->f_cap);
+    const size_t smem = 8 * (size_t)kf_pow2 + 8 * (size_t)f_pow2 + 4 * (size_t)(kf_pow2 + 1) + 4 * (size_t)(a->kf_cap > a->f_cap ? a->kf_cap : a->f_cap) + (size_t)a->f_cap + 16;
     if (smem > 40 * 1024)      // per device and cheap: set whenever the default 48 KB would not do
         SGS_CUDA_TRY(cudaFuncSetAttribute(bow_search_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    bow_search_kernel<<<nframes, kBowThreads, smem, (cudaStream_t)stream>>>(A);
+    bow_search_kernel<<<nframes, kBowThreads, smem, (cudaStream_t)stream>>>(*a, kf_pow2, f_pow2);
     SGS_CUDA_TRY(cudaGetLastError());
     return SGS_OK;
 }

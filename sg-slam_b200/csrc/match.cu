@@ -60,12 +60,12 @@ __device__ __forceinline__ void carve(uint8_t* base, int cap, FrameSmem& s) {
 struct GridScale { float w_inv, h_inv; };
 
 // Frame::mfGridElementWidthInv / mfGridElementHeightInv (src/Frame.cc:183-184)
-__device__ __forceinline__ GridScale grid_scale(const MatchCam& cam) {
+__device__ __forceinline__ GridScale grid_scale(const sgs_camera& cam) {
     return {__fdiv_rn((float)kGridCols, __fsub_rn(cam.max_x, cam.min_x)), __fdiv_rn((float)kGridRows, __fsub_rn(cam.max_y, cam.min_y))};
 }
 
 // Frame::PosInGrid (src/Frame.cc:409-419): round() is half away from zero; cell = ix * kGridRows + iy
-__device__ __forceinline__ bool pos_in_grid(const MatchCam& cam, GridScale g, float x, float y, int& cell) {
+__device__ __forceinline__ bool pos_in_grid(const sgs_camera& cam, GridScale g, float x, float y, int& cell) {
     const int px = (int)roundf(__fmul_rn(__fsub_rn(x, cam.min_x), g.w_inv));
     const int py = (int)roundf(__fmul_rn(__fsub_rn(y, cam.min_y), g.h_inv));
     cell = px * kGridRows + py;
@@ -74,7 +74,7 @@ __device__ __forceinline__ bool pos_in_grid(const MatchCam& cam, GridScale g, fl
 
 // The cells Frame::GetFeaturesInArea (src/Frame.cc:354-407) visits for the window of half-size r around (x, y): columns min_cx..max_cx,
 // rows min_cy..max_cy.  False when the window misses the grid.
-__device__ __forceinline__ bool feature_window(const MatchCam& cam, GridScale g, float x, float y, float r, int& min_cx, int& max_cx, int& min_cy,
+__device__ __forceinline__ bool feature_window(const sgs_camera& cam, GridScale g, float x, float y, float r, int& min_cx, int& max_cx, int& min_cy,
                                                int& max_cy) {
     min_cx = max(0, (int)floorf(__fmul_rn(__fsub_rn(__fsub_rn(x, cam.min_x), r), g.w_inv)));
     max_cx = min(kGridCols - 1, (int)ceilf(__fmul_rn(__fadd_rn(__fsub_rn(x, cam.min_x), r), g.w_inv)));
@@ -84,7 +84,7 @@ __device__ __forceinline__ bool feature_window(const MatchCam& cam, GridScale g,
 }
 
 // counting sort by cell; entries of a cell end up in ascending keypoint index (== push_back order of AssignFeaturesToGrid)
-__device__ void build_frame_grid(const MatchCam& cam, const sgs_keypoint* __restrict__ kps, const float* __restrict__ uright, int n, FrameSmem& s) {
+__device__ void build_frame_grid(const sgs_camera& cam, const sgs_keypoint* __restrict__ kps, const float* __restrict__ uright, int n, FrameSmem& s) {
     __shared__ int s_scan[kMatchThreads];
     const GridScale g = grid_scale(cam);
     const int tid = threadIdx.x;
@@ -160,7 +160,7 @@ __device__ __forceinline__ void topk_insert(TopK& t, uint32_t k) {   // insertio
 //   use_claims : skip keypoints whose `claimed` flag is set (phase-3 rescans); phase 2 passes false
 // Returns the kTopK smallest (dist, position) keys seen by this lane and how many candidates passed the gates;
 // *ncand accumulates this lane's share of |vIndices|.
-__device__ TopK scan_window(const MatchCam& cam, const FrameSmem& s, const uint4* __restrict__ cur_desc, float x, float y, float r,
+__device__ TopK scan_window(const sgs_camera& cam, const FrameSmem& s, const uint4* __restrict__ cur_desc, float x, float y, float r,
                             int min_level, int max_level, const uint4& d0, const uint4& d1, bool use_claims, float ur_pred, float ur_tol,
                             int* ncand, int gl = 0, int gsize = 1) {
     TopK t; topk_init(t);
@@ -416,7 +416,7 @@ __global__ void __launch_bounds__(kMatchThreads) match_lastframe_kernel(const __
                         if (fwd) { mn = oct; mx = -1; } else if (bwd) { mn = 0; mx = oct; } else { mn = oct - 1; mx = oct + 1; }
                     }
                     if (ok) {
-                        const float radius = __fmul_rn(A.th, A.cam.scale[oct]);
+                        const float radius = __fmul_rn(A.th, A.cam.scale_factors[oct]);
                         pp.valid = 1; pp.u = u; pp.v = v; pp.invz = invz; pp.radius = radius; pp.min_level = mn; pp.max_level = mx;
                         const uint4* dm = reinterpret_cast<const uint4*>(A.last_desc + 32 * (lo + i));
                         const float ur_pred = __fsub_rn(u, __fmul_rn(A.cam.bf, invz));
@@ -460,7 +460,7 @@ __global__ void __launch_bounds__(kMatchThreads) match_lastframe_kernel(const __
 
 // ---------------------------------------------------------------------------------------------------------------------
 struct LocalPolicy {
-    const LocalMapArgs& A; FrameSmem& s; const uint4* cur_desc; int32_t* f_mp; uint8_t* f_obs; int64_t lo; int point;
+    const sgs_localmap_batch& A; FrameSmem& s; const uint4* cur_desc; int32_t* f_mp; uint8_t* f_obs; int64_t lo; int point;
     __device__ bool uses_second() const { return true; }
     __device__ bool reject_is_final() const { return false; }    // a ratio-test rejection can flip once a top-2 keypoint is claimed
     __device__ bool blocks_others() const { return A.mp_obs[lo + point] != 0; }
@@ -478,7 +478,7 @@ struct LocalPolicy {
         lvl = A.level[lo + point];
         float r = ((double)A.view_cos[lo + point] > 0.998) ? 2.5f : 4.0f;   // RadiusByViewingCos :131-137 (compared in double)
         if (A.th != 1.0f) r = __fmul_rn(r, A.th);                           // bFactor :50,:67-68
-        rr = __fmul_rn(r, A.cam.scale[lvl]);
+        rr = __fmul_rn(r, A.cam.scale_factors[lvl]);
     }
     __device__ TopK rescan() const {
         float rr; int lvl;
@@ -496,23 +496,26 @@ struct LocalPolicy {
     }
 };
 
-__global__ void __launch_bounds__(kMatchThreads) match_localmap_kernel(const __grid_constant__ LocalMapArgs A) {
+// cur_cap / mp_cap: the matcher's capacities, lpre: its per-point scratch [nframes][mp_cap].  The values that come beside the ABI struct are
+// __grid_constant__ like it: the kernel reads them from the parameter bank where it uses them instead of holding them in registers throughout.
+__global__ void __launch_bounds__(kMatchThreads) match_localmap_kernel(const __grid_constant__ sgs_localmap_batch A, const __grid_constant__ int cur_cap,
+                                                                       LocalPre* const __grid_constant__ lpre, const __grid_constant__ int mp_cap) {
     extern __shared__ __align__(16) uint8_t smem[];
     __shared__ int s_nmatch;
     const int f = blockIdx.x;
-    const int n = min(A.cur_n[f], A.cur_cap);
-    const int nmp = min(A.mp_n[f], A.mp_cap);
+    const int n = min(A.cur_n[f], cur_cap);
+    const int nmp = min(A.mp_n[f], mp_cap);
     FrameSmem s;
-    carve(smem, A.cur_cap, s);
-    const sgs_keypoint* kps = A.cur_kps + (int64_t)f * A.cur_cap;
-    const uint4* cur_desc = reinterpret_cast<const uint4*>(A.cur_desc + (int64_t)f * A.cur_cap * 32);
-    int32_t* f_mp = A.f_mp + (int64_t)f * A.cur_cap;
-    uint8_t* f_obs = A.f_mp_obs + (int64_t)f * A.cur_cap;
-    const int64_t lo = (int64_t)f * A.mp_cap;
-    build_frame_grid(A.cam, kps, A.cur_uright + (int64_t)f * A.cur_cap, n, s);
+    carve(smem, cur_cap, s);
+    const sgs_keypoint* kps = A.cur_kps + (int64_t)f * cur_cap;
+    const uint4* cur_desc = reinterpret_cast<const uint4*>(A.cur_desc + (int64_t)f * cur_cap * 32);
+    int32_t* f_mp = A.f_mp + (int64_t)f * cur_cap;
+    uint8_t* f_obs = A.f_mp_obs + (int64_t)f * cur_cap;
+    const int64_t lo = (int64_t)f * mp_cap;
+    build_frame_grid(A.cam, kps, A.cur_uright + (int64_t)f * cur_cap, n, s);
     for (int i = threadIdx.x; i < n; i += blockDim.x) { s.claimed[i] = (f_mp[i] >= 0 && f_obs[i]) ? 1 : 0; s.tent[i] = 0; }
     __syncthreads();
-    LocalPre* pre = A.pre + lo;
+    LocalPre* pre = lpre + lo;
     int ncand = 0;
     const int gl = threadIdx.x & (kGroup - 1);
     const int ngroups = blockDim.x / kGroup;
@@ -550,7 +553,7 @@ __global__ void __launch_bounds__(kMatchThreads) match_localmap_kernel(const __g
         if (threadIdx.x == 0) s_nmatch = nmatch;
     }
     __syncthreads();
-    write_totals(ncand, s_nmatch, &A.ncand[f], &A.nmatches[f]);
+    write_totals(ncand, s_nmatch, reinterpret_cast<unsigned long long*>(A.ncand) + f, &A.nmatches[f]);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -558,7 +561,7 @@ __global__ void __launch_bounds__(kMatchThreads) match_localmap_kernel(const __g
 // independent (the reference's side effects -- Replace / AddObservation -- do not feed back into the search), so the block only shares
 // the key frame's grid: kGroup lanes per map point scan its window, the best (distance, grid position) key is min-reduced over the
 // group, which is the first minimum of the reference's loop over vIndices.
-__global__ void __launch_bounds__(kMatchThreads) fuse_search_kernel(const __grid_constant__ FuseArgs A) {
+__global__ void __launch_bounds__(kMatchThreads) fuse_search_kernel(const __grid_constant__ sgs_fuse_batch A, const __grid_constant__ float log_sf) {
     extern __shared__ __align__(16) uint8_t smem[];
     FrameSmem s;
     carve(smem, A.kf_cap, s);
@@ -610,8 +613,8 @@ __global__ void __launch_bounds__(kMatchThreads) fuse_search_kernel(const __grid
             const float* N = A.mp_normal + 3 * (lo + i);
             ok = ok && (cam2 || !((((double)px * N[0] + (double)py * N[1]) + (double)pz * N[2]) < 0.5 * (double)dist));
             if (ok) {
-                const int lvl = predict_scale(maxd, dist, A.log_sf, A.cam.nlevels);
-                const float r = __fmul_rn(A.th, A.cam.scale[lvl]);
+                const int lvl = predict_scale(maxd, dist, log_sf, A.cam.nlevels);
+                const float r = __fmul_rn(A.th, A.cam.scale_factors[lvl]);
                 int min_cx, max_cx, min_cy, max_cy;
                 if (feature_window(A.cam, g, u, v, r, min_cx, max_cx, min_cy, max_cy)) {
                     const uint4* dm = reinterpret_cast<const uint4*>(A.mp_desc + 32 * (lo + i));
@@ -630,10 +633,10 @@ __global__ void __launch_bounds__(kMatchThreads) fuse_search_kernel(const __grid
                             } else if (kr >= 0.f) {
                                 const float er = __fsub_rn(ur, kr);
                                 const float e2 = __fadd_rn(__fadd_rn(__fmul_rn(ex, ex), __fmul_rn(ey, ey)), __fmul_rn(er, er));
-                                if ((double)__fmul_rn(e2, A.inv_sigma2[o]) > 7.8) continue;
+                                if ((double)__fmul_rn(e2, A.inv_level_sigma2[o]) > 7.8) continue;
                             } else {
                                 const float e2 = __fadd_rn(__fmul_rn(ex, ex), __fmul_rn(ey, ey));
-                                if ((double)__fmul_rn(e2, A.inv_sigma2[o]) > 5.99) continue;
+                                if ((double)__fmul_rn(e2, A.inv_level_sigma2[o]) > 5.99) continue;
                             }
                             const uint32_t k = ((uint32_t)descriptor_distance(d0, d1, __ldg(&kf_desc[2 * idx]), __ldg(&kf_desc[2 * idx + 1])) << 16) | (uint32_t)j;
                             best = min(best, k);
@@ -691,7 +694,7 @@ __device__ __forceinline__ BestTwo merge_two(BestTwo a, BestTwo b) {
     return r;
 }
 
-__global__ void __launch_bounds__(kMatchThreads) search_init_kernel(const __grid_constant__ InitArgs A) {
+__global__ void __launch_bounds__(kMatchThreads) search_init_kernel(const __grid_constant__ sgs_init_batch A) {
     extern __shared__ __align__(16) uint8_t smem[];
     FrameSmem s;
     carve(smem, A.f2_cap, s);
@@ -716,7 +719,7 @@ __global__ void __launch_bounds__(kMatchThreads) search_init_kernel(const __grid
     if (tid == 0) s_nm = 0;
     __syncthreads();
     const GridScale g = grid_scale(A.cam);
-    const float r = (float)A.window;
+    const float r = (float)A.window_size;
     for (int i1 = 0; i1 < n1; ++i1) {
         if (k1[i1].octave > 0) continue;                                                    // level1 > 0 (:424-426), block-uniform
         const float x = prev[2 * i1], y = prev[2 * i1 + 1];
@@ -755,7 +758,7 @@ __global__ void __launch_bounds__(kMatchThreads) search_init_kernel(const __grid
                 if (best_d <= kThLow && (float)best_d < __fmul_rn(second_f, A.nnratio)) {
                     if (m21[idx2] >= 0) { m12[m21[idx2]] = -1; s_nm = s_nm - 1; }
                     m12[i1] = idx2; m21[idx2] = i1; mdist[idx2] = best_d; s_nm = s_nm + 1;
-                    if (A.check_ori) {
+                    if (A.check_orientation) {
                         const int bin = rotation_bin(k1[i1].angle, k2[idx2].angle);
                         hist[bin] = hist[bin] + 1; bin_of[i1] = (int8_t)bin;
                     }
@@ -764,7 +767,7 @@ __global__ void __launch_bounds__(kMatchThreads) search_init_kernel(const __grid
         }
         __syncthreads();
     }
-    if (A.check_ori) {
+    if (A.check_orientation) {
         __shared__ int keep[3];
         if (tid == 0) three_maxima(hist, keep[0], keep[1], keep[2]);
         __syncthreads();
@@ -783,27 +786,27 @@ __global__ void __launch_bounds__(kMatchThreads) search_init_kernel(const __grid
 
 // One block of kMatchThreads per frame.  The frame grid keeps keypoint indices in 16 bits, so no capacity may exceed 65535, and `smem` bytes
 // of dynamic shared memory hold it (plus the kernel's own per-keypoint arrays).
-template <class Args>
-static int launch_per_frame(void (*kernel)(Args), const Args& A, size_t smem, int cap, int nframes, cudaStream_t st) {
+template <class... Params, class... Args>
+static int launch_per_frame(void (*kernel)(Params...), size_t smem, int cap, int nframes, cudaStream_t st, const Args&... args) {
     if (smem > 200 * 1024 || cap > 65535) { set_error("matcher: capacity %d too large for shared memory", cap); return SGS_ERR_UNSUPPORTED; }
     SGS_CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    kernel<<<nframes, kMatchThreads, smem, st>>>(A);
+    kernel<<<nframes, kMatchThreads, smem, st>>>(args...);
     SGS_CUDA_TRY(cudaGetLastError());
     return SGS_OK;
 }
 
 int launch_matcher(const LastFrameArgs& A, int nframes, cudaStream_t st) {
-    return launch_per_frame(match_lastframe_kernel, A, frame_smem_bytes(A.cur_cap), A.cur_cap, nframes, st);
+    return launch_per_frame(match_lastframe_kernel, frame_smem_bytes(A.cur_cap), A.cur_cap, nframes, st, A);
 }
-int launch_matcher(const LocalMapArgs& A, int nframes, cudaStream_t st) {
-    return launch_per_frame(match_localmap_kernel, A, frame_smem_bytes(A.cur_cap), A.cur_cap, nframes, st);
+int launch_matcher(const sgs_localmap_batch& A, int cur_cap, LocalPre* pre, int mp_cap, int nframes, cudaStream_t st) {
+    return launch_per_frame(match_localmap_kernel, frame_smem_bytes(cur_cap), cur_cap, nframes, st, A, cur_cap, pre, mp_cap);
 }
-int launch_matcher(const FuseArgs& A, int nframes, cudaStream_t st) {
-    return launch_per_frame(fuse_search_kernel, A, frame_smem_bytes(A.kf_cap), A.kf_cap, nframes, st);
+int launch_matcher(const sgs_fuse_batch& A, float log_sf, int nframes, cudaStream_t st) {
+    return launch_per_frame(fuse_search_kernel, frame_smem_bytes(A.kf_cap), A.kf_cap, nframes, st, A, log_sf);
 }
-int launch_matcher(const InitArgs& A, int nframes, cudaStream_t st) {     // + vMatchedDistance, vnMatches21 and the rotation bins of F1
+int launch_matcher(const sgs_init_batch& A, int nframes, cudaStream_t st) {     // + vMatchedDistance, vnMatches21 and the rotation bins of F1
     const size_t smem = frame_smem_bytes(A.f2_cap) + (size_t)A.f2_cap * 8 + (size_t)((A.f1_cap + 15) & ~15);
-    return launch_per_frame(search_init_kernel, A, smem, max(A.f1_cap, A.f2_cap), nframes, st);
+    return launch_per_frame(search_init_kernel, smem, max(A.f1_cap, A.f2_cap), nframes, st, A);
 }
 
 }  // namespace sgs

@@ -24,14 +24,6 @@ namespace {
 
 using MatcherPtr = std::unique_ptr<sgs_matcher, void (*)(sgs_matcher*)>;     // the scratch handle of a single-frame call
 
-MatchCam to_cam(const sgs_camera& c) {
-    MatchCam m;
-    m.min_x = c.min_x; m.min_y = c.min_y; m.max_x = c.max_x; m.max_y = c.max_y;
-    m.fx = c.fx; m.fy = c.fy; m.cx = c.cx; m.cy = c.cy; m.bf = c.bf; m.nlevels = c.nlevels;
-    for (int i = 0; i < kMaxLevels; ++i) m.scale[i] = c.scale_factors[i];
-    return m;
-}
-
 sgs_camera view_cam(const sgs_frame_view* v) {
     sgs_camera c;
     std::memset(&c, 0, sizeof c);
@@ -45,7 +37,7 @@ sgs_camera view_cam(const sgs_frame_view* v) {
 template <class Batch>
 LastFrameArgs projection_args(const sgs_matcher* m, const Batch* a) {
     LastFrameArgs A{};
-    A.cam = to_cam(a->cam);
+    A.cam = a->cam;
     A.cur_kps = a->cur_kps; A.cur_desc = a->cur_desc; A.cur_uright = a->cur_uright; A.cur_n = a->cur_n; A.cur_cap = m->cur_cap;
     A.last_cap = m->point_cap; A.tcw_cur = a->tcw_cur; A.th = a->th; A.check_ori = a->check_orientation;
     A.cur_mp = a->cur_mp; A.nmatches = a->nmatches; A.ncand = (unsigned long long*)a->ncand;
@@ -96,18 +88,9 @@ SGS_API int sgs_fuse_search_batch_device(const sgs_fuse_batch* a, int nframes, v
         set_error("sgs_fuse_search_batch_device: bad argument"); return SGS_ERR_INVALID;
     }
     if (a->cam.nlevels < 2 || a->cam.nlevels > kMaxLevels || !(a->cam.scale_factors[1] > 1.f)) { set_error("sgs_fuse_search_batch_device: camera scale table missing"); return SGS_ERR_INVALID; }
-    FuseArgs A;
-    A.cam = to_cam(a->cam);
-    A.kf_kps = a->kf_kps; A.kf_desc = a->kf_desc; A.kf_uright = a->kf_uright; A.kf_n = a->kf_n; A.kf_cap = a->kf_cap;
-    A.tcw = a->tcw; A.ow = a->ow; A.mp_xyz = a->mp_xyz; A.mp_normal = a->mp_normal; A.mp_min_dist = a->mp_min_dist; A.mp_max_dist = a->mp_max_dist;
-    A.mp_desc = a->mp_desc; A.mp_valid = a->mp_valid; A.mp_n = a->mp_n; A.mp_cap = a->mp_cap; A.th = a->th; A.log_sf = logf(a->cam.scale_factors[1]);
-    for (int l = 0; l < kMaxLevels; ++l) A.inv_sigma2[l] = a->inv_level_sigma2[l];
-    A.sim3_variant = a->sim3_variant; A.xform2 = a->xform2;
     if (a->sim3_variant < 0 || a->sim3_variant > 3 || (a->sim3_variant == 2 && !a->xform2) || (a->sim3_variant == 3 && !a->kf_matched)) {
         set_error("sgs_fuse_search_batch_device: bad variant"); return SGS_ERR_INVALID; }
-    A.best_idx = a->best_idx; A.best_dist = a->best_dist;
-    A.kf_matched = a->kf_matched; A.nmatches = a->nmatches;
-    return launch_matcher(A, nframes, (cudaStream_t)stream);
+    return launch_matcher(*a, logf(a->cam.scale_factors[1]), nframes, (cudaStream_t)stream);
 }
 
 SGS_API int sgs_match_project_keyframe_batch_device(sgs_matcher* m, const sgs_keyframe_batch* a, int nframes, void* stream) {
@@ -125,16 +108,7 @@ SGS_API int sgs_match_project_keyframe_batch_device(sgs_matcher* m, const sgs_ke
 SGS_API int sgs_match_project_localmap_batch_device(sgs_matcher* m, const sgs_localmap_batch* a, int nframes, void* stream) {
     if (!m || !a) { set_error("sgs_match_project_localmap_batch_device: NULL"); return SGS_ERR_INVALID; }
     if (nframes < 1 || nframes > m->max_frames) { set_error("nframes outside [1,max_frames]"); return SGS_ERR_INVALID; }
-    LocalMapArgs A;
-    A.cam = to_cam(a->cam);
-    A.cur_kps = a->cur_kps; A.cur_desc = a->cur_desc; A.cur_uright = a->cur_uright; A.cur_n = a->cur_n;
-    A.cur_cap = m->cur_cap;
-    A.mp_inview = a->mp_inview; A.proj_x = a->proj_x; A.proj_y = a->proj_y; A.proj_xr = a->proj_xr; A.level = a->level;
-    A.view_cos = a->view_cos; A.mp_desc = a->mp_desc; A.mp_obs = a->mp_obs; A.mp_n = a->mp_n; A.mp_cap = m->point_cap;
-    A.th = a->th; A.nnratio = a->nnratio; A.id_base = a->id_base;
-    A.f_mp = a->f_mp; A.f_mp_obs = a->f_mp_obs; A.nmatches = a->nmatches; A.ncand = (unsigned long long*)a->ncand;
-    A.pre = m->d_lpre;
-    return launch_matcher(A, nframes, (cudaStream_t)stream);
+    return launch_matcher(*a, m->cur_cap, m->d_lpre, m->point_cap, nframes, (cudaStream_t)stream);
 }
 
 SGS_API int sgs_match_project_lastframe(const sgs_frame_view* cur, const float* tcw_cur, const float* tcw_last, int nlast,
@@ -251,12 +225,7 @@ SGS_API int sgs_fuse_search(const sgs_frame_view* kf, const float* tcw, const fl
 SGS_API int sgs_search_for_initialization_batch_device(const sgs_init_batch* a, int nframes, void* stream) {
     if (!a || !a->f1_kps || !a->f1_desc || !a->f1_n || !a->f2_kps || !a->f2_desc || !a->f2_n || !a->prev_xy || !a->match12 || nframes < 1 || a->f1_cap < 1 || a->f2_cap < 1 ||
         a->window_size < 0 || !(a->cam.max_x > a->cam.min_x) || !(a->cam.max_y > a->cam.min_y)) { set_error("sgs_search_for_initialization_batch_device: bad argument"); return SGS_ERR_INVALID; }
-    InitArgs A;
-    A.cam = to_cam(a->cam);
-    A.f1_kps = a->f1_kps; A.f1_desc = a->f1_desc; A.f1_n = a->f1_n; A.f1_cap = a->f1_cap;
-    A.f2_kps = a->f2_kps; A.f2_desc = a->f2_desc; A.f2_n = a->f2_n; A.f2_cap = a->f2_cap;
-    A.prev_xy = a->prev_xy; A.window = a->window_size; A.nnratio = a->nnratio; A.check_ori = a->check_orientation; A.match12 = a->match12; A.nmatches = a->nmatches;
-    return launch_matcher(A, nframes, (cudaStream_t)stream);
+    return launch_matcher(*a, nframes, (cudaStream_t)stream);
 }
 
 SGS_API int sgs_search_for_initialization(const sgs_frame_view* f1, const sgs_frame_view* f2, float* prev_xy, int window_size, float nnratio, int check_orientation,

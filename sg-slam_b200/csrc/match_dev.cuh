@@ -1,5 +1,6 @@
-// match_dev.cuh -- argument blocks of the batched projection matchers (match.cu).  All pointers are DEVICE pointers;
-// per-frame arrays are laid out [nframes][cap] with the given capacities.
+// match_dev.cuh -- launchers of the batched matchers (match.cu), the last-frame matcher's argument block and the per-point scratch of the
+// projection matchers.  The other matchers read their sgs_abi.h batch struct as it is.  All pointers are DEVICE pointers; per-frame arrays
+// are laid out [nframes][cap] with the given capacities.
 #pragma once
 #include <cuda_runtime.h>
 
@@ -7,13 +8,6 @@
 #include "sgs_common.h"
 
 namespace sgs {
-
-struct MatchCam {                 // Frame statics (src/Frame.cc:176-196) + the extractor's scale factors
-    float min_x, min_y, max_x, max_y;
-    float fx, fy, cx, cy, bf;
-    int32_t nlevels;
-    float scale[kMaxLevels];
-};
 
 constexpr int kTopK = 4;          // candidates kept per map point by the optimistic scan
 
@@ -28,7 +22,7 @@ struct PointPre {                 // phase-2 result of one last-frame point
 struct LocalPre { uint32_t k[kTopK]; int32_t ngated; };
 
 struct LastFrameArgs {
-    MatchCam cam;
+    sgs_camera cam;
     // current frames
     const sgs_keypoint* cur_kps; const uint8_t* cur_desc; const float* cur_uright; const int32_t* cur_n;
     int32_t cur_cap;
@@ -47,45 +41,11 @@ struct LastFrameArgs {
     PointPre* pre; int32_t* events;
 };
 
-struct LocalMapArgs {
-    MatchCam cam;
-    const sgs_keypoint* cur_kps; const uint8_t* cur_desc; const float* cur_uright; const int32_t* cur_n;
-    int32_t cur_cap;
-    const uint8_t* mp_inview; const float* proj_x; const float* proj_y; const float* proj_xr; const int32_t* level;
-    const float* view_cos; const uint8_t* mp_desc; const uint8_t* mp_obs; const int32_t* mp_n; int32_t mp_cap;
-    float th, nnratio; int32_t id_base;
-    int32_t* f_mp; uint8_t* f_mp_obs; int32_t* nmatches; unsigned long long* ncand;
-    LocalPre* pre;
-};
-
-struct FuseArgs {                 // search half of ORBmatcher::Fuse(KeyFrame*, vpMapPoints, th), src/ORBmatcher.cc:829-980
-    MatchCam cam;
-    const sgs_keypoint* kf_kps; const uint8_t* kf_desc; const float* kf_uright; const int32_t* kf_n; int32_t kf_cap;
-    const float* tcw; const float* ow;            // [nframes][16], [nframes][3]
-    const float* mp_xyz; const float* mp_normal; const float* mp_min_dist; const float* mp_max_dist; const uint8_t* mp_desc; const uint8_t* mp_valid;
-    const int32_t* mp_n; int32_t mp_cap;
-    float th, log_sf; float inv_sigma2[kMaxLevels];
-    const float* xform2;          // [nframes][12]: sR21 (3x3 row major) + t21, variant 2 only
-    int32_t sim3_variant;         // 2: one direction of SearchBySim3 (:1106-1330): second transform xform2, distance |p3Dc2|, no viewing-angle test;
-                                  // 1: Fuse(KeyFrame*, Scw, ...) (:982-1104): pose already decomposed by the caller, invz = 1.0 / z in double, no chi-square gates
-                                  // 3: SearchByProjection(KeyFrame*, Scw, ...) (:292-405): as 1 with invz = 1 / z in float; occupied features are skipped and claimed in point order
-    int32_t* best_idx; int32_t* best_dist;
-    int32_t* kf_matched; int32_t* nmatches;   // variant 3 (SearchByProjection(KeyFrame*, Scw, vpPoints, vpMatched, th), :292-405): vpMatched in/out [nframes][kf_cap], matches per frame
-};
-
-struct InitArgs {                 // ORBmatcher::SearchForInitialization(F1, F2, vbPrevMatched, vnMatches12, windowSize), src/ORBmatcher.cc:407-522
-    MatchCam cam;                 // image bounds of F2 (its feature grid)
-    const sgs_keypoint* f1_kps; const uint8_t* f1_desc; const int32_t* f1_n; int32_t f1_cap;
-    const sgs_keypoint* f2_kps; const uint8_t* f2_desc; const int32_t* f2_n; int32_t f2_cap;
-    float* prev_xy;               // in/out [nframes][f1_cap][2]
-    int32_t window; float nnratio; int32_t check_ori;
-    int32_t* match12; int32_t* nmatches;
-};
-
-// one block per frame of the matcher that takes these arguments; SGS_ERR_UNSUPPORTED when its frame grid does not fit in shared memory
+// one block per frame of the matcher that takes these arguments; SGS_ERR_UNSUPPORTED when its frame grid does not fit in shared memory.
+// The local-map matcher takes the capacities and the scratch of its sgs_matcher; the fuse search takes log_sf = logf(cam.scale_factors[1]).
 int launch_matcher(const LastFrameArgs& A, int nframes, cudaStream_t st);
-int launch_matcher(const LocalMapArgs& A, int nframes, cudaStream_t st);
-int launch_matcher(const FuseArgs& A, int nframes, cudaStream_t st);
-int launch_matcher(const InitArgs& A, int nframes, cudaStream_t st);
+int launch_matcher(const sgs_localmap_batch& A, int cur_cap, LocalPre* pre, int mp_cap, int nframes, cudaStream_t st);
+int launch_matcher(const sgs_fuse_batch& A, float log_sf, int nframes, cudaStream_t st);
+int launch_matcher(const sgs_init_batch& A, int nframes, cudaStream_t st);
 
 }  // namespace sgs

@@ -106,17 +106,6 @@ __device__ bool po_ldlt6(const double* Hin, const double* b, double* x) {
     return true;
 }
 
-struct PoArgs {
-    float fx, fy, cx, cy, bf;
-    const float* tcw_in; const sgs_keypoint* kps; const float* uright; const int32_t* n; int cap;
-    const uint8_t* has_mp; const int32_t* mp_index; const float* points_xyz; int point_cap;
-    const float* points2_xyz; int id_base2, point2_cap;      // optional second point array (local-map points of the chained call)
-    float inv_sigma2[16];
-    float* tcw_out; uint8_t* outlier; int32_t* ninliers;
-    double* err;          // scratch [F][cap][3]: the error vector each edge carries between evaluations
-    uint8_t* level;       // scratch [F][cap]: 1 = excluded from the next round (the edge's g2o level)
-};
-
 // sum of `v` over the block, result in every thread (fixed tree order: deterministic)
 __device__ double po_block_sum(double v, double* s_red) {
 #pragma unroll
@@ -130,7 +119,9 @@ __device__ double po_block_sum(double v, double* s_red) {
     return t;
 }
 
-__global__ void __launch_bounds__(kPoThreads) pose_opt_kernel(const PoArgs A) {
+// A.scratch_err [F][cap][3]: the error vector each edge carries between evaluations; A.scratch_level [F][cap]: 1 = excluded from the next round
+// (the edge's g2o level).  Without mp_index, point_cap == cap and points2_xyz == NULL (sgs_pose_optimization_batch_device sees to both).
+__global__ void __launch_bounds__(kPoThreads) pose_opt_kernel(const __grid_constant__ sgs_poseopt_batch A) {
     __shared__ PoSE3 s_est;
     __shared__ double s_red[kPoThreads / 32];
     __shared__ double s_sys[28];          // 21 upper-triangular entries of H, 6 of b, robust chi2
@@ -139,7 +130,7 @@ __global__ void __launch_bounds__(kPoThreads) pose_opt_kernel(const PoArgs A) {
     const int f = blockIdx.x, tid = threadIdx.x;
     const int n = min(A.n[f], A.cap);
     const int64_t ko = (int64_t)f * A.cap;
-    const double fx = A.fx, fy = A.fy, cx = A.cx, cy = A.cy, bf = A.bf;
+    const double fx = A.cam.fx, fy = A.cam.fy, cx = A.cam.cx, cy = A.cam.cy, bf = A.cam.bf;
     const float deltaMono = (float)sqrt(5.991), deltaStereo = (float)sqrt(7.815);
 
     auto has = [&](int i) -> bool { return A.mp_index ? A.mp_index[ko + i] >= 0 : A.has_mp[ko + i] != 0; };
@@ -170,7 +161,7 @@ __global__ void __launch_bounds__(kPoThreads) pose_opt_kernel(const PoArgs A) {
     for (int i = tid; i < n; i += kPoThreads) {
         const bool h = has(i);
         n_initial += h ? 1 : 0;
-        A.level[ko + i] = 0;
+        A.scratch_level[ko + i] = 0;
         if (h) A.outlier[ko + i] = 0;
     }
     n_initial = (int)po_block_sum((double)n_initial, s_red);
@@ -187,19 +178,19 @@ __global__ void __launch_bounds__(kPoThreads) pose_opt_kernel(const PoArgs A) {
             s_est.r = po_quat_from_matrix(R); po_normalize(s_est.r);
         }
         __syncthreads();
-        // evaluation at s_est: errors of the active edges (kept in A.err), robust chi2, optionally the normal equations
+        // evaluation at s_est: errors of the active edges (kept in A.scratch_err), robust chi2, optionally the normal equations
         auto evaluate = [&](bool with_system) {
             double acc[28];
 #pragma unroll
             for (int q = 0; q < 28; ++q) acc[q] = 0;
             const PoSE3 est = s_est;
             for (int i = tid; i < n; i += kPoThreads) {
-                if (!has(i) || A.level[ko + i]) continue;
+                if (!has(i) || A.scratch_level[ko + i]) continue;
                 double e[3], pc[3];
                 const bool stereo = edge_error(i, est, e, pc);
-                double* E = A.err + 3 * (ko + i);
+                double* E = A.scratch_err + 3 * (ko + i);
                 E[0] = e[0]; E[1] = e[1]; E[2] = e[2];
-                const double info = A.inv_sigma2[A.kps[ko + i].octave];
+                const double info = A.inv_level_sigma2[A.kps[ko + i].octave];
                 const double c = (e[0] * e[0] + e[1] * e[1] + (stereo ? e[2] * e[2] : 0.0)) * info;
                 const double delta = stereo ? deltaStereo : deltaMono, dsqr = delta * delta;
                 double w = 1.0;
@@ -231,7 +222,7 @@ __global__ void __launch_bounds__(kPoThreads) pose_opt_kernel(const PoArgs A) {
         };
         // number of active edges (initializeOptimization(0)): nothing to optimise when there is none
         int n_active = 0;
-        for (int i = tid; i < n; i += kPoThreads) n_active += (has(i) && !A.level[ko + i]) ? 1 : 0;
+        for (int i = tid; i < n; i += kPoThreads) n_active += (has(i) && !A.scratch_level[ko + i]) ? 1 : 0;
         n_active = (int)po_block_sum((double)n_active, s_red);
         if (n_active > 0) {
             double lambda = 0, ni = 2; int nbad_lm = 0;
@@ -292,15 +283,15 @@ __global__ void __launch_bounds__(kPoThreads) pose_opt_kernel(const PoArgs A) {
         const PoSE3 est = s_est;
         for (int i = tid; i < n; i += kPoThreads) {
             if (!has(i)) continue;
-            double* E = A.err + 3 * (ko + i);
+            double* E = A.scratch_err + 3 * (ko + i);
             double e[3] = {E[0], E[1], E[2]}, pc[3];
             const float ur = A.uright[ko + i];
             const bool stereo = !(ur < 0);
             if (A.outlier[ko + i]) { edge_error(i, est, e, pc); E[0] = e[0]; E[1] = e[1]; E[2] = e[2]; }
-            const double info = A.inv_sigma2[A.kps[ko + i].octave];
+            const double info = A.inv_level_sigma2[A.kps[ko + i].octave];
             const float chi2 = (float)((e[0] * e[0] + e[1] * e[1] + (stereo ? e[2] * e[2] : 0.0)) * info);
-            if (chi2 > (stereo ? 7.815f : 5.991f)) { A.outlier[ko + i] = 1; A.level[ko + i] = 1; ++bad; }
-            else { A.outlier[ko + i] = 0; A.level[ko + i] = 0; }
+            if (chi2 > (stereo ? 7.815f : 5.991f)) { A.outlier[ko + i] = 1; A.scratch_level[ko + i] = 1; ++bad; }
+            else { A.outlier[ko + i] = 0; A.scratch_level[ko + i] = 0; }
         }
         n_bad = (int)po_block_sum((double)bad, s_red);
         __syncthreads();
@@ -327,13 +318,8 @@ extern "C" {
 SGS_API int sgs_pose_optimization_batch_device(const sgs_poseopt_batch* a, int nframes, void* stream) {
     if (!a || !a->tcw_in || !a->kps || !a->uright || !a->n || !a->points_xyz || !a->tcw_out || !a->outlier || !a->ninliers || !a->scratch_err || !a->scratch_level ||
         (!a->has_mp && !a->mp_index) || a->cap < 1 || nframes < 1) { set_error("sgs_pose_optimization_batch_device: bad argument"); return SGS_ERR_INVALID; }
-    PoArgs A;
-    A.fx = a->cam.fx; A.fy = a->cam.fy; A.cx = a->cam.cx; A.cy = a->cam.cy; A.bf = a->cam.bf;
-    A.tcw_in = a->tcw_in; A.kps = a->kps; A.uright = a->uright; A.n = a->n; A.cap = a->cap;
-    A.has_mp = a->has_mp; A.mp_index = a->mp_index; A.points_xyz = a->points_xyz; A.point_cap = a->mp_index ? a->point_cap : a->cap;
-    A.points2_xyz = a->mp_index ? a->points2_xyz : nullptr; A.id_base2 = a->id_base2; A.point2_cap = a->point2_cap;
-    for (int l = 0; l < 16; ++l) A.inv_sigma2[l] = a->inv_level_sigma2[l];
-    A.tcw_out = a->tcw_out; A.outlier = a->outlier; A.ninliers = a->ninliers; A.err = a->scratch_err; A.level = a->scratch_level;
+    sgs_poseopt_batch A = *a;
+    if (!A.mp_index) { A.point_cap = A.cap; A.points2_xyz = nullptr; }      // keypoint i reads points_xyz[i]; there is no second point array
     pose_opt_kernel<<<nframes, kPoThreads, 0, (cudaStream_t)stream>>>(A);
     SGS_CUDA_TRY(cudaGetLastError());
     return SGS_OK;
